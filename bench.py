@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py -- rendered rays/second of the SelfOcc hot path on B200 (see DESIGN.md "Measurement").
+"""bench.py -- rendered rays/second of the SelfOcc hot path on an H100 (see DESIGN.md "Measurement").
 
 A step = ONE pass of the hot path over one synthetic 6-camera frame:
     TPVQueryLifter -> TPVFormerEncoder (4 layers of self + image cross attention) -> NeuSHead.prepare
@@ -10,7 +10,8 @@ color_dims=3 (decode writes 4 channels, colour is composited), render_bkgd='rand
 head of config/nuscenes/nuscenes_depth.py on the same ray grid (a second workload, stated in config.color_dims).  The image backbone (third-party cuDNN ResNet/FPN) is
 outside the hot path: the step starts from synthetic FPN features.
 
-  python bench.py --gpus N --steps K --warmup W            # this repo's sm_100a path
+  python bench.py --gpus N --steps K --warmup W            # this repo's sm_90a path
+  python bench.py ... --dump-outputs DIR                    # + the last timed step's outputs as DIR/<name>.npy
   python bench.py --impl reference --gpus N ...            # the CPU oracle port (the reference is not installable)
 
 N > 1 (torchrun): data-parallel frames exactly like the reference's DDP evaluation -- rank r lifts and renders
@@ -56,6 +57,8 @@ def parse():
     ap.add_argument('--no-strong', action='store_true', help='skip the strong-scaling (one frame sharded over the ranks) measurement')
     ap.add_argument('--scaling', default='weak', choices=['weak', 'strong'], help='which measurement is the headline `value`')
     ap.add_argument('--no-reference-gpu', action='store_true', help='skip the reference-style eager-PyTorch-on-GPU side figure')
+    ap.add_argument('--dump-outputs', metavar='DIR', help='write what the last timed step computed as DIR/<name>.npy (float32; a fixed, '
+                    'seeded sample of 2^20 rays when the frame has more)')
     return ap.parse_args()
 
 
@@ -137,7 +140,37 @@ class ClockSampler:
         return {'sm_mhz': sm[len(sm) // 2], 'sm_max_mhz': mx, 'reasons': sorted(reasons), 'samples': len(sm)}
 
 
-# ------------------------------------------------------------------------------------------ B200 arm
+# ------------------------------------------------------------------------------------------ output dump
+def dump_outputs(out, outdir, n_cam, n_ray, budget=60 * 10 ** 6, max_rays=1 << 20, seed=0):
+    """Write the render outputs a caller of the step receives (``model.head.render``) as ``outdir/<name>.npy``, float32.
+    Per-ray arrays are sampled on the same fixed, seeded set of at most ``max_rays`` rays (all rays when the frame has
+    fewer), and the files stay under ``budget`` bytes in all;
+    ``ray_index.npy`` (float64) holds the flat (camera, pixel) index of every sampled ray, and the per-pixel ray table
+    ``ms_rays`` is sampled on the pixels of those rays.  Two builds run with the same arguments compare file by file."""
+    import numpy as np
+    R = n_cam * n_ray
+    arrays = {}
+    for k, v in out.items():
+        ts = list(v) if isinstance(v, (list, tuple)) else [v]
+        for i, t in enumerate(ts):
+            if torch.is_tensor(t) and t.numel() and t.is_floating_point():
+                arrays[k if len(ts) == 1 else '%s_%d' % (k, i)] = t.detach()
+    per_ray = lambda t: t.numel() % R == 0
+    per_pix = lambda t: not per_ray(t) and t.numel() % n_ray == 0
+    width = sum(t.numel() // R if per_ray(t) else t.numel() // n_ray for t in arrays.values() if per_ray(t) or per_pix(t))
+    n = min(R, max_rays, budget // (8 + 4 * width))
+    idx = np.arange(R) if n == R else np.sort(np.random.default_rng(seed).choice(R, n, replace=False))
+    os.makedirs(outdir, exist_ok=True)
+    np.save(os.path.join(outdir, 'ray_index.npy'), idx.astype(np.float64))
+    for name, t in arrays.items():
+        if per_ray(t):
+            t = t.reshape(R, -1)[torch.as_tensor(idx, device=t.device)]
+        elif per_pix(t):
+            t = t.reshape(n_ray, -1)[torch.as_tensor(idx % n_ray, device=t.device)]
+        np.save(os.path.join(outdir, name + '.npy'), t.float().cpu().numpy())
+
+
+# ------------------------------------------------------------------------------------------ GPU arm
 def run_b200(args):
     import torch.distributed as dist
     from selfocc_b200 import _lib
@@ -169,7 +202,7 @@ def run_b200(args):
     metas_d = [dict(lidar2img=to_dev('lidar2img'), img2lidar=to_dev('img2lidar'), img_shape=metas[0]['img_shape'])]
     n_cam, n_ray = 6, model.head.ray_sampler.ray_number
     rays_per_frame = n_cam * n_ray
-    flush = torch.empty(256 << 20, dtype=torch.uint8, device=dev)   # > 126 MB L2
+    flush = torch.empty(256 << 20, dtype=torch.uint8, device=dev)   # > the 50 MB L2 of an H100
 
     @torch.no_grad()
     def step(feats, m):
@@ -242,7 +275,12 @@ def run_b200(args):
     K, W = args.steps, max(args.warmup, 3)
     _lib.profile_enable(True)
     sampler = ClockSampler(local) if rank == 0 else None
-    total_ms, launches, clocks = timed(lambda: gather(step(feats_d, metas_d)), K, W, sampler, sample_clocks=True,
+    last = {}
+
+    def step_eager():
+        last['out'] = step(feats_d, metas_d)
+        return gather(last['out'])
+    total_ms, launches, clocks = timed(step_eager, K, W, sampler, sample_clocks=True,
                                        finalize=gather_join if world > 1 else None)
     prof = _lib.profile_read()
     ms_per_step_eager = total_ms / K
@@ -278,8 +316,11 @@ def run_b200(args):
                 return gather(g_out)
             total_ms, _, _ = timed(step_graph, K, W, finalize=gather_join if world > 1 else None)
             issue = 'CUDA graph replay of the step (collective outside the graph)'
+            last['out'] = g_out
         else:
             issue = 'eager issue (graph capture failed: %s)' % why
+    if args.dump_outputs and rank == 0:              # before the side measurements below replay the graph again
+        dump_outputs(last['out'], args.dump_outputs, n_cam, n_ray)
     ms_per_step = total_ms / K
     value = world * rays_per_frame / (ms_per_step * 1e-3)
 
@@ -425,12 +466,7 @@ def run_b200(args):
         if world > 1:
             dist.destroy_process_group()
         return
-    peaks = {}
-    try:
-        peaks = json.load(open(os.path.join(ROOT, 'MEASURED_PEAKS.json')))
-    except Exception:
-        pass
-    hbm_peak = float(peaks.get('hbm_gbs', 6650.0))
+    hbm_peak = 3350.0                          # H100 SXM data sheet, HBM3
     r_ms, r_calls = prof.get('render_infer', (0.0, 0))
     d = model.head.model.field.desc
     # algorithmic bytes of one render launch (DESIGN.md section 4): per ray the outputs actually written (rays are generated
@@ -442,9 +478,8 @@ def run_b200(args):
     achieved = alg_bytes / dur / 1e9 if dur > 0 else 0.0
     flop_per_ray = 256 * 150.0                # SURVEY 8d estimate: ~150 flop per sample
     roofline = {'kernel': 'render_packed_kernel<RGB=%d>' % int(has_rgb), 'bound': 'hbm', 'achieved': achieved, 'peak': hbm_peak,
-                'unit': 'GB/s', 'frac': achieved / hbm_peak, 'peak_source': 'measured' if peaks else 'fallback',
+                'unit': 'GB/s', 'frac': achieved / hbm_peak, 'peak_source': 'H100 SXM data sheet',
                 'launch_ms': dur * 1e3, 'algorithmic_bytes_per_launch': alg_bytes}
-    roofline.update(static_ncu_facts(has_rgb, args.workload))
     roofline['note'] = ('inference render is issue-slot bound by construction (~600 flop/B, SURVEY 8d caveat), not HBM-bound: '
                         'fp32 throughput estimate %.1f TFLOP/s; the HBM-bound form of this kernel is `roofline_train_form`'
                         % (rays_per_frame * flop_per_ray / dur / 1e12 if dur > 0 else 0))
@@ -493,25 +528,8 @@ def run_b200(args):
         sys.exit(3)
 
 
-def static_ncu_facts(has_rgb, workload):
-    """DRAM traffic and pipe utilisation of the render kernel cannot be measured inside a timed run; they come from the committed
-    `ncu --set full` capture of this same kernel and workload (profiles/, file named here).  `traffic` stays null until such a
-    capture exists for the variant."""
-    path = os.path.join(ROOT, 'profiles', 'r2_render_packed_ncu.json')
-    out = {'traffic': None, 'traffic_source': None}
-    try:
-        facts = json.load(open(path))
-        f = facts.get(workload, {}).get('rgb' if has_rgb else 'depth')
-        if f:
-            out = {'traffic': f['dram_bytes_read'] + f['dram_bytes_write'], 'traffic_source': 'static: profiles/r2_render_packed_ncu.json '
-                   '(ncu --set full of this kernel at this workload), not a measurement of this run', 'ncu': f}
-    except Exception:
-        pass
-    return out
-
-
 def reference_style_gpu(dev, color_dims, our_launch_s, rays_per_frame):
-    """BASELINE.md section 3 "reference-style GPU path": the oracle port in EAGER PyTorch on this B200 with the reference's own
+    """BASELINE.md section 3 "reference-style GPU path": the oracle port in EAGER PyTorch on this GPU with the reference's own
     structure -- python chunk loop of 90 000 rays (`--batch 90000`), autograd `grid_sample` field query, `cumprod`
     compositing, max-depth on the CPU (neus_head.py:329-374, 430-438).  Stands in for "the reference GPU path" of the
     north-star's >= 10x target (the reference cannot be installed offline).  Render only; bounded sample: 1 camera x
@@ -673,8 +691,8 @@ def cpu_reference(workload, steps, warmup, color_dims=3):
     from oracle.mapping import GridMeterMappingRef
     from oracle import lifting as ol, render as orender, rays as orays
     from selfocc_b200 import synth
-    # 32 OpenMP threads: on the shared 128-core hosts of this pool 128 threads spin against the other tenants and the same
-    # sample took 0.28 s .. 11.3 s from run to run (BENCH_r01, profiles/r2_bench_v1_rgb.json); `cores` reports what is used
+    # at most 32 OpenMP threads: on a shared many-core host, one thread per core spins against the other tenants and the
+    # sample time varies by an order of magnitude from run to run; `cores` reports what is used
     torch.set_num_threads(min(32, os.cpu_count()))
     w = WORKLOADS[workload]
     feats, metas, shapes = make_frame(workload, seed=100)

@@ -1,5 +1,5 @@
 /*
- * selfocc_b200 -- C ABI of the sm_100a hot-path library (libselfocc_b200.so).
+ * selfocc_b200 -- C ABI of the sm_90a hot-path library (libselfocc_b200.so).
  *
  * The reference (huang-yh/SelfOcc) has no FFI of its own: its boundary for this path is the
  * mmengine registry + nn.Module contracts (SURVEY.md section 8b).  This C ABI sits UNDER
@@ -105,7 +105,7 @@ int so_tpv_decode_bwd_hidden(float* z1_a1, const float* g_vol_sdf, const float* 
                              void* stream);
 int so_tpv_decode_bwd_input(float* g0, const float* a0, int64_t n, void* stream);
 
-/* Test hook: force the fp32 SIMT decode kernel (default: the tcgen05 3xTF32 kernel whenever C % 32 == 0). */
+/* Test hook: force the fp32 SIMT decode kernel (default: the wgmma 3xTF32 kernel whenever C % 32 == 0). */
 int so_tpv_decode_force_simt(int on);
 
 /* ---------------------------------------------------------------------------------------
@@ -270,14 +270,14 @@ int so_msda_backward(const float* value, const int64_t* spatial_shapes, const in
                      int32_t B, int32_t Nv, int32_t Hd, int32_t Dh, int32_t Nq, int32_t L, int32_t P,
                      void* stream);
 
-/* A6/A9  dense projection on the tcgen05 tensor cores with fp32-level accuracy ("3xTF32" operand splitting):
+/* A6/A9  dense projection on the Hopper tensor cores (wgmma) with fp32-level accuracy ("3xTF32" operand splitting):
  *     y[M,N] = act(x[M,K] * w[N,K]^T + bias[N]) (+ residual[M,N])
  * Replaces the nn.Linear calls of the attention modules and the FFN (image_cross_attention.py:36,218-223,309-317,
  * cross_view_hybrid_attention.py:79-86,118, tpvformer_encoder_layer.py:198-206).  w_hi / w_lo = so_split_tf32(w)
- * (w_hi = w with the low 13 mantissa bits cleared, w_lo = w - w_hi), computed once per weight.  K % 96 == 0;
- * x, w_hi, w_lo 16-byte aligned; relu: 0/1; bias / residual may be NULL. */
-/* Test hook: 1 = so_linear_3xtf32 with both MMA operands in shared memory (SS, the round-1 pipeline); 0 (default) = the X
- * operand split into tensor memory (TS).  Both are parity-tested. */
+ * (w_hi = w with the low 13 mantissa bits cleared, w_lo = w - w_hi), computed once per weight.  K % 96 == 0, N even;
+ * x, w_hi, w_lo 16-byte aligned (TMA), y and residual 8-byte aligned; relu: 0/1; bias / residual may be NULL. */
+/* Test hook: 1 = so_linear_3xtf32 with both MMA operands in shared memory; 0 (default) = the X operand split in
+ * registers.  Both are parity-tested. */
 int so_linear_force_ss(int on);
 int so_split_tf32(const float* w, float* w_hi, float* w_lo, int64_t n, void* stream);
 int so_linear_3xtf32(const float* x, const float* w_hi, const float* w_lo, const float* bias, const float* residual,

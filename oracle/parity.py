@@ -4,9 +4,8 @@ Why three comparisons.  The reference's field is a trilinear interpolant (bev_ne
 (``use_numerical_gradients=False``, config/nuscenes/nuscenes_depth.py:315) feeds the NeuS alpha; that gradient jumps
 across cell faces.  A sample that lies within fp32 rounding of a face (|g - round(g)| ~ 1e-5 grid units) is therefore
 assigned to one cell by any fp32 evaluation -- the reference's own included -- and possibly to the neighbour by an fp64
-evaluation, and on a low-accumulation ray one such sample moves the expected depth by up to ~1e-2 relative.  (Measured
-at BASELINE size, profiles/r2_parity_diag.json: the fp32 ORACLE differs from the fp64 oracle by 1.4e-2 on the same rays
-the kernel does, and by > 1e-4 on 2 075 of 21 600 rays versus 33 for the kernel.)  So the gate separates the questions:
+evaluation, and on a low-accumulation ray one such sample moves the expected depth by up to ~1e-2 relative (the fp32
+ORACLE misses the fp64 oracle on such rays as well; scripts/parity_diag.py reports both).  So the gate separates the questions:
 
   (a) geometry   : the kernel's sample coordinates (probe output) equal the fp64 oracle's within rounding
                    (|dg| <= geo_tol grid units) -- a continuous quantity, no discontinuity involved;

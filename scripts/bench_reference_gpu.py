@@ -1,4 +1,4 @@
-"""The "reference-style GPU path" of BASELINE.md section 3: the oracle port run in eager PyTorch ON the B200 with the
+"""The "reference-style GPU path" of BASELINE.md section 3: the oracle port run in eager PyTorch ON the GPU with the
 reference's own structure -- python chunk loop of 90 000 rays (`--batch 90000`), one autograd `grid_sample` field query
 per chunk, `cumprod` compositing, and the max-depth step on the CPU (neus_head.py:329-374, 430-438).  It stands in for
 "the reference GPU path" (the reference itself cannot be installed offline) in the north-star's >= 10x comparison.
@@ -36,6 +36,6 @@ run()
 ts = [run()[0] for _ in range(2)]
 t = min(ts)
 rays = 900 * 1600
-print(json.dumps({'impl': 'reference-style eager PyTorch on B200 (oracle port, chunked 90000 rays, CPU max-depth)',
+print(json.dumps({'impl': 'reference-style eager PyTorch on the GPU (oracle port, chunked 90000 rays, CPU max-depth)',
                   'rays': rays, 'seconds': t, 'rays_per_s_render_only': rays / t,
                   'frame_ms_extrapolated_6cams': 6 * t * 1e3}))

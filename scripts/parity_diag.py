@@ -4,7 +4,7 @@
 Renders a strided sub-grid of the bench frame with the CUDA kernels and with the oracle in several
 combinations so that a kernel bug, a decode (3xTF32) error and an ill-conditioned ray can be told apart:
 
-  K(tc)    kernel render of the tcgen05-decoded volume          (what bench.py's parity block measured)
+  K(tc)    kernel render of the tensor-core-decoded volume          (what bench.py's parity block measured)
   K(simt)  kernel render of the SIMT-decoded volume
   O64      fp64 oracle decode + fp64 oracle render              (the tolerance anchor)
   O64(tc)  fp64 oracle render of the kernel's own decoded volume (isolates the render kernel)

@@ -1,4 +1,4 @@
-"""Build libselfocc_b200.so in-tree with nvcc for sm_100a (no torch types, plain C ABI)."""
+"""Build libselfocc_b200.so in-tree with nvcc for sm_90a (H100; no torch types, plain C ABI)."""
 import os
 import subprocess
 import sys
@@ -10,7 +10,7 @@ LIB = os.path.join(LIB_DIR, 'libselfocc_b200.so')
 SOURCES = ['abi.cu', 'render.cu', 'render_fast.cu', 'field_hess.cu', 'metric.cu', 'render_train.cu', 'decode.cu', 'msda.cu', 'gemm.cu', 'norm.cu']
 # approx-unit math (ex2/rcp/rsq) without the denormal range-scaling wrappers: ~20 instructions per render sample
 PER_SOURCE_FLAGS = {'render.cu': ['-ftz=true'], 'render_fast.cu': ['-ftz=true'], 'render_train.cu': ['-ftz=true'], 'msda.cu': ['-ftz=true'], 'decode.cu': ['-ftz=true']}
-NVCC_FLAGS = ['-gencode', 'arch=compute_100a,code=sm_100a', '-O3', '-lineinfo', '-std=c++17',
+NVCC_FLAGS = ['-gencode', 'arch=compute_90a,code=sm_90a', '-O3', '-lineinfo', '-std=c++17',
               '--expt-relaxed-constexpr', '-Xcompiler', '-fPIC', '-Xptxas', '-v']
 
 
@@ -58,7 +58,7 @@ def build(force=False, verbose=False, out=None, defines=()):
     if verbose:
         print('\n'.join(log))
     target = LIB if out is None else os.path.join(LIB_DIR, os.path.basename(out))
-    cmd = [_nvcc(), '-shared', '-gencode', 'arch=compute_100a,code=sm_100a', '-o', target] + objs + ['-lcudart']
+    cmd = [_nvcc(), '-shared', '-gencode', 'arch=compute_90a,code=sm_90a', '-o', target] + objs + ['-lcudart']
     r = subprocess.run(cmd, stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True)
     if r.returncode != 0:
         raise RuntimeError('link failed:\n' + r.stdout)

@@ -10,6 +10,17 @@ thread_local int g_last_cuda_error = 0;
 static std::atomic<long long> g_launches{0};
 void note_launch(int n) { g_launches.fetch_add(n, std::memory_order_relaxed); }
 
+int num_sms() {
+  static std::atomic<int> cache[64];
+  int dev = 0, n = 0;
+  if (cudaGetDevice(&dev) != cudaSuccess) return 1;
+  std::atomic<int>& c = cache[dev & 63];
+  if ((n = c.load(std::memory_order_relaxed)) > 0) return n;
+  if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n < 1) return 1;
+  c.store(n, std::memory_order_relaxed);
+  return n;
+}
+
 // ---- optional device timing ---------------------------------------------------------------------------
 static bool g_prof_on = false;
 struct ProfTag {

@@ -1,4 +1,4 @@
-// Shared device/host helpers of libselfocc_b200 (sm_100a only).
+// Shared device/host helpers of libselfocc_b200 (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -20,7 +20,9 @@ inline int check_cuda(cudaError_t e) {
 // Launch-error check without synchronising.
 inline int check_launch() { return check_cuda(cudaGetLastError()); }
 
-constexpr int kNumSMs = 148;  // B200
+// SM count of the current device (cached per device ordinal): sizes the persistent grids of the GEMM and the decode and
+// caps the grid-stride kernels, so a 132-SM H100 SXM, a 114-SM H100 PCIe or a partitioned device each get one wave.
+int num_sms();
 
 // cudaFuncSetAttribute is PER DEVICE: a process-wide `static bool` would leave the second GPU of a multi-device process
 // without its opt-in shared-memory size.  One bit per device ordinal; setting the attribute twice is harmless, so the

@@ -122,15 +122,16 @@ __global__ void __launch_bounds__(kThreads) tpv_decode_kernel(
 }
 
 // ---------------------------------------------------------------------------------------------------------------------
-// Tensor-core variant (tcgen05, same 3xTF32 operand splitting as gemm.cu so the decoded sdf keeps fp32-level accuracy).
-// Persistent CTA per SM, 14 warps:
-//   warps 0-7  builders   A tile = softplus(hw + zh + wz) for 128 voxels x 32 channels at a time, split into TF32 hi / lo and
-//                         written straight into the 128B-swizzled K-major UMMA layout (no TMA: the operand is computed)
-//   warp  8    MMA        12 x tcgen05.mma.kind::tf32 per atom (hi*hi, lo*hi, hi*lo) into a double-buffered TMEM accumulator
-//   warps 10-13 epilogue   tcgen05.ld -> +b1 -> softplus -> second Linear (1 + n_feat outputs, register dot products) -> volume
+// Tensor-core variant (wgmma, same 3xTF32 operand splitting as gemm.cu so the decoded sdf keeps fp32-level accuracy).
+// Persistent CTA per SM, 16 warps:
+//   warps 0-7   builders   A tile = softplus(hw + zh + wz) for 128 voxels x 32 channels at a time, split into TF32 hi / lo and
+//                          written straight into the 128B-swizzled K-major operand layout (no TMA: the operand is computed)
+//   warps 8-15  two consumer warpgroups, 64 voxels each: 12 x wgmma.m64nCk8.tf32 per atom (hi*hi, lo*hi, hi*lo) into a
+//                          register accumulator; epilogue +b1 -> softplus -> second Linear (1 + n_feat outputs, dot products
+//                          over the 4 threads that share a row) -> volume
 // W1 (hi and lo, swizzled) stays resident in shared memory for the whole kernel.
-constexpr int kDecThreads = 448;
 constexpr int kDecBuilders = 256;
+constexpr int kDecThreads = kDecBuilders + 256;
 constexpr int kDecStagesMax = 4;
 
 struct DecSmem {
@@ -152,19 +153,19 @@ __host__ __device__ inline DecSmem dec_smem(int C, int n_out) {
   return m;
 }
 
-__device__ __forceinline__ uint32_t swz_off(int row, int chunk) { return (uint32_t)(row * 128 + ((chunk ^ (row & 7)) << 4)); }
-
-// NOUT = compile-time upper bound of the second layer's width (1 + n_feat): the per-row outputs stay in registers
-template <int NOUT>
+// C = channels (wgmma N); NOUT = compile-time upper bound of the second layer's width (1 + n_feat): the per-row outputs
+// stay in registers
+template <int C, int NOUT>
 __global__ void __launch_bounds__(kDecThreads, 1)
 tpv_decode_tc_kernel(const float* __restrict__ hw, const float* __restrict__ zh, const float* __restrict__ wz,
                      const float* __restrict__ w1, const float* __restrict__ b1, const float* __restrict__ w2,
-                     const float* __restrict__ b2, int C, int H, int W, int Z, int zpitch, int n_out, int feat_pitch,
+                     const float* __restrict__ b2, int H, int W, int Z, int zpitch, int n_out, int feat_pitch,
                      float* __restrict__ vol_sdf, float* __restrict__ vol_feat, int tiles_per_row, int n_tiles, int h_begin) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* sm = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
   const DecSmem L = dec_smem(C, n_out);
-  const int KA = L.atoms, stages = L.stages;
+  constexpr int KA = C / kAtomK;
+  const int stages = L.stages;
   uint8_t* w_hi = sm;
   uint8_t* w_lo = sm + KA * C * 128;
   uint8_t* ring = sm + L.ring;
@@ -173,18 +174,13 @@ tpv_decode_tc_kernel(const float* __restrict__ hw, const float* __restrict__ zh,
   float* b2s = reinterpret_cast<float*>(sm + L.b2);
   uint64_t* conv = reinterpret_cast<uint64_t*>(sm + L.bars);
   uint64_t* empty = conv + kDecStagesMax;
-  uint64_t* tmem_full = empty + kDecStagesMax;
-  uint64_t* tmem_empty = tmem_full + 2;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tmem_empty + 2);
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int WZ = W * Z;
 
   if (tid == 0) {
-    for (int s = 0; s < kDecStagesMax; ++s) { mbar_init(conv + s, kDecBuilders); mbar_init(empty + s, 1); }
-    for (int a = 0; a < 2; ++a) { mbar_init(tmem_full + a, 1); mbar_init(tmem_empty + a, 128); }
+    for (int s = 0; s < kDecStagesMax; ++s) { mbar_init(conv + s, kDecBuilders); mbar_init(empty + s, 8); }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  if (warp == 9) tmem_alloc(tmem_slot, 256);
   // W1 [out j][in k] is K-major already: split it and lay it out as KA swizzled atoms of [C rows x 32 k]
   for (int i = tid; i < C * C / 4; i += kDecThreads) {
     int j = (i * 4) / C, k = (i * 4) % C;
@@ -199,10 +195,7 @@ tpv_decode_tc_kernel(const float* __restrict__ hw, const float* __restrict__ zh,
   for (int i = tid; i < C; i += kDecThreads) b1s[i] = __ldg(b1 + i);
   for (int i = tid; i < n_out; i += kDecThreads) b2s[i] = __ldg(b2 + i);
   asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
 
   if (warp < 8) {
     // ===== builders: thread owns 16-byte chunk c4 of rows r = tid/8 + 32 j =====
@@ -252,78 +245,90 @@ tpv_decode_tc_kernel(const float* __restrict__ hw, const float* __restrict__ zh,
         if (++s == stages) { s = 0; ph ^= 1; }
       }
     }
-  } else if (warp == 8) {
-    // ===== MMA issuer =====
-    if (lane == 0) {
-      const uint32_t idesc = make_idesc(C);
-      const uint32_t whi = smem_u32(w_hi), wlo = smem_u32(w_lo);
-      int s = 0; uint32_t ph = 0;
-      int acc = 0; uint32_t acc_ph = 0;
-      for (int t = blockIdx.x; t < n_tiles; t += gridDim.x) {
-        mbar_wait(tmem_empty + acc, acc_ph ^ 1);
-        tc_fence_after();
-        const uint32_t d_tmem = tmem_base + (uint32_t)(acc * 128);
-        uint32_t accum = 0;
-        for (int a = 0; a < KA; ++a) {
-          mbar_wait(conv + s, ph);
-          tc_fence_after();
-          const uint32_t ahi = smem_u32(ring + s * 2 * kAtomBytesA), alo = ahi + kAtomBytesA;
-          const uint32_t bhi = whi + a * C * 128, blo = wlo + a * C * 128;
+  } else {
+    // ===== consumers: warpgroup wg owns voxels 64 wg .. 64 wg + 63 of every tile =====
+    const int wg = (warp - 8) >> 2, wl = warp & 3, g = lane >> 2, t4 = lane & 3;
+    const int frag_row = wg * kWgRows + wl * 16 + g;          // this thread's voxel rows: frag_row and frag_row + 8
+    const uint32_t whi = smem_u32(w_hi), wlo = smem_u32(w_lo);
+    float acc[C / 2];
 #pragma unroll
-          for (int prod = 0; prod < 3; ++prod) {
-            const uint32_t ab = prod == 1 ? alo : ahi;
-            const uint32_t bb = prod == 2 ? blo : bhi;
+    for (int i = 0; i < C / 2; ++i) acc[i] = 0.f;
+    int s = 0; uint32_t ph = 0;
+    for (int t = blockIdx.x; t < n_tiles; t += gridDim.x) {
+      const int hr = t / tiles_per_row, h = h_begin + hr, v0 = (t - hr * tiles_per_row) * kBM;
+      uint32_t accum = 0;
+      for (int a = 0; a < KA; ++a) {
+        mbar_wait(conv + s, ph);
+        const uint32_t ahi = smem_u32(ring + s * 2 * kAtomBytesA) + wg * kWgRows * 128, alo = ahi + kAtomBytesA;
+        const uint32_t bhi = whi + a * C * 128, blo = wlo + a * C * 128;
 #pragma unroll
-            for (int k = 0; k < kAtomK / 8; ++k) {
-              umma_tf32(d_tmem, make_desc(ab + k * 32), make_desc(bb + k * 32), idesc, accum);
-              accum = 1u;
+        for (int i = 0; i < C / 2; ++i) asm volatile("" : "+f"(acc[i])::"memory");
+        wg_fence();
+#pragma unroll
+        for (int prod = 0; prod < 3; ++prod) {
+          const uint32_t ab = prod == 1 ? alo : ahi;
+          const uint32_t bb = prod == 2 ? blo : bhi;
+#pragma unroll
+          for (int k = 0; k < kAtomK / 8; ++k) {
+            Wgmma<C>::ss(acc, make_desc(ab + k * 32), make_desc(bb + k * 32), accum);
+            accum = 1u;
+          }
+        }
+        wg_commit();
+        wg_wait0();
+#pragma unroll
+        for (int i = 0; i < C / 2; ++i) asm volatile("" : "+f"(acc[i])::"memory");
+        __syncwarp();
+        if (lane == 0) mbar_arrive(empty + s);
+        if (++s == stages) { s = 0; ph ^= 1; }
+      }
+      // ===== epilogue: hidden = softplus(acc + b1); out = W2 hidden + b2 =====
+      // RP voxel rows per pass over the 8-column blocks.  With a narrow second layer both rows go in one pass, so each
+      // block's accumulator registers die as it is consumed; with NOUT = 32 one row at a time keeps 32 sums live, not 64.
+      // Either way a row's sums are accumulated in the same order.
+      constexpr int RP = NOUT <= 4 ? 2 : 1;
+#pragma unroll
+      for (int p = 0; p < 2 / RP; ++p) {
+        float out[RP][NOUT];
+#pragma unroll
+        for (int r = 0; r < RP; ++r)
+#pragma unroll
+          for (int c = 0; c < NOUT; ++c) out[r][c] = 0.f;
+#pragma unroll
+        for (int j = 0; j < C / 8; ++j) {
+          const int col = 8 * j + 2 * t4;
+#pragma unroll
+          for (int r = 0; r < RP; ++r) {
+            const int hh = p * RP + r;
+            const float h0 = softplus_fast(acc[4 * j + 2 * hh] + b1s[col]);
+            const float h1 = softplus_fast(acc[4 * j + 2 * hh + 1] + b1s[col + 1]);
+#pragma unroll
+            for (int c = 0; c < NOUT; ++c)
+              if (c < n_out) out[r][c] = fmaf(h1, W2s[c * C + col + 1], fmaf(h0, W2s[c * C + col], out[r][c]));
+          }
+        }
+#pragma unroll
+        for (int r = 0; r < RP; ++r) {
+#pragma unroll
+          for (int c = 0; c < NOUT; ++c) {
+            out[r][c] += __shfl_xor_sync(0xffffffffu, out[r][c], 1);
+            out[r][c] += __shfl_xor_sync(0xffffffffu, out[r][c], 2);
+          }
+          const int v = v0 + frag_row + 8 * (p * RP + r);
+          if (v < WZ) {
+            const int w = v / Z, z = v - w * Z;
+#pragma unroll
+            for (int c = 0; c < NOUT; ++c) {
+              if (c >= n_out || (c & 3) != t4) continue;
+              const float o = out[r][c] + b2s[c];
+              if (c == 0) vol_sdf[((size_t)h * W + w) * zpitch + z] = o;
+              else vol_feat[(((size_t)h * W + w) * Z + z) * feat_pitch + (c - 1)] = o;
             }
           }
-          umma_commit(empty + s);
-          if (++s == stages) { s = 0; ph ^= 1; }
         }
-        umma_commit(tmem_full + acc);
-        if (++acc == 2) { acc = 0; acc_ph ^= 1; }
-      }
-    }
-  } else if (warp >= 10) {
-    // ===== epilogue: hidden = softplus(acc + b1); out = W2 hidden + b2 =====
-    const int q = warp & 3;                               // warps 10..13 -> TMEM lane quarters 2,3,0,1
-    const int r = q * 32 + lane;
-    int acc = 0; uint32_t acc_ph = 0;
-    for (int t = blockIdx.x; t < n_tiles; t += gridDim.x) {
-      const int hr = t / tiles_per_row, h = h_begin + hr, v = (t - hr * tiles_per_row) * kBM + r;
-      mbar_wait(tmem_full + acc, acc_ph);
-      tc_fence_after();
-      float out[NOUT];
-#pragma unroll
-      for (int c = 0; c < NOUT; ++c) out[c] = c < n_out ? b2s[c] : 0.f;
-      for (int c0 = 0; c0 < C; c0 += 32) {
-        uint32_t rg[32];
-        tmem_ld32(tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(acc * 128 + c0), rg);
-#pragma unroll
-        for (int j = 0; j < 32; ++j) {
-          const float hdn = softplus_fast(__uint_as_float(rg[j]) + b1s[c0 + j]);
-#pragma unroll
-          for (int c = 0; c < NOUT; ++c)
-            if (c < n_out) out[c] = fmaf(hdn, W2s[c * C + c0 + j], out[c]);
-        }
-      }
-      tc_fence_before();
-      mbar_arrive(tmem_empty + acc);
-      if (++acc == 2) { acc = 0; acc_ph ^= 1; }
-      if (v < WZ) {
-        const int w = v / Z, z = v - w * Z;
-        vol_sdf[((size_t)h * W + w) * zpitch + z] = out[0];
-#pragma unroll
-        for (int c = 1; c < NOUT; ++c)
-          if (c < n_out) vol_feat[(((size_t)h * W + w) * Z + z) * feat_pitch + (c - 1)] = out[c];
       }
     }
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 9) tmem_dealloc(tmem_base, 256);
 }
 
 __global__ void zero_pad_kernel(float* vol_sdf, long long columns, int Z, int zpitch) {
@@ -358,7 +363,7 @@ int launch_decode(const float* hw, const float* zh, const float* wz, const float
 using namespace so;
 
 static bool g_decode_force_simt = false;
-// Test hook: 1 = use the fp32 SIMT decode kernel even where the tcgen05 kernel applies (both are parity-tested).
+// Test hook: 1 = use the fp32 SIMT decode kernel even where the tensor-core kernel applies (both are parity-tested).
 extern "C" int so_tpv_decode_force_simt(int on) { g_decode_force_simt = on != 0; return SO_OK; }
 
 extern "C" int so_tpv_decode(const float* tpv_hw, const float* tpv_zh, const float* tpv_wz, int32_t C, const float* w1,
@@ -393,19 +398,29 @@ extern "C" int so_tpv_decode_rows(const float* tpv_hw, const float* tpv_zh, cons
     if (Ls.stages >= 2) {
       static PerDeviceOnce attr_tc;
       if ((rc = attr_tc.run([] {
-             int r;
-             if ((r = check_cuda(cudaFuncSetAttribute(tpv_decode_tc_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024)))) return r;
-             if ((r = check_cuda(cudaFuncSetAttribute(tpv_decode_tc_kernel<4>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024)))) return r;
-             return check_cuda(cudaFuncSetAttribute(tpv_decode_tc_kernel<32>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
+             int r = SO_OK;
+#define SO_DEC_ATTR(C_, NO) if (!r) r = check_cuda(cudaFuncSetAttribute(tpv_decode_tc_kernel<C_, NO>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024))
+#define SO_DEC_ATTR_C(C_) SO_DEC_ATTR(C_, 1); SO_DEC_ATTR(C_, 4); SO_DEC_ATTR(C_, 32)
+             SO_DEC_ATTR_C(32); SO_DEC_ATTR_C(64); SO_DEC_ATTR_C(96); SO_DEC_ATTR_C(128);
+#undef SO_DEC_ATTR_C
+#undef SO_DEC_ATTR
+             return r;
            })))
         return rc;
       const int tiles_per_row = (int)ceil_div64((int64_t)d->W * d->Z, kBM);
       const int n_tiles = tiles_per_row * h_count;
-      const int grid = n_tiles < kNumSMs ? n_tiles : kNumSMs;
+      const int sms = num_sms(), grid = n_tiles < sms ? n_tiles : sms;
       ProfScope prof(1, st);
-#define SO_DEC_TC(NO) tpv_decode_tc_kernel<NO><<<grid, kDecThreads, Ls.total, st>>>(tpv_hw, tpv_zh, tpv_wz, w1, b1, w2, b2, C, d->H, d->W, d->Z, \
-                                                                                  d->zpitch, n_out, d->feat_pitch, vol_sdf, vol_feat, tiles_per_row, n_tiles, h_begin)
-      if (n_out == 1) SO_DEC_TC(1); else if (n_out <= 4) SO_DEC_TC(4); else SO_DEC_TC(32);
+#define SO_DEC_TC(C_, NO) tpv_decode_tc_kernel<C_, NO><<<grid, kDecThreads, Ls.total, st>>>(tpv_hw, tpv_zh, tpv_wz, w1, b1, w2, b2, d->H, d->W, \
+                                                                                  d->Z, d->zpitch, n_out, d->feat_pitch, vol_sdf, vol_feat, tiles_per_row, n_tiles, h_begin)
+#define SO_DEC_TC_C(C_) if (n_out == 1) SO_DEC_TC(C_, 1); else if (n_out <= 4) SO_DEC_TC(C_, 4); else SO_DEC_TC(C_, 32)
+      switch (C) {
+        case 32: SO_DEC_TC_C(32); break;
+        case 64: SO_DEC_TC_C(64); break;
+        case 96: SO_DEC_TC_C(96); break;
+        default: SO_DEC_TC_C(128); break;
+      }
+#undef SO_DEC_TC_C
 #undef SO_DEC_TC
       note_launch(1);
       return check_launch();
@@ -423,7 +438,7 @@ extern "C" int so_tpv_decode_rows(const float* tpv_hw, const float* tpv_zh, cons
 // ---------------------------------------------------------------------------------------------------------------------
 // Backward of the decode MLP, one slab of h rows at a time (reference: autograd through TPVDecoder.forward,
 // model/head/base_head... the SDF/colour MLP in model/head/neus_head/bev_nerf.py:150-190 at the 1.65 M voxel centres).
-// The two M x C x C products of each slab run on the tcgen05 3xTF32 GEMM (so_linear_3xtf32); the kernels here are the
+// The two M x C x C products of each slab run on the tensor-core 3xTF32 GEMM (so_linear_3xtf32); the kernels here are the
 // element-wise pieces fused around them so every slab intermediate is written once and read once:
 //   features:  a0 = softplus(hw + zh + wz)                                       (recomputed, never stored by forward)
 //   hidden:    z1 -> a1 = softplus(z1);  g1 = (W2^T g_out) * sigmoid(z1);  g_out packed [rows][n_out]
@@ -498,7 +513,7 @@ static int bwd_slab_check(const so_volume_desc* d, int32_t C, int32_t h_begin, i
   return SO_OK;
 }
 static unsigned bwd_grid(long long n_vec) {
-  long long g = ceil_div64(n_vec, 256), cap = (long long)kNumSMs * 16;
+  long long g = ceil_div64(n_vec, 256), cap = (long long)num_sms() * 16;
   return (unsigned)(g < cap ? g : cap);
 }
 

@@ -1,27 +1,33 @@
-// Dense projections of the lifting path on the 5th-gen tensor cores (SURVEY.md section 8a rows A6, A9: value / offset /
+// Dense projections of the lifting path on the Hopper tensor cores (SURVEY.md section 8a rows A6, A9: value / offset /
 // weight / output Linear, FFN) with fp32-level accuracy:  Y = act(X W^T + b) [+ R]
 //
 //   X [M, K] fp32, W [N, K] fp32 (torch Linear layout, both K-major)  ->  Y [M, N] fp32
 //
 // Accuracy: the path feeds a 1e-4-relative depth bar, so plain TF32 (10-bit mantissa) is not acceptable.  Each
 // operand is split  v = hi + lo,  hi = v rounded to the nearest TF32 number (low 13 mantissa bits zero), lo = v - hi
-// (exact in fp32), and the product is accumulated as  hi*hi + lo*hi + hi*lo  in the fp32 TMEM accumulator
-// ("3xTF32", error ~2^-21).  W is split once on the host side (so_split_tf32); X is split in shared memory.
+// (exact in fp32), and the product is accumulated as  hi*hi + lo*hi + hi*lo  in the fp32 register accumulator
+// ("3xTF32", error ~2^-21).  W is split once on the host side (so_split_tf32); X is split by the consumer warps.
 //
-// Structure (one CTA = one 128 x BN output tile, 4 warps):
-//   TMA (cp.async.bulk.tensor.2d, 128B swizzle)  global -> smem   X tile [128 x 96] raw, W_hi / W_lo tiles [BN x 96]
-//   all threads: split X in place (hi) + second buffer (lo); fence.proxy.async
-//   one thread:  36 x tcgen05.mma.cta_group::1.kind::tf32  (3 products x 12 k-steps of 8), fp32 accumulator in TMEM
-//   tcgen05.commit -> mbarrier;  epilogue: tcgen05.ld 32x32b -> +bias, ReLU, +residual -> smem stage -> coalesced stores
-// K is consumed in chunks of 96 (3 swizzle atoms of 32 floats) that reuse the same buffers, so K = 192 (FFN) works too.
-// These GEMMs are HBM/L2-bound (K is tiny): M x (K + N) x 4 bytes per call.
+// Persistent, warp-specialised pipeline (one CTA per SM, 9 warps):
+//   warp 8      TMA producer   W tile (hi, lo; all K) once per CTA, then X atoms [128 x 32] (128B swizzle) into a ring of stages
+//   warps 0-7   two consumer warpgroups, 64 rows of the 128-row tile each: split the X atom into hi / lo, then
+//               3 products x 4 k-steps of wgmma.m64nBNk8.f32.tf32 into a register accumulator; epilogue (+bias, ReLU,
+//               +residual, optional LayerNorm over the row) straight from the accumulator registers to global memory.
+// A CTA owns ONE n-tile (its W tile stays resident in shared memory) and walks m-tiles, so the streamed traffic per
+// output tile is the X tile and the Y tile only.  mbarriers: w_full | full[s] (TMA landed) -> empty[s] (stage consumed).
+//
+// The A operand (X hi / lo) comes from REGISTERS by default: each thread loads its wgmma fragment from the swizzled
+// stage and splits it in registers, so the tensor core reads only W from shared memory and the stage is released as
+// soon as it has been loaded.  so_linear_force_ss(1) selects the variant with both operands in shared memory (the X
+// atom is split in place into hi plus a second lo buffer); both issue the same products in the same order.
 #include "tc_common.cuh"
 
 namespace so {
 
-constexpr int kChunkAtoms = 3;      // K chunk = 96
+constexpr int kGemmConsumers = 256;                 // two warpgroups
+constexpr int kGemmThreads = kGemmConsumers + 32;   // + the TMA producer warp
+constexpr int kMaxStages = 8;
 constexpr int kMaxBN = 128;
-constexpr int kGemmThreads = 128;
 
 typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
                                   const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
@@ -52,99 +58,66 @@ static int make_tmap(CUtensorMap* m, const float* base, int64_t rows, int64_t co
   return r == CUDA_SUCCESS ? SO_OK : SO_ERR_CUDA;
 }
 
-struct GemmSmem {
-  // offsets are relative to a 1024-byte aligned base
-  static constexpr int a_hi = 0;
-  static constexpr int a_lo = a_hi + kChunkAtoms * kAtomBytesA;
-  static constexpr int b_hi = a_lo + kChunkAtoms * kAtomBytesA;
-  static constexpr int b_lo = b_hi + kChunkAtoms * kMaxBN * 128;
-  static constexpr int bars = b_lo + kChunkAtoms * kMaxBN * 128;
-  static constexpr int total = bars + 64;
-};
-
-// ---------------------------------------------------------------------------------------------------------------------
-// Persistent, warp-specialised pipeline (one CTA per SM, 12 warps):
-//   warp 0      TMA producer   W tile (hi, lo; all K) once per CTA, then X atoms [128 x 32] into a ring of stages
-//   warp 1      MMA issuer     per atom: 3 products x 4 k-steps of tcgen05.mma.kind::tf32 into one of 2 TMEM accumulators
-//   warps 4-7   converters     split each raw X atom into hi (in place) and lo (second buffer), fence.proxy.async
-//   warps 8-11  epilogue       tcgen05.ld -> bias / ReLU / residual -> per-warp smem transpose -> coalesced stores
-// A CTA owns ONE n-tile (its W tile stays resident in shared memory) and walks m-tiles, so the streamed traffic per
-// output tile is the X tile and the Y tile only -- the HBM-bound minimum for these K = 96 projections.
-// mbarriers: w_full | full[s] (TMA landed) -> conv[s] (split done) -> empty[s] (MMAs retired) | tmem_full[a] / tmem_empty[a].
-constexpr int kStageBytes = 2 * kAtomBytesA;        // raw/hi atom + lo atom
-constexpr int kEpiWarpBytes = 32 * 128;             // per-warp TMA-store staging tile: 32 rows x 32 floats, 128B-swizzled
-constexpr int kPipeThreads = 384;
-constexpr int kMaxStages = 4;
-
 struct PipeCfg {
   int BN, KA, stages;       // n-tile width, atoms along K (K / 32), ring depth
-  int epi_bufs;             // TMA-store staging tiles per epilogue warp (2 when shared memory allows: store i overlaps staging i+1)
+  int stage_bytes;          // raw X atom (A from registers) or raw/hi + lo atoms (A from shared memory)
   int w_bytes;              // resident W bytes = 2 * KA * BN * 128
   int smem;                 // dynamic shared memory request (incl. 1 KB alignment slack)
 };
 
-// TS variant: a stage is the raw X atom only (16 KB); at most 4 stages (TMEM holds 4 x (hi | lo) x 32 columns next to the
-// two accumulators)
-static PipeCfg make_pipe_cfg_ts(int N, int K) {
+// n-tile width: the fewest padded columns, ties to the wider tile (fewer passes over X)
+static int pick_bn(int N) {
+  int best = kMaxBN, best_cols = (int)ceil_div64(N, kMaxBN) * kMaxBN;
+  for (int bn : {96, 64, 32}) {
+    const int cols = (int)ceil_div64(N, bn) * bn;
+    if (cols < best_cols) { best = bn; best_cols = cols; }
+  }
+  return best;
+}
+
+static PipeCfg make_pipe_cfg(int N, int K, bool reg_a) {
   PipeCfg c;
-  c.BN = (N % 128 == 0) ? 128 : (N % 96 == 0 ? 96 : (N % 112 == 0 ? 112 : (N <= 128 ? ((N + 15) / 16) * 16 : 128)));
+  c.BN = pick_bn(N);
   c.KA = K / kAtomK;
   c.w_bytes = 2 * c.KA * c.BN * 128;
-  c.epi_bufs = 2;
-  int fixed = c.w_bytes + 4 * c.epi_bufs * kEpiWarpBytes + kMaxBN * 12 + 256;
-  int budget = 227 * 1024 - 1024 - fixed;
-  if (budget / kAtomBytesA < 3) {
-    c.epi_bufs = 1;
-    fixed = c.w_bytes + 4 * kEpiWarpBytes + kMaxBN * 12 + 256;
-    budget = 227 * 1024 - 1024 - fixed;
-  }
-  c.stages = budget / kAtomBytesA;
+  c.stage_bytes = reg_a ? kAtomBytesA : 2 * kAtomBytesA;
+  const int fixed = c.w_bytes + 256;                          // + mbarriers
+  c.stages = (227 * 1024 - 1024 - fixed) / c.stage_bytes;
   if (c.stages > kMaxStages) c.stages = kMaxStages;
-  c.smem = fixed + c.stages * kAtomBytesA + 1024;
+  c.smem = fixed + c.stages * c.stage_bytes + 1024;
   return c;
 }
 
-static PipeCfg make_pipe_cfg(int N, int K) {
-  PipeCfg c;
-  c.BN = (N % 128 == 0) ? 128 : (N % 96 == 0 ? 96 : (N % 112 == 0 ? 112 : (N <= 128 ? ((N + 15) / 16) * 16 : 128)));
-  c.KA = K / kAtomK;
-  c.w_bytes = 2 * c.KA * c.BN * 128;
-  c.epi_bufs = 2;
-  int fixed = c.w_bytes + 4 * c.epi_bufs * kEpiWarpBytes + kMaxBN * 12 + 256;
-  int budget = 227 * 1024 - 1024 - fixed;
-  if (budget / kStageBytes < 3) {            // K = 192: the resident W tile leaves no room; keep the deeper load ring
-    c.epi_bufs = 1;
-    fixed = c.w_bytes + 4 * kEpiWarpBytes + kMaxBN * 12 + 256;
-    budget = 227 * 1024 - 1024 - fixed;
-  }
-  c.stages = budget / kStageBytes;
-  if (c.stages > kMaxStages) c.stages = kMaxStages;
-  c.smem = fixed + c.stages * kStageBytes + 1024;
-  return c;
+// keeps the compiler from moving accumulator / A-fragment reads and writes across the asynchronous wgmma
+template <int NR>
+__device__ __forceinline__ void fence_regs(float* r) {
+#pragma unroll
+  for (int i = 0; i < NR; ++i) asm volatile("" : "+f"(r[i])::"memory");
+}
+template <int NR>
+__device__ __forceinline__ void fence_regs(uint32_t* r) {
+#pragma unroll
+  for (int i = 0; i < NR; ++i) asm volatile("" : "+r"(r[i])::"memory");
 }
 
-
-__global__ void __launch_bounds__(kPipeThreads, 1)
-linear_3xtf32_pipe_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_constant__ CUtensorMap map_whi,
-                          const __grid_constant__ CUtensorMap map_wlo, const __grid_constant__ CUtensorMap map_y,
-                          const float* __restrict__ bias, const float* __restrict__ residual, long long M, int N, int BN, int KA,
-                          int stages, int n_tiles, int m_tiles, int relu, int epi_bufs) {
+template <int BN, bool kRegA>
+__global__ void __launch_bounds__(kGemmThreads, 1)
+linear_3xtf32_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_constant__ CUtensorMap map_whi,
+                     const __grid_constant__ CUtensorMap map_wlo, const float* __restrict__ bias,
+                     const float* __restrict__ residual, float* __restrict__ y, long long M, int N, int KA, int stages,
+                     int n_tiles, int m_tiles, int relu, const float* __restrict__ ln_gamma, const float* __restrict__ ln_beta,
+                     float ln_eps) {
+  constexpr int kStageBytes = kRegA ? kAtomBytesA : 2 * kAtomBytesA;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* sm = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
   const int w_bytes = 2 * KA * BN * 128;
   uint8_t* w_hi = sm;
   uint8_t* w_lo = sm + KA * BN * 128;
-  uint8_t* ring = sm + w_bytes;                                   // stages x [hi 16 KB | lo 16 KB], 1 KB aligned
-  uint8_t* epi = ring + stages * kStageBytes;                     // 4 x epi_bufs x 4 KB, 1 KB aligned (swizzle atoms)
-  float* bias_s = reinterpret_cast<float*>(epi + 4 * epi_bufs * kEpiWarpBytes);
-  uint64_t* bars = reinterpret_cast<uint64_t*>(bias_s + kMaxBN);
+  uint8_t* ring = sm + w_bytes;                                   // stages x kStageBytes, 1 KB aligned
+  uint64_t* bars = reinterpret_cast<uint64_t*>(ring + stages * kStageBytes);
   uint64_t* w_full = bars;
   uint64_t* full = bars + 1;
-  uint64_t* conv = full + kMaxStages;
-  uint64_t* empty = conv + kMaxStages;
-  uint64_t* tmem_full = empty + kMaxStages;
-  uint64_t* tmem_empty = tmem_full + 2;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tmem_empty + 2);
+  uint64_t* empty = full + kMaxStages;
 
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int n_tile = blockIdx.x % n_tiles;
@@ -153,17 +126,12 @@ linear_3xtf32_pipe_kernel(const __grid_constant__ CUtensorMap map_x, const __gri
 
   if (tid == 0) {
     mbar_init(w_full, 1);
-    for (int s = 0; s < kMaxStages; ++s) { mbar_init(full + s, 1); mbar_init(conv + s, 128); mbar_init(empty + s, 1); }
-    for (int a = 0; a < 2; ++a) { mbar_init(tmem_full + a, 1); mbar_init(tmem_empty + a, 128); }
+    for (int s = 0; s < kMaxStages; ++s) { mbar_init(full + s, 1); mbar_init(empty + s, kGemmConsumers / 32); }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  if (warp == 2) tmem_alloc(tmem_slot, 256);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
 
-  if (warp == 0) {
+  if (warp == kGemmConsumers / 32) {
     // ===== TMA producer =====
     if (lane == 0) {
       mbar_expect_tx(w_full, (uint32_t)w_bytes);
@@ -190,525 +158,159 @@ linear_3xtf32_pipe_kernel(const __grid_constant__ CUtensorMap map_x, const __gri
         }
       }
     }
-  } else if (warp == 1) {
-    // ===== MMA issuer =====
-    if (lane == 0) {
-      const uint32_t idesc = make_idesc(BN);
-      mbar_wait(w_full, 0);
-      int s = 0; uint32_t ph = 0;
-      int acc = 0; uint32_t acc_ph = 0;
-      const uint32_t whi = smem_u32(w_hi), wlo = smem_u32(w_lo);
-      for (int mt = group; mt < m_tiles; mt += n_groups) {
-        mbar_wait(tmem_empty + acc, acc_ph ^ 1);
-        tc_fence_after();
-        const uint32_t d_tmem = tmem_base + (uint32_t)(acc * 128);
-        uint32_t accum = 0;
-        for (int a = 0; a < KA; ++a) {
-          mbar_wait(conv + s, ph);
-          tc_fence_after();
-          const uint32_t ahi = smem_u32(ring + s * kStageBytes), alo = ahi + kAtomBytesA;
-          const uint32_t bhi = whi + a * BN * 128, blo = wlo + a * BN * 128;
+    return;
+  }
+
+  // ===== consumers: warpgroup wg owns rows 64 wg .. 64 wg + 63 of every m-tile =====
+  const int wg = warp >> 2, wl = warp & 3, g = lane >> 2, t = lane & 3;
+  const int frag_row = wg * kWgRows + wl * 16 + g;                // this thread's rows: frag_row and frag_row + 8
+  float acc[BN / 2];
 #pragma unroll
-          for (int prod = 0; prod < 3; ++prod) {
-            const uint32_t ab = prod == 1 ? alo : ahi;
-            const uint32_t bb = prod == 2 ? blo : bhi;
+  for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
+  const uint32_t whi = smem_u32(w_hi), wlo = smem_u32(w_lo);
+  mbar_wait(w_full, 0);
+  int s = 0; uint32_t ph = 0;
+  for (int mt = group; mt < m_tiles; mt += n_groups) {
+    uint32_t accum = 0;
+    for (int a = 0; a < KA; ++a) {
+      mbar_wait(full + s, ph);
+      uint8_t* stage = ring + s * kStageBytes;
+      const uint32_t bhi = whi + a * BN * 128, blo = wlo + a * BN * 128;
+      if constexpr (kRegA) {
+        // fragment of k-step kk: rows frag_row (+8), k = 8 kk + t and 8 kk + t + 4, i.e. 16-byte chunks 2 kk and 2 kk + 1;
+        // both rows have (row & 7) == g, so the swizzle is the same for the pair
+        const uint8_t* r0 = stage + frag_row * 128 + 4 * t;
+        uint32_t ah[16], al[16];
 #pragma unroll
-            for (int k = 0; k < kAtomK / 8; ++k) {
-              umma_tf32(d_tmem, make_desc(ab + k * 32), make_desc(bb + k * 32), idesc, accum);
-              accum = 1u;
-            }
+        for (int kk = 0; kk < 4; ++kk) {
+          const float v[4] = {*reinterpret_cast<const float*>(r0 + (((2 * kk) ^ g) << 4)),
+                              *reinterpret_cast<const float*>(r0 + 8 * 128 + (((2 * kk) ^ g) << 4)),
+                              *reinterpret_cast<const float*>(r0 + (((2 * kk + 1) ^ g) << 4)),
+                              *reinterpret_cast<const float*>(r0 + 8 * 128 + (((2 * kk + 1) ^ g) << 4))};
+#pragma unroll
+          for (int i = 0; i < 4; ++i) {
+            const float h = tf32_rn(v[i]);
+            ah[4 * kk + i] = __float_as_uint(h);
+            al[4 * kk + i] = __float_as_uint(v[i] - h);
           }
-          umma_commit(empty + s);                       // stage reusable once these MMAs have read it
-          if (++s == stages) { s = 0; ph ^= 1; }
         }
-        umma_commit(tmem_full + acc);                   // accumulator complete
-        if (++acc == 2) { acc = 0; acc_ph ^= 1; }
-      }
-    }
-  } else if (warp >= 4 && warp < 8) {
-    // ===== converters: X = hi + lo =====
-    const int ct = tid - 128;
-    int s = 0; uint32_t ph = 0;
-    for (int mt = group; mt < m_tiles; mt += n_groups) {
-      for (int a = 0; a < KA; ++a) {
-        mbar_wait(full + s, ph);
-        float4* hi = reinterpret_cast<float4*>(ring + s * kStageBytes);
-        float4* lo = reinterpret_cast<float4*>(ring + s * kStageBytes + kAtomBytesA);
+        fence_regs<16>(ah);
+        fence_regs<16>(al);
+        __syncwarp();
+        if (lane == 0) mbar_arrive(empty + s);          // the stage is in registers: the producer may refill it
+        fence_regs<BN / 2>(acc);
+        wg_fence();
 #pragma unroll
-        for (int i = 0; i < kAtomBytesA / 16 / 128; ++i) {
-          float4 v = hi[ct + i * 128], h, l;
+        for (int prod = 0; prod < 3; ++prod) {
+          const uint32_t* af = prod == 1 ? al : ah;
+          const uint32_t bb = prod == 2 ? blo : bhi;
+#pragma unroll
+          for (int kk = 0; kk < kAtomK / 8; ++kk) {
+            Wgmma<BN>::rs(acc, af + 4 * kk, make_desc(bb + kk * 32), accum);
+            accum = 1u;
+          }
+        }
+        wg_commit();
+        wg_wait0();
+        fence_regs<BN / 2>(acc);
+      } else {
+        // split this warpgroup's 64 rows in place: raw -> hi, lo into the second half of the stage.  Element-wise, so the
+        // swizzle is irrelevant.
+        float4* hi = reinterpret_cast<float4*>(stage + wg * kWgRows * 128);
+        float4* lo = reinterpret_cast<float4*>(stage + kAtomBytesA + wg * kWgRows * 128);
+        const int wt = tid & 127;
+#pragma unroll
+        for (int i = 0; i < kWgRows * 128 / 16 / 128; ++i) {
+          float4 v = hi[wt + i * 128], h, l;
           h.x = tf32_rn(v.x); l.x = v.x - h.x;
           h.y = tf32_rn(v.y); l.y = v.y - h.y;
           h.z = tf32_rn(v.z); l.z = v.z - h.z;
           h.w = tf32_rn(v.w); l.w = v.w - h.w;
-          hi[ct + i * 128] = h;
-          lo[ct + i * 128] = l;
+          hi[wt + i * 128] = h;
+          lo[wt + i * 128] = l;
         }
-        asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-        mbar_arrive(conv + s);
-        if (++s == stages) { s = 0; ph ^= 1; }
-      }
-    }
-  } else if (warp >= 8) {
-    // ===== epilogue: TMEM -> registers (+bias, ReLU, +residual) -> swizzled smem tile -> TMA store =====
-    const int q = warp & 3;                              // TMEM lane quarter of this warp
-    uint8_t* tile0 = epi + q * epi_bufs * kEpiWarpBytes;
-    int ebuf = 0;
-    for (int i = tid - 256; i < BN; i += 128) bias_s[i] = (bias && n0 + i < N) ? __ldg(bias + n0 + i) : 0.f;
-    asm volatile("bar.sync 1, 128;" ::: "memory");        // the 4 epilogue warps only
-    int acc = 0; uint32_t acc_ph = 0;
-    for (int mt = group; mt < m_tiles; mt += n_groups) {
-      mbar_wait(tmem_full + acc, acc_ph);
-      tc_fence_after();
-      const long long gr = (long long)mt * kBM + q * 32 + lane;      // this thread's output row
-      for (int c0 = 0; c0 < BN; c0 += 32) {
-        uint32_t r[32];
-        tmem_ld32(tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(acc * 128 + c0), r);
-        uint8_t* tile = tile0 + ebuf * kEpiWarpBytes;
-        if (lane == 0) {                                  // the store that last used THIS staging tile has finished reading it
-          if (epi_bufs == 2) tma_store_wait_read1(); else tma_store_wait_read();
-        }
-        if (epi_bufs == 2) ebuf ^= 1;
-        __syncwarp();
+        asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // generic-proxy smem writes -> visible to wgmma
+        wg_sync(1 + wg);
+        const uint32_t ahi = smem_u32(stage + wg * kWgRows * 128), alo = ahi + kAtomBytesA;
+        fence_regs<BN / 2>(acc);
+        wg_fence();
 #pragma unroll
-        for (int j = 0; j < 8; ++j) {
-          float4 bv = *reinterpret_cast<const float4*>(bias_s + c0 + 4 * j);
-          float4 v = make_float4(__uint_as_float(r[4 * j]) + bv.x, __uint_as_float(r[4 * j + 1]) + bv.y,
-                                 __uint_as_float(r[4 * j + 2]) + bv.z, __uint_as_float(r[4 * j + 3]) + bv.w);
-          if (relu) { v.x = fmaxf(v.x, 0.f); v.y = fmaxf(v.y, 0.f); v.z = fmaxf(v.z, 0.f); v.w = fmaxf(v.w, 0.f); }
-          if (residual) {
-            const int gc = n0 + c0 + 4 * j;
-            if (gr < M && gc + 3 < N) {
-              float4 rr = __ldg(reinterpret_cast<const float4*>(residual + gr * N + gc));
-              v.x += rr.x; v.y += rr.y; v.z += rr.z; v.w += rr.w;
-            } else if (gr < M) {
-              if (gc < N) v.x += __ldg(residual + gr * N + gc);
-              if (gc + 1 < N) v.y += __ldg(residual + gr * N + gc + 1);
-              if (gc + 2 < N) v.z += __ldg(residual + gr * N + gc + 2);
-            }
-          }
-          // 128-byte swizzle: 16-byte chunk j of row `lane` lives at chunk (j ^ (lane & 7))
-          *reinterpret_cast<float4*>(tile + lane * 128 + ((j ^ (lane & 7)) << 4)) = v;
-        }
-        asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-        __syncwarp();
-        // TMA clips rows >= M and columns >= N; chunks that start beyond this n-tile's width are skipped
-        if (lane == 0 && n0 + c0 < N) tma_store_2d(&map_y, tile, n0 + c0, mt * kBM + q * 32);
-      }
-      tc_fence_before();
-      mbar_arrive(tmem_empty + acc);
-      if (++acc == 2) { acc = 0; acc_ph ^= 1; }
-    }
-    if (lane == 0) tma_store_wait_all();
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 2) tmem_dealloc(tmem_base, 256);
-}
-
-// LayerNorm-fused epilogue of one 32-row slice of an m-tile (one epilogue warp, thread = row).  NCH = BN / 32 accumulator
-// chunks are read into registers (compile-time count: no local memory), the accumulator is released to the MMA warp right
-// away, then mean / variance (two passes over the registers), scale / shift, swizzled staging and one TMA store per chunk.
-template <int NCH>
-__device__ __forceinline__ void epilogue_ln(uint32_t tm, const float* __restrict__ bias_s, const float* __restrict__ gamma_s,
-                                            const float* __restrict__ beta_s, const float* __restrict__ residual, int relu, long long gr,
-                                            long long M, int N, float eps, uint8_t* tile0, int& ebuf, int epi_bufs, int lane,
-                                            const CUtensorMap* map_y, int row0, uint64_t* tmem_empty_bar) {
-  float v[NCH][32];
+        for (int prod = 0; prod < 3; ++prod) {
+          const uint32_t ab = prod == 1 ? alo : ahi;
+          const uint32_t bb = prod == 2 ? blo : bhi;
 #pragma unroll
-  for (int c = 0; c < NCH; ++c) {
-    uint32_t r[32];
-    tmem_ld32(tm + (uint32_t)(c * 32), r);
-#pragma unroll
-    for (int i = 0; i < 32; ++i) {
-      float t = __uint_as_float(r[i]) + bias_s[c * 32 + i];
-      if (relu) t = fmaxf(t, 0.f);
-      v[c][i] = t;
-    }
-    if (residual && gr < M) {
-#pragma unroll
-      for (int j = 0; j < 8; ++j) {
-        const float4 rr = __ldg(reinterpret_cast<const float4*>(residual + gr * N + c * 32 + 4 * j));
-        v[c][4 * j] += rr.x; v[c][4 * j + 1] += rr.y; v[c][4 * j + 2] += rr.z; v[c][4 * j + 3] += rr.w;
-      }
-    }
-  }
-  tc_fence_before();
-  mbar_arrive(tmem_empty_bar);                            // the accumulator is in registers: the MMA warp may overwrite it
-  float sum = 0.f;
-#pragma unroll
-  for (int c = 0; c < NCH; ++c)
-#pragma unroll
-    for (int i = 0; i < 32; ++i) sum += v[c][i];
-  const float mean = sum / (float)(NCH * 32);
-  float sq = 0.f;
-#pragma unroll
-  for (int c = 0; c < NCH; ++c)
-#pragma unroll
-    for (int i = 0; i < 32; ++i) { const float d = v[c][i] - mean; sq = fmaf(d, d, sq); }
-  const float rstd = rsqrtf(sq / (float)(NCH * 32) + eps);
-#pragma unroll
-  for (int c = 0; c < NCH; ++c) {
-    uint8_t* tile = tile0 + ebuf * kEpiWarpBytes;
-    if (lane == 0) {
-      if (epi_bufs == 2) tma_store_wait_read1(); else tma_store_wait_read();
-    }
-    if (epi_bufs == 2) ebuf ^= 1;
-    __syncwarp();
-#pragma unroll
-    for (int j = 0; j < 8; ++j) {
-      float4 o;
-      o.x = (v[c][4 * j] - mean) * rstd * gamma_s[c * 32 + 4 * j] + beta_s[c * 32 + 4 * j];
-      o.y = (v[c][4 * j + 1] - mean) * rstd * gamma_s[c * 32 + 4 * j + 1] + beta_s[c * 32 + 4 * j + 1];
-      o.z = (v[c][4 * j + 2] - mean) * rstd * gamma_s[c * 32 + 4 * j + 2] + beta_s[c * 32 + 4 * j + 2];
-      o.w = (v[c][4 * j + 3] - mean) * rstd * gamma_s[c * 32 + 4 * j + 3] + beta_s[c * 32 + 4 * j + 3];
-      *reinterpret_cast<float4*>(tile + lane * 128 + ((j ^ (lane & 7)) << 4)) = o;
-    }
-    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-    __syncwarp();
-    if (lane == 0) tma_store_2d(map_y, tile, c * 32, row0);
-  }
-}
-
-// ---------------------------------------------------------------------------------------------------------------------
-// TS variant of the pipeline: the A operand (X split into hi / lo) lives in TENSOR MEMORY instead of shared memory.
-// Why: with both operands in shared memory every one of the 12 MMAs of an atom re-reads a 4 KB A slice and a 4 KB B slice,
-// and the converters write hi and lo back to shared memory: ~180 KB of shared-memory traffic per 16 KB atom = ~1 400
-// cycles at 128 B/clk against 768 cycles of tensor-core time -- the SS pipeline is shared-memory-bandwidth bound
-// (ncu: tensor pipe <= 11 %).  With A in TMEM the MMAs read only B from shared memory and the converters write to TMEM
-// (tcgen05.st, 256 B/clk): ~100 KB per atom.  TMEM: columns [0, 256) two accumulators, [256, 512) 4 stages x (hi | lo) x 32.
-__global__ void __launch_bounds__(kPipeThreads, 1)
-linear_3xtf32_ts_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_constant__ CUtensorMap map_whi,
-                          const __grid_constant__ CUtensorMap map_wlo, const __grid_constant__ CUtensorMap map_y,
-                          const float* __restrict__ bias, const float* __restrict__ residual, long long M, int N, int BN, int KA,
-                          int stages, int n_tiles, int m_tiles, int relu, int epi_bufs, const float* __restrict__ ln_gamma,
-                          const float* __restrict__ ln_beta, float ln_eps) {
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t* sm = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-  const int w_bytes = 2 * KA * BN * 128;
-  uint8_t* w_hi = sm;
-  uint8_t* w_lo = sm + KA * BN * 128;
-  uint8_t* ring = sm + w_bytes;                                   // stages x raw X atom (16 KB), 1 KB aligned
-  uint8_t* epi = ring + stages * kAtomBytesA;                     // 4 x epi_bufs x 4 KB, 1 KB aligned (swizzle atoms)
-  float* bias_s = reinterpret_cast<float*>(epi + 4 * epi_bufs * kEpiWarpBytes);
-  float* gamma_s = bias_s + kMaxBN;                               // LayerNorm-fused epilogue (ln_gamma != nullptr): scale / shift
-  float* beta_s = gamma_s + kMaxBN;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(beta_s + kMaxBN);
-  uint64_t* w_full = bars;
-  uint64_t* full = bars + 1;
-  uint64_t* conv = full + kMaxStages;
-  uint64_t* empty = conv + kMaxStages;
-  uint64_t* tmem_full = empty + kMaxStages;
-  uint64_t* tmem_empty = tmem_full + 2;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tmem_empty + 2);
-
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  const int n_tile = blockIdx.x % n_tiles;
-  const int group = blockIdx.x / n_tiles, n_groups = gridDim.x / n_tiles;
-  const int n0 = n_tile * BN;
-
-  if (tid == 0) {
-    mbar_init(w_full, 1);
-    for (int s = 0; s < kMaxStages; ++s) { mbar_init(full + s, 1); mbar_init(conv + s, 128); mbar_init(empty + s, 1); }
-    for (int a = 0; a < 2; ++a) { mbar_init(tmem_full + a, 1); mbar_init(tmem_empty + a, 128); }
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  }
-  if (warp == 2) tmem_alloc(tmem_slot, 512);          // [0, 256): two accumulators; [256, 512): stages x (A hi | A lo) x 32 columns
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-
-  if (warp == 0) {
-    // ===== TMA producer =====
-    if (lane == 0) {
-      mbar_expect_tx(w_full, (uint32_t)w_bytes);
-      for (int a = 0; a < KA; ++a) {
-        tma_load_2d(w_hi + a * BN * 128, &map_whi, a * kAtomK, n0, w_full);
-        tma_load_2d(w_lo + a * BN * 128, &map_wlo, a * kAtomK, n0, w_full);
-      }
-      int s = 0; uint32_t ph = 0;
-      constexpr int kPrefetchTiles = 4;                 // X tiles requested into L2 ahead of the smem ring
-      for (int p = 0; p < kPrefetchTiles; ++p) {
-        int mt = group + p * n_groups;
-        if (mt < m_tiles)
-          for (int a = 0; a < KA; ++a) tma_prefetch_l2_2d(&map_x, a * kAtomK, mt * kBM);
-      }
-      for (int mt = group; mt < m_tiles; mt += n_groups) {
-        const int mt_pf = mt + kPrefetchTiles * n_groups;
-        if (mt_pf < m_tiles)
-          for (int a = 0; a < KA; ++a) tma_prefetch_l2_2d(&map_x, a * kAtomK, mt_pf * kBM);
-        for (int a = 0; a < KA; ++a) {
-          mbar_wait(empty + s, ph ^ 1);
-          mbar_expect_tx(full + s, (uint32_t)kAtomBytesA);
-          tma_load_2d(ring + s * kAtomBytesA, &map_x, a * kAtomK, mt * kBM, full + s);
-          if (++s == stages) { s = 0; ph ^= 1; }
-        }
-      }
-    }
-  } else if (warp == 1) {
-    // ===== MMA issuer =====
-    if (lane == 0) {
-      const uint32_t idesc = make_idesc(BN);
-      mbar_wait(w_full, 0);
-      int s = 0; uint32_t ph = 0;
-      int acc = 0; uint32_t acc_ph = 0;
-      const uint32_t whi = smem_u32(w_hi), wlo = smem_u32(w_lo);
-      for (int mt = group; mt < m_tiles; mt += n_groups) {
-        mbar_wait(tmem_empty + acc, acc_ph ^ 1);
-        tc_fence_after();
-        const uint32_t d_tmem = tmem_base + (uint32_t)(acc * 128);
-        uint32_t accum = 0;
-        for (int a = 0; a < KA; ++a) {
-          mbar_wait(conv + s, ph);
-          tc_fence_after();
-          const uint32_t ahi = tmem_base + 256u + (uint32_t)(s * 64), alo = ahi + 32u;     // A operand in tensor memory
-          const uint32_t bhi = whi + a * BN * 128, blo = wlo + a * BN * 128;
-#pragma unroll
-          for (int prod = 0; prod < 3; ++prod) {
-            const uint32_t ab = prod == 1 ? alo : ahi;
-            const uint32_t bb = prod == 2 ? blo : bhi;
-#pragma unroll
-            for (int k = 0; k < kAtomK / 8; ++k) {
-              umma_tf32_ts(d_tmem, ab + (uint32_t)(k * 8), make_desc(bb + k * 32), idesc, accum);
-              accum = 1u;
-            }
-          }
-          umma_commit(empty + s);                       // stage reusable once these MMAs have read it
-          if (++s == stages) { s = 0; ph ^= 1; }
-        }
-        umma_commit(tmem_full + acc);                   // accumulator complete
-        if (++acc == 2) { acc = 0; acc_ph ^= 1; }
-      }
-    }
-  } else if (warp >= 4 && warp < 8) {
-    // ===== converters: X = hi + lo, written into TENSOR MEMORY (the A operand of the MMAs) =====
-    // warp w owns TMEM lanes 32 (w & 3) .. + 31 = tile rows; thread = one row: its 32 k-values are one 128-byte swizzled
-    // shared-memory row (chunk j lives at j ^ (row & 7)); hi and lo go to 32 TMEM columns each with tcgen05.st.
-    const int q = warp & 3;
-    const int row = q * 32 + lane;
-    int s = 0; uint32_t ph = 0;
-    for (int mt = group; mt < m_tiles; mt += n_groups) {
-      for (int a = 0; a < KA; ++a) {
-        mbar_wait(full + s, ph);
-        const uint8_t* src = ring + s * kAtomBytesA + row * 128;
-        uint32_t hi[32], lo[32];
-#pragma unroll
-        for (int j = 0; j < 8; ++j) {
-          const float4 v = *reinterpret_cast<const float4*>(src + ((j ^ (row & 7)) << 4));
-          float h;
-          h = tf32_rn(v.x); hi[4 * j] = __float_as_uint(h); lo[4 * j] = __float_as_uint(v.x - h);
-          h = tf32_rn(v.y); hi[4 * j + 1] = __float_as_uint(h); lo[4 * j + 1] = __float_as_uint(v.y - h);
-          h = tf32_rn(v.z); hi[4 * j + 2] = __float_as_uint(h); lo[4 * j + 2] = __float_as_uint(v.z - h);
-          h = tf32_rn(v.w); hi[4 * j + 3] = __float_as_uint(h); lo[4 * j + 3] = __float_as_uint(v.w - h);
-        }
-        const uint32_t ta = tmem_base + ((uint32_t)(q * 32) << 16) + 256u + (uint32_t)(s * 64);
-        tmem_st32(ta, hi);
-        tmem_st32(ta + 32u, lo);
-        tmem_st_wait();
-        tc_fence_before();
-        mbar_arrive(conv + s);
-        if (++s == stages) { s = 0; ph ^= 1; }
-      }
-    }
-  } else if (warp >= 8) {
-    // ===== epilogue: TMEM -> registers (+bias, ReLU, +residual) -> swizzled smem tile -> TMA store =====
-    const int q = warp & 3;                              // TMEM lane quarter of this warp
-    uint8_t* tile0 = epi + q * epi_bufs * kEpiWarpBytes;
-    int ebuf = 0;
-    for (int i = tid - 256; i < BN; i += 128) {
-      bias_s[i] = (bias && n0 + i < N) ? __ldg(bias + n0 + i) : 0.f;
-      gamma_s[i] = (ln_gamma && n0 + i < N) ? __ldg(ln_gamma + n0 + i) : 0.f;
-      beta_s[i] = (ln_beta && n0 + i < N) ? __ldg(ln_beta + n0 + i) : 0.f;
-    }
-    asm volatile("bar.sync 1, 128;" ::: "memory");        // the 4 epilogue warps only
-    int acc = 0; uint32_t acc_ph = 0;
-    for (int mt = group; mt < m_tiles; mt += n_groups) {
-      mbar_wait(tmem_full + acc, acc_ph);
-      tc_fence_after();
-      const long long gr = (long long)mt * kBM + q * 32 + lane;      // this thread's output row
-      if (ln_gamma) {
-        // LayerNorm over the row (the launcher guarantees one n-tile: BN == N): y = LN(x W^T + b [relu] [+ residual]) * gamma + beta.
-        // A thread owns a whole output row, so the statistics need no cross-thread traffic.
-        const uint32_t tm = tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(acc * 128);
-        switch (BN >> 5) {
-          case 1: epilogue_ln<1>(tm, bias_s, gamma_s, beta_s, residual, relu, gr, M, N, ln_eps, tile0, ebuf, epi_bufs, lane, &map_y, mt * kBM + q * 32, tmem_empty + acc); break;
-          case 2: epilogue_ln<2>(tm, bias_s, gamma_s, beta_s, residual, relu, gr, M, N, ln_eps, tile0, ebuf, epi_bufs, lane, &map_y, mt * kBM + q * 32, tmem_empty + acc); break;
-          case 3: epilogue_ln<3>(tm, bias_s, gamma_s, beta_s, residual, relu, gr, M, N, ln_eps, tile0, ebuf, epi_bufs, lane, &map_y, mt * kBM + q * 32, tmem_empty + acc); break;
-          default: epilogue_ln<4>(tm, bias_s, gamma_s, beta_s, residual, relu, gr, M, N, ln_eps, tile0, ebuf, epi_bufs, lane, &map_y, mt * kBM + q * 32, tmem_empty + acc); break;
-        }
-        if (++acc == 2) { acc = 0; acc_ph ^= 1; }
-        continue;
-      }
-      for (int c0 = 0; c0 < BN; c0 += 32) {
-        uint32_t r[32];
-        tmem_ld32(tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(acc * 128 + c0), r);
-        uint8_t* tile = tile0 + ebuf * kEpiWarpBytes;
-        if (lane == 0) {                                  // the store that last used THIS staging tile has finished reading it
-          if (epi_bufs == 2) tma_store_wait_read1(); else tma_store_wait_read();
-        }
-        if (epi_bufs == 2) ebuf ^= 1;
-        __syncwarp();
-#pragma unroll
-        for (int j = 0; j < 8; ++j) {
-          float4 bv = *reinterpret_cast<const float4*>(bias_s + c0 + 4 * j);
-          float4 v = make_float4(__uint_as_float(r[4 * j]) + bv.x, __uint_as_float(r[4 * j + 1]) + bv.y,
-                                 __uint_as_float(r[4 * j + 2]) + bv.z, __uint_as_float(r[4 * j + 3]) + bv.w);
-          if (relu) { v.x = fmaxf(v.x, 0.f); v.y = fmaxf(v.y, 0.f); v.z = fmaxf(v.z, 0.f); v.w = fmaxf(v.w, 0.f); }
-          if (residual) {
-            const int gc = n0 + c0 + 4 * j;
-            if (gr < M && gc + 3 < N) {
-              float4 rr = __ldg(reinterpret_cast<const float4*>(residual + gr * N + gc));
-              v.x += rr.x; v.y += rr.y; v.z += rr.z; v.w += rr.w;
-            } else if (gr < M) {
-              if (gc < N) v.x += __ldg(residual + gr * N + gc);
-              if (gc + 1 < N) v.y += __ldg(residual + gr * N + gc + 1);
-              if (gc + 2 < N) v.z += __ldg(residual + gr * N + gc + 2);
-            }
-          }
-          // 128-byte swizzle: 16-byte chunk j of row `lane` lives at chunk (j ^ (lane & 7))
-          *reinterpret_cast<float4*>(tile + lane * 128 + ((j ^ (lane & 7)) << 4)) = v;
-        }
-        asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-        __syncwarp();
-        // TMA clips rows >= M and columns >= N; chunks that start beyond this n-tile's width are skipped
-        if (lane == 0 && n0 + c0 < N) tma_store_2d(&map_y, tile, n0 + c0, mt * kBM + q * 32);
-      }
-      tc_fence_before();
-      mbar_arrive(tmem_empty + acc);
-      if (++acc == 2) { acc = 0; acc_ph ^= 1; }
-    }
-    if (lane == 0) tma_store_wait_all();
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 2) tmem_dealloc(tmem_base, 512);
-}
-
-__global__ void __launch_bounds__(kGemmThreads, 1)
-linear_3xtf32_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_constant__ CUtensorMap map_whi,
-                     const __grid_constant__ CUtensorMap map_wlo, const float* __restrict__ bias,
-                     const float* __restrict__ residual, float* __restrict__ y, long long M, int N, int K, int BN, int relu) {
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t* sm = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-  uint64_t* bar_load = reinterpret_cast<uint64_t*>(sm + GemmSmem::bars);
-  uint64_t* bar_mma = bar_load + 1;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bar_load + 2);
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  const long long m0 = (long long)blockIdx.x * kBM;
-  const int n0 = blockIdx.y * BN;
-
-  if (tid == 0) {
-    mbar_init(bar_load, 1);
-    mbar_init(bar_mma, 1);
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  }
-  if (warp == 0) tmem_alloc(tmem_slot, kMaxBN);
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-  const uint32_t idesc = make_idesc(BN);
-  const int n_chunks = K / (kChunkAtoms * kAtomK);
-  const uint32_t chunk_bytes = kChunkAtoms * (kAtomBytesA + 2 * BN * 128);
-
-  for (int ch = 0; ch < n_chunks; ++ch) {
-    const uint32_t parity = ch & 1;
-    if (tid == 0) {
-      mbar_expect_tx(bar_load, chunk_bytes);
-      for (int a = 0; a < kChunkAtoms; ++a) {
-        int k0 = (ch * kChunkAtoms + a) * kAtomK;
-        tma_load_2d(sm + GemmSmem::a_hi + a * kAtomBytesA, &map_x, k0, (int)m0, bar_load);
-        tma_load_2d(sm + GemmSmem::b_hi + a * BN * 128, &map_whi, k0, n0, bar_load);
-        tma_load_2d(sm + GemmSmem::b_lo + a * BN * 128, &map_wlo, k0, n0, bar_load);
-      }
-    }
-    mbar_wait(bar_load, parity);
-    // split X: hi = nearest TF32 number, lo = exact remainder.  Element-wise, so the swizzle is irrelevant.
-    {
-      float4* hi = reinterpret_cast<float4*>(sm + GemmSmem::a_hi);
-      float4* lo = reinterpret_cast<float4*>(sm + GemmSmem::a_lo);
-      constexpr int n4 = kChunkAtoms * kAtomBytesA / 16;
-#pragma unroll 4
-      for (int i = tid; i < n4; i += kGemmThreads) {
-        float4 v = hi[i], h, l;
-        h.x = tf32_rn(v.x); l.x = v.x - h.x;
-        h.y = tf32_rn(v.y); l.y = v.y - h.y;
-        h.z = tf32_rn(v.z); l.z = v.z - h.z;
-        h.w = tf32_rn(v.w); l.w = v.w - h.w;
-        hi[i] = h;
-        lo[i] = l;
-      }
-    }
-    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // generic-proxy smem writes -> visible to the tensor core
-    tc_fence_before();
-    __syncthreads();
-    if (tid == 0) {
-      tc_fence_after();
-      const uint32_t ahi = smem_u32(sm + GemmSmem::a_hi), alo = smem_u32(sm + GemmSmem::a_lo);
-      const uint32_t bhi = smem_u32(sm + GemmSmem::b_hi), blo = smem_u32(sm + GemmSmem::b_lo);
-      uint32_t accum = ch > 0 ? 1u : 0u;
-#pragma unroll
-      for (int prod = 0; prod < 3; ++prod) {
-        const uint32_t abase = prod == 1 ? alo : ahi;
-        const uint32_t bbase = prod == 2 ? blo : bhi;
-        for (int a = 0; a < kChunkAtoms; ++a) {
-#pragma unroll
-          for (int k = 0; k < kAtomK / 8; ++k) {     // UMMA K = 8 tf32 = 32 bytes inside the 128-byte swizzle atom
-            uint64_t da = make_desc(abase + a * kAtomBytesA + k * 32);
-            uint64_t db = make_desc(bbase + a * BN * 128 + k * 32);
-            umma_tf32(tmem_base, da, db, idesc, accum);
+          for (int kk = 0; kk < kAtomK / 8; ++kk) {
+            Wgmma<BN>::ss(acc, make_desc(ab + kk * 32), make_desc(bb + kk * 32), accum);
             accum = 1u;
           }
         }
+        wg_commit();
+        wg_wait0();
+        fence_regs<BN / 2>(acc);
+        __syncwarp();
+        if (lane == 0) mbar_arrive(empty + s);          // this warpgroup's MMAs have finished reading the stage
       }
-      umma_commit(bar_mma);     // implies tcgen05.fence::before_thread_sync
+      if (++s == stages) { s = 0; ph ^= 1; }
     }
-    mbar_wait(bar_mma, parity);  // the MMAs have consumed this chunk's smem; accumulators (after the last chunk) are final
-    tc_fence_after();
-  }
 
-  // ---- epilogue: TMEM -> registers -> (+bias, relu, +residual) -> smem stage -> coalesced global stores
-  float* stage = reinterpret_cast<float*>(sm);                 // reuses the A buffers: 128 x 132 floats <= 96 KB
-  const int ldst = ((BN + 31) / 32) * 32 + 4;                  // tcgen05.ld works in 32-column groups
-  const int row = warp * 32 + lane;                            // TMEM lane == tile row
-  for (int c0 = 0; c0 < BN; c0 += 32) {
-    uint32_t r[32];
-    tmem_ld32(tmem_base + ((uint32_t)(warp * 32) << 16) + (uint32_t)c0, r);
+    // ===== epilogue: accumulator registers -> (+bias, ReLU, +residual [, LayerNorm]) -> global =====
+    const long long row[2] = {(long long)mt * kBM + frag_row, (long long)mt * kBM + frag_row + 8};
 #pragma unroll
-    for (int j = 0; j < 32; j += 4) {
-      float4 v = make_float4(__uint_as_float(r[j]), __uint_as_float(r[j + 1]), __uint_as_float(r[j + 2]), __uint_as_float(r[j + 3]));
-      *reinterpret_cast<float4*>(stage + row * ldst + c0 + j) = v;
-    }
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 0) tmem_dealloc(tmem_base, kMaxBN);
-  const int vec_per_row = BN / 4;
-  for (int i = tid; i < kBM * vec_per_row; i += kGemmThreads) {
-    int r_ = i / vec_per_row, c4 = (i - r_ * vec_per_row) * 4;
-    long long gr = m0 + r_;
-    int gc = n0 + c4;
-    if (gr >= M || gc >= N) continue;
-    float4 v = *reinterpret_cast<const float4*>(stage + r_ * ldst + c4);
-    float o[4] = {v.x, v.y, v.z, v.w};
+    for (int j = 0; j < BN / 8; ++j) {
+      const int gc = n0 + 8 * j + 2 * t;                // N is even: the column pair is in range or out of range together
+      const float b0 = (bias && gc < N) ? __ldg(bias + gc) : 0.f, b1 = (bias && gc < N) ? __ldg(bias + gc + 1) : 0.f;
 #pragma unroll
-    for (int j = 0; j < 4; ++j) {
-      if (gc + j < N) {
-        float t = o[j] + (bias ? __ldg(bias + gc + j) : 0.f);
-        if (relu) t = fmaxf(t, 0.f);
-        o[j] = t;
+      for (int h = 0; h < 2; ++h) {
+        float v0 = acc[4 * j + 2 * h] + b0, v1 = acc[4 * j + 2 * h + 1] + b1;
+        if (relu) { v0 = fmaxf(v0, 0.f); v1 = fmaxf(v1, 0.f); }
+        if (residual && row[h] < M && gc < N) {
+          const float2 rr = __ldg(reinterpret_cast<const float2*>(residual + row[h] * N + gc));
+          v0 += rr.x; v1 += rr.y;
+        }
+        acc[4 * j + 2 * h] = v0;
+        acc[4 * j + 2 * h + 1] = v1;
       }
     }
-    float* dst = y + gr * N + gc;
-    if (gc + 3 < N && ((reinterpret_cast<uintptr_t>(dst) & 15) == 0)) {
-      if (residual) {
-        float4 rr = __ldg(reinterpret_cast<const float4*>(residual + gr * N + gc));
-        o[0] += rr.x; o[1] += rr.y; o[2] += rr.z; o[3] += rr.w;
+    if (ln_gamma) {
+      // LayerNorm over the row (the launcher guarantees one n-tile: BN == N).  A row is spread over the 4 threads of a quad.
+      float mean[2], rstd[2];
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        float sum = 0.f;
+#pragma unroll
+        for (int j = 0; j < BN / 8; ++j) sum += acc[4 * j + 2 * h] + acc[4 * j + 2 * h + 1];
+        sum += __shfl_xor_sync(0xffffffffu, sum, 1);
+        sum += __shfl_xor_sync(0xffffffffu, sum, 2);
+        mean[h] = sum / (float)BN;
+        float sq = 0.f;
+#pragma unroll
+        for (int j = 0; j < BN / 8; ++j) {
+          const float d0 = acc[4 * j + 2 * h] - mean[h], d1 = acc[4 * j + 2 * h + 1] - mean[h];
+          sq = fmaf(d0, d0, sq);
+          sq = fmaf(d1, d1, sq);
+        }
+        sq += __shfl_xor_sync(0xffffffffu, sq, 1);
+        sq += __shfl_xor_sync(0xffffffffu, sq, 2);
+        rstd[h] = rsqrtf(sq / (float)BN + ln_eps);
       }
-      *reinterpret_cast<float4*>(dst) = make_float4(o[0], o[1], o[2], o[3]);
-    } else {
-      for (int j = 0; j < 4 && gc + j < N; ++j) dst[j] = o[j] + (residual ? __ldg(residual + gr * N + gc + j) : 0.f);
+#pragma unroll
+      for (int j = 0; j < BN / 8; ++j) {
+        const int c = 8 * j + 2 * t;
+        const float g0 = __ldg(ln_gamma + c), g1 = __ldg(ln_gamma + c + 1), e0 = __ldg(ln_beta + c), e1 = __ldg(ln_beta + c + 1);
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          acc[4 * j + 2 * h] = (acc[4 * j + 2 * h] - mean[h]) * rstd[h] * g0 + e0;
+          acc[4 * j + 2 * h + 1] = (acc[4 * j + 2 * h + 1] - mean[h]) * rstd[h] * g1 + e1;
+        }
+      }
+    }
+#pragma unroll
+    for (int j = 0; j < BN / 8; ++j) {
+      const int gc = n0 + 8 * j + 2 * t;
+      if (gc >= N) continue;
+#pragma unroll
+      for (int h = 0; h < 2; ++h)
+        if (row[h] < M) *reinterpret_cast<float2*>(y + row[h] * N + gc) = make_float2(acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1]);
     }
   }
 }
@@ -722,12 +324,17 @@ __global__ void split_tf32_kernel(const float* __restrict__ w, float* __restrict
   lo[i] = v - h;
 }
 
+template <int BN, bool kRegA>
+static int set_smem_attr() {
+  return check_cuda(cudaFuncSetAttribute(linear_3xtf32_kernel<BN, kRegA>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
+}
+
 }  // namespace so
 
 using namespace so;
 
 static bool g_linear_force_ss = false;
-// Test hook: 1 = both MMA operands from shared memory (the round-1 pipeline); 0 (default) = A operand in tensor memory.
+// Test hook: 1 = both MMA operands from shared memory; 0 (default) = A operand from registers.
 extern "C" int so_linear_force_ss(int on) { g_linear_force_ss = on != 0; return SO_OK; }
 
 extern "C" int so_split_tf32(const float* w, float* hi, float* lo, int64_t n, void* stream) {
@@ -748,7 +355,7 @@ extern "C" int so_linear_3xtf32(const float* x, const float* w_hi, const float* 
 }
 
 // y = LayerNorm(act(x w^T + bias) + residual) * gamma + beta over the N output columns, in the GEMM epilogue.
-// N must be a multiple of 32 and <= 128 (one n-tile holds the whole row); tensor-memory (TS) pipeline only.
+// N must be a multiple of 32 and <= 128 (one n-tile holds the whole row); register-A pipeline only.
 extern "C" int so_linear_3xtf32_ln(const float* x, const float* w_hi, const float* w_lo, const float* bias, const float* residual,
                                    const float* gamma, const float* beta, float eps, float* y, int64_t M, int32_t N, int32_t K,
                                    int32_t relu, void* stream) {
@@ -761,42 +368,53 @@ static int linear_impl(const float* x, const float* w_hi, const float* w_lo, con
                        int64_t M, int32_t N, int32_t K, int32_t relu, const float* ln_gamma, const float* ln_beta, float ln_eps,
                        void* stream) {
   if (!x || !w_hi || !w_lo || !y || M < 0 || N < 1 || K < 1) return SO_ERR_INVALID_ARG;
-  if (K % (kChunkAtoms * kAtomK) != 0 || K > 192) return SO_ERR_UNSUPPORTED;      // K = 96 or 192
+  if (K % 96 != 0 || K > 192) return SO_ERR_UNSUPPORTED;                         // K = 96 or 192
   if ((reinterpret_cast<uintptr_t>(x) | reinterpret_cast<uintptr_t>(w_hi) | reinterpret_cast<uintptr_t>(w_lo)) & 15)
     return SO_ERR_INVALID_ARG;                                                    // TMA needs 16-byte aligned bases
   if (M == 0) return SO_OK;
   if (M > 0x7fffffffLL) return SO_ERR_UNSUPPORTED;
-  const bool ts = !g_linear_force_ss;
-  PipeCfg cfg = ts ? make_pipe_cfg_ts(N, K) : make_pipe_cfg(N, K);
+  // the epilogue stores Y and reads the residual as column pairs (float2)
+  if ((reinterpret_cast<uintptr_t>(y) & 7) || (reinterpret_cast<uintptr_t>(residual) & 7) || (N % 2)) return SO_ERR_UNSUPPORTED;
+  const bool reg_a = !g_linear_force_ss;
+  PipeCfg cfg = make_pipe_cfg(N, K, reg_a);
   if (cfg.stages < 2) return SO_ERR_UNSUPPORTED;
+  if (ln_gamma && cfg.BN != N) return SO_ERR_UNSUPPORTED;
   CUtensorMap mx, mhi, mlo;
   int rc;
   if ((rc = make_tmap(&mx, x, M, K, kBM))) return rc;
   if ((rc = make_tmap(&mhi, w_hi, N, K, cfg.BN))) return rc;
   if ((rc = make_tmap(&mlo, w_lo, N, K, cfg.BN))) return rc;
-  if ((reinterpret_cast<uintptr_t>(y) & 15) || (N % 4)) return SO_ERR_UNSUPPORTED;   // TMA store: 16-byte aligned rows
-  CUtensorMap my;
-  if ((rc = make_tmap(&my, y, M, N, 32))) return rc;                                 // store box: 32 rows x 32 floats
   static PerDeviceOnce smem_attr;
   if ((rc = smem_attr.run([] {
-         int r = check_cuda(cudaFuncSetAttribute(linear_3xtf32_pipe_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
-         if (r) return r;
-         return check_cuda(cudaFuncSetAttribute(linear_3xtf32_ts_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
+         int r;
+         if ((r = set_smem_attr<32, true>()) || (r = set_smem_attr<64, true>()) || (r = set_smem_attr<96, true>()) ||
+             (r = set_smem_attr<128, true>()) || (r = set_smem_attr<32, false>()) || (r = set_smem_attr<64, false>()) ||
+             (r = set_smem_attr<96, false>()) || (r = set_smem_attr<128, false>()))
+           return r;
+         return SO_OK;
        })))
     return rc;
   cudaStream_t st = (cudaStream_t)stream;
   const int n_tiles = (int)ceil_div64(N, cfg.BN), m_tiles = (int)ceil_div64(M, kBM);
-  int groups = kNumSMs / n_tiles;
+  int groups = num_sms() / n_tiles;
   if (groups < 1) groups = 1;
   if (groups > m_tiles) groups = m_tiles;
   ProfScope prof(8, st);
-  if (ts)
-    linear_3xtf32_ts_kernel<<<n_tiles * groups, kPipeThreads, cfg.smem, st>>>(mx, mhi, mlo, my, bias, residual, (long long)M, N, cfg.BN,
-                                                                            cfg.KA, cfg.stages, n_tiles, m_tiles, relu, cfg.epi_bufs,
-                                                                            ln_gamma, ln_beta, ln_eps);
-  else
-    linear_3xtf32_pipe_kernel<<<n_tiles * groups, kPipeThreads, cfg.smem, st>>>(mx, mhi, mlo, my, bias, residual, (long long)M, N, cfg.BN,
-                                                                              cfg.KA, cfg.stages, n_tiles, m_tiles, relu, cfg.epi_bufs);
+#define SO_GEMM(BN_, REGA)                                                                                                     \
+  linear_3xtf32_kernel<BN_, REGA><<<n_tiles * groups, kGemmThreads, cfg.smem, st>>>(mx, mhi, mlo, bias, residual, y, (long long)M, \
+                                                                                   N, cfg.KA, cfg.stages, n_tiles, m_tiles, relu,  \
+                                                                                   ln_gamma, ln_beta, ln_eps)
+  switch (cfg.BN * 2 + (reg_a ? 1 : 0)) {
+    case 32 * 2 + 1: SO_GEMM(32, true); break;
+    case 64 * 2 + 1: SO_GEMM(64, true); break;
+    case 96 * 2 + 1: SO_GEMM(96, true); break;
+    case 128 * 2 + 1: SO_GEMM(128, true); break;
+    case 32 * 2: SO_GEMM(32, false); break;
+    case 64 * 2: SO_GEMM(64, false); break;
+    case 96 * 2: SO_GEMM(96, false); break;
+    default: SO_GEMM(128, false); break;
+  }
+#undef SO_GEMM
   note_launch(1);
   return check_launch();
 }

@@ -3,21 +3,25 @@
 // Thread mapping of every sampling kernel: one "item" = one (query, head); DH/4 lanes own an item and
 // each lane owns 4 consecutive channels (one float4) of the head, so a bilinear corner is one coalesced
 // 64-byte (DH=16) read per item and the (query, head*DH) output row is written as float4, 512 B per warp.
-// Value tensors are 30-65 MB fp32, i.e. L2-resident on B200 (126 MB): these kernels are L2/L1-gather
+// Value tensors are 30-65 MB fp32, i.e. largely L2-resident on H100 (50 MB): these kernels are L2/L1-gather
 // bound, not HBM bound.
 #include "common.cuh"
 #include <math.h>
+// Tuning knobs, timed on an H100 SXM (700 W) over the bench frame with `bench.py`'s per-kernel breakdown, ms per step.
+// Cross-attention: 4.63-4.66 at the defaults (two runs); unroll 2 / 8: 4.65 / 4.63; 4 / 6 CTAs per SM: 4.66 / 4.63.
+// Self-attention: 1.66-1.67 at the defaults; unroll 4: 1.66; 3 / 5 CTAs per SM: 1.67 / 1.67.  Every alternative is
+// within the run-to-run spread, so the defaults stay.
 #ifndef SO_ATTN_UNROLL
-#define SO_ATTN_UNROLL 4         // cross-attention: 4.66 / 4.72 / 4.74 ms per step for unroll 4 / 2 / 8
+#define SO_ATTN_UNROLL 4
 #endif
 #ifndef SO_SELF_ATTN_MIN_CTAS
-#define SO_SELF_ATTN_MIN_CTAS 4  // 64 registers, no spills: 1.55 ms vs 1.64 ms at 5 CTAs (cross-attention is equal at 4 and 5)
+#define SO_SELF_ATTN_MIN_CTAS 4
 #endif
 #ifndef SO_SELF_ATTN_UNROLL
-#define SO_SELF_ATTN_UNROLL 8    // self-attention: 1.65 / 1.70 / 1.77 ms per step for unroll 8 / 4 / 2
+#define SO_SELF_ATTN_UNROLL 8
 #endif
 #ifndef SO_ATTN_MIN_CTAS
-#define SO_ATTN_MIN_CTAS 5     // 48 registers; 6 (40 registers) spills more and measured slower
+#define SO_ATTN_MIN_CTAS 5
 #endif
 
 namespace so {
@@ -308,7 +312,7 @@ __global__ void __launch_bounds__(256, SO_SELF_ATTN_MIN_CTAS) tpv_self_attn_kern
 // v2 of the two fused attention cores: the per-sample set-up is computed ONCE per (query, head, sample) instead of once
 // per lane.  In the kernels above the DH/4 lanes of an item each redo the whole set-up of every sample (location
 // arithmetic, floor, bounds, 4 bilinear weights, softmax weight: ~70 of the ~116 instructions per sample, plus three
-// parameter loads and spill traffic under the register cap; ncu r1: l1tex 83 %, issue 65 %).  Here the LANES lanes of an
+// parameter loads and spill traffic under the register cap).  Here the LANES lanes of an
 // item set up LANES DIFFERENT samples of a round (lane j: point d0 + j), park the result -- 4 corner weights already
 // multiplied by the attention weight and by the zero-padding mask, and the 4 (clamped, always in-bounds) absolute pixel
 // indices -- in 32 bytes of shared memory, and then each 4-lane sub-group walks over its 4 samples of the round reading
@@ -318,8 +322,7 @@ __global__ void __launch_bounds__(256, SO_SELF_ATTN_MIN_CTAS) tpv_self_attn_kern
 struct SamplePark { float w[4]; int p[4]; };     // 32 B: parked as one float4 + one int4 in two shared arrays
 // Slot layout inside a warp's 32 entries (conflict-free on both sides): the lane L = 4 g + j that sets sample j of sub-group
 // g up writes slot j * 8 + g; at step j the 8 sub-groups read slots j * 8 + 0..7 = 128 contiguous bytes (one wavefront; the
-// first version parked array-of-structs at a 128-byte stride between sub-groups: 8-way bank conflicts, ncu counted more
-// shared-memory wavefronts than global ones, profiles/r2_attn2_ncu.txt).
+// first version parked array-of-structs at a 128-byte stride between sub-groups: 8-way bank conflicts).
 __device__ __forceinline__ int park_write_slot(int lane) { return (lane & 3) * 8 + (lane >> 2); }
 __device__ __forceinline__ int park_read_slot(int lane, int j) { return j * 8 + (lane >> 2); }
 

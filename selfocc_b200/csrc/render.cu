@@ -8,7 +8,8 @@
 // recurrence is kept in registers in the reference's order (exclusive cumprod, first-max argmax).
 #include "render_common.cuh"
 #ifndef SO_RENDER_UNROLL
-#define SO_RENDER_UNROLL 1     // measured 10.20 / 10.56 / 10.44 ms for unroll 1 / 2 / 4 at 8.64 M rays
+// H100 SXM (700 W), 8.64 M rays, depth-only / colour ms: unroll 1 11.9 / 28.5, unroll 2 10.7 / 29.9, unroll 4 10.8 / 28.9
+#define SO_RENDER_UNROLL 4
 #endif
 #ifndef SO_RENDER_BLOCK
 #define SO_RENDER_BLOCK 128
@@ -46,7 +47,7 @@ __global__ void __launch_bounds__(256) bounds_kernel(RayDev R, RenderDev P, floa
     chunk = R.chunk_len > 0 ? gid / R.chunk_len : 0;
   }
   // aggregate per warp, then per CTA, when everybody sits in one chunk (the common case): ONE atomic pair per CTA.
-  // (One pair per warp -- 270 k same-address atomics for 8.64 M rays -- made this pre-pass 165 us, ncu r2_launches.)
+  // (One pair per warp means ~270 k same-address atomics for 8.64 M rays, which serialise in L2.)
   unsigned full = __activemask();
   long long c0 = __shfl_sync(full, chunk, 0);
   bool uniform = __all_sync(full, (!ok) || chunk == c0);

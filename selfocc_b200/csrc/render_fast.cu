@@ -6,8 +6,8 @@
 //      n_feat == 0 : float2 [H][W][zpitch]  {sdf[z], sdf[z+1]}     -> the 8 trilinear taps are 4 aligned 64-bit loads
 //      n_feat == 3 : float4 [H][W][Z]       {r, g, b, sdf}          -> 8 aligned 128-bit loads fetch sdf AND colour
 //    (the reference gathers 8 + 24 scalars per sample for colour, bev_nerf.py:99-117);
-//  * the trilinear interpolation runs on Blackwell's packed fp32 pipe (fma.rn.f32x2 / add.rn.f32x2 -> FFMA2 / FADD2):
-//    the two lanes of a loaded register pair are lerped together, the sdf gradient falls out of the lerp differences;
+//  * the trilinear interpolation works on register pairs: the two lanes of a loaded pair are lerped together, the sdf
+//    gradient falls out of the lerp differences;
 //  * "all 8 corners inside the volume" is decided ONCE per ray: for the affine metre->grid map g(t) = g0 + gd * t is
 //    monotone along the ray (so is its fp32 evaluation fma(gd, t, g0)), so if the first and the last sample are interior,
 //    every sample is; warps with a non-interior ray take the general zero-padding loop;
@@ -18,6 +18,9 @@
 //    < 1e-9 relative and cannot hold the max-depth argmax (a later w is <= T < 1e-9 <= max_s w_s since sum_s w_s >= 1 - T).
 #include "render_common.cuh"
 
+// Tuning knobs, timed on an H100 SXM (400 W) with scripts/bench_render.py, analytic scene, 8.64 M rays, depth-only / colour
+// ms: defaults (unroll 4; 6 / 4 CTAs per SM) 6.93-7.18 / 12.06-12.12 over two runs; unroll 1 7.27 / 12.08, unroll 2
+// 7.04 / 12.18; 4 / 3 CTAs 6.98 / 12.14; 8 / 5 CTAs 6.92 / 12.12.  No alternative beats the run-to-run spread.
 #ifndef SO_RF_BLOCK
 #define SO_RF_BLOCK 128
 #endif
@@ -28,7 +31,7 @@
 #define SO_RF_MIN_CTAS_RGB 4
 #endif
 #ifndef SO_RF_UNROLL
-#define SO_RF_UNROLL 4      // measured (render ms, colour / depth-only): unroll 1 11.22 / 6.93, 2 11.01 / 6.94, 4 10.97 / 6.82
+#define SO_RF_UNROLL 4
 #endif
 #ifndef SO_RF_EXIT_T
 #define SO_RF_EXIT_T 1e-9f
@@ -55,8 +58,11 @@ struct RayGeo {        // per-ray constants of the affine march (grid units)
 
 __device__ __forceinline__ float2 f2(float a, float b) { return make_float2(a, b); }
 __device__ __forceinline__ float2 bc2(float a) { return make_float2(a, a); }
-__device__ __forceinline__ float2 sub2(float2 a, float2 b) { return __ffma2_rn(b, make_float2(-1.f, -1.f), a); }   // a - b, exact
-__device__ __forceinline__ float2 lerp2(float2 t, float2 d, float2 a) { return __ffma2_rn(t, d, a); }               // a + t * d
+// two-lane helpers: one rounded fmaf / add per lane (sm_90 has no packed fp32x2 pipe; the results are the same)
+__device__ __forceinline__ float2 fma2(float2 a, float2 b, float2 c) { return make_float2(fmaf(a.x, b.x, c.x), fmaf(a.y, b.y, c.y)); }
+__device__ __forceinline__ float2 add2(float2 a, float2 b) { return make_float2(a.x + b.x, a.y + b.y); }
+__device__ __forceinline__ float2 sub2(float2 a, float2 b) { return fma2(b, make_float2(-1.f, -1.f), a); }   // a - b, exact
+__device__ __forceinline__ float2 lerp2(float2 t, float2 d, float2 a) { return fma2(t, d, a); }               // a + t * d
 
 // NeuS alpha, one-reciprocal form (see the file header).  s2 = sdf * inv_s * log2(e), h2 = half * inv_s * log2(e) <= 0.
 // The exponents are clamped at 64: beyond that alpha is 1 (A huge) or the 1e-5 floor (B huge) to within 2^-40.
@@ -175,16 +181,16 @@ render_packed_kernel(VolumeDev V, const void* __restrict__ pack, RayDev R, Rende
     constexpr int kUnroll = SO_RF_UNROLL;
 #pragma unroll kUnroll
     for (int s = 0; s < S; ++s) {
-      const float2 mid2 = __ffma2_rn(bm2, span2, tn2);
-      bm2 = __fadd2_rn(bm2, step2);
+      const float2 mid2 = fma2(bm2, span2, tn2);
+      bm2 = add2(bm2, step2);
       const float mid = mid2.x;
-      const float2 ghw = __ffma2_rn(gdhw, mid2, ghw0);
+      const float2 ghw = fma2(gdhw, mid2, ghw0);
       const float gd = fmaf(G.gdd, mid, G.gd0);
       if (DBG) { dbg_ray[3 * s] = ghw.x; dbg_ray[3 * s + 1] = ghw.y; dbg_ray[3 * s + 2] = gd; }
       const float flh = floorf(ghw.x), flw = floorf(ghw.y), flz = floorf(gd);
       const float2 fhw = sub2(ghw, f2(flh, flw));
       const float fz = gd - flz;
-      const float2 rhw = __fadd2_rn(f2(flh, flw), magic2);
+      const float2 rhw = add2(f2(flh, flw), magic2);
       const float rz = flz + kMagic;
       const unsigned idx = __float_as_uint(rhw.x) * wz + (__float_as_uint(rhw.y) * zp + (__float_as_uint(rz) + kcorr));
       const float2 fh2 = bc2(fhw.x), fw2 = bc2(fhw.y);
@@ -239,7 +245,7 @@ render_packed_kernel(VolumeDev V, const void* __restrict__ pack, RayDev R, Rende
       composite(a, alpha, mid, dgw * G.kw, dgh * G.kh, dgd * G.kd, s, w);
       if (RGB) {
         // SH degree 0, relu activation (sh_render.py:84-94); the launcher routes sh_act != 0 to the general kernel
-        const float2 c2 = __ffma2_rn(rg, bc2(kC0), bc2(0.5f));
+        const float2 c2 = fma2(rg, bc2(kC0), bc2(0.5f));
         const float r0 = fmaxf(c2.x, 0.f), r1 = fmaxf(c2.y, 0.f), r2 = fmaxf(fmaf(bl, kC0, 0.5f), 0.f);
         a.c_r = fmaf(w, r0, a.c_r); a.c_g = fmaf(w, r1, a.c_g); a.c_b = fmaf(w, r2, a.c_b);
       }

@@ -8,7 +8,7 @@
 // 32-sample chunk + a carried prefix); the backward needs the matching suffix sums and runs the chunks in reverse.
 #include "render_common.cuh"
 #ifndef SO_TRAIN_FWD_MIN_CTAS
-#define SO_TRAIN_FWD_MIN_CTAS 8   // 64 registers: 0.122 ms vs 0.153 ms at 4 CTAs/SM (cfg-5 sizes); the kernel is latency-bound
+#define SO_TRAIN_FWD_MIN_CTAS 8   // H100 SXM (700 W), cfg-5 sizes, Cf = 25: 0.664-0.668 ms, 4 CTAs/SM the same; latency-bound
 #endif
 
 #ifndef SO_TRAIN_FWD24_MIN_CTAS
@@ -133,8 +133,7 @@ __device__ __forceinline__ void sample_colour(const VolumeDev& V, const RenderDe
 // SEM template parameter of the one-ray-per-warp kernels: 0 = no semantics, 1 = any channel count (runtime loops over
 // scalar gathers), 24 = exactly 24 feature channels with feat_pitch 24: a voxel's 96 bytes are read / accumulated as six
 // float4 (48 LDG.128 instead of 192 LDG.32 per sample; 48 128-bit reductions instead of 192 atomics in the backward) and every
-// per-class array has a compile-time size, so nothing lives in local memory (the runtime-count arrays of SEM = 1 spill:
-// 115-152 LDL/STL per sample, profiles/r1_sass_loop_mix.txt).
+// per-class array has a compile-time size, so nothing lives in local memory (runtime-count arrays spill to local memory).
 constexpr int kSem24 = 21;
 
 __device__ __forceinline__ void gather_feat24(const VolumeDev& v, const Taps& t, float out[24]) {
@@ -344,7 +343,7 @@ __global__ void __launch_bounds__(128, SEM == 24 ? SO_TRAIN_FWD24_MIN_CTAS : SO_
 // ---- forward, batched rays + U chunks in flight + z-pair volume ---------------------------------------------------
 // Same contract and the same per-sample arithmetic as render_train_fwd_kernel<., false, true> (lane = sample, so the 32
 // lanes of a load touch neighbouring voxels: the gathers are bound by distinct 128-byte lines per L1 request), with the
-// three things ncu showed that kernel to lack:
+// three things that kernel lacks:
 //  (a) a warp takes a BATCH of consecutive rays: lane b computes ray b's set-up (camera ray, slab test, affine
 //      grid-space ray: ~300 instructions the one-ray-per-warp kernel repeats in all 32 lanes) and, after the batch, its
 //      tail (depth clip, divisions, per-ray stores); the 12 per-ray constants are broadcast with shuffles;
@@ -356,7 +355,7 @@ __global__ void __launch_bounds__(128, SEM == 24 ? SO_TRAIN_FWD24_MIN_CTAS : SO_
 // fma(w_i, u_i, max(i - 1/2, 0)) * step with w_i = 1 (1/2 at the two ends); for power-of-two S this is the same
 // fp32 value as the one-ray-per-warp kernel's.
 #ifndef SO_TRAIN_FWD5_U
-#define SO_TRAIN_FWD5_U 4            // measured (cfg-5 sizes, us): U=1 137, U=2 119, U=4 109 -- the kernel is latency-bound
+#define SO_TRAIN_FWD5_U 4            // H100 SXM (700 W), cfg-5 sizes, Cf = 1, ms: U=2 0.129, U=4 0.125, U=8 0.160 (latency-bound)
 #endif
 #ifndef SO_TRAIN_FWD5_PREFETCH
 #define SO_TRAIN_FWD5_PREFETCH 1     // 1 / 2: prefetch.global.L2 / .L1 of the batch's jitter rows before the ray set-up (109 -> 101 us)
@@ -868,9 +867,10 @@ extern "C" int so_render_train_forward(const float* vol_sdf, const float* vol_fe
   RenderDev P = make_render_dev(*pr, jitter);
   if ((rc = launch_depth_bounds(R, P, workspace, st))) return rc;
   TrainOut O{depth, acc, fars, rgb, sem, max_depth, weights, ts, deltas, eik_grad, sample_sdf};
-  // persistent-style grid: warps stride over rays; 4 warps per CTA, enough CTAs to fill 148 SMs several times over
+  // persistent-style grid: warps stride over rays; 4 warps per CTA, enough CTAs to fill 132 SMs several times over
   long long ctas = ceil_div64(R.ray_count, 4);
-  unsigned grid = (unsigned)(ctas < (long long)kNumSMs * 16 ? ctas : (long long)kNumSMs * 16);
+  const long long cap = (long long)num_sms() * 16;
+  unsigned grid = (unsigned)(ctas < cap ? ctas : cap);
   ProfScope prof(6, st);
   const bool fast = V.ax[0].k1 == 0.f && V.ax[1].k1 == 0.f && V.ax[2].k1 == 0.f && (P.S & (P.S - 1)) == 0 && P.S >= 32 &&
                     P.cos_anneal == 1.0f && P.anchor_mid;
@@ -926,7 +926,8 @@ extern "C" int so_render_train_backward(const float* vol_sdf, const float* vol_f
   if ((rc = launch_depth_bounds(R, P, workspace, st))) return rc;
   TrainGrad G{g_depth, g_acc, g_rgb, g_sem, g_weights, g_eik, g_sdf, g_vol_sdf, g_vol_feat, g_inv_s};
   long long ctas = ceil_div64(R.ray_count, 4);
-  unsigned grid = (unsigned)(ctas < (long long)kNumSMs * 16 ? ctas : (long long)kNumSMs * 16);
+  const long long cap = (long long)num_sms() * 16;
+  unsigned grid = (unsigned)(ctas < cap ? ctas : cap);
   ProfScope prof(7, st);
   const bool sem24 = V.n_feat == 24 && V.feat_pitch == 24 && (want_rgb || want_sem) && !g_force_sem_generic &&
                      ((reinterpret_cast<uintptr_t>(vol_feat) | reinterpret_cast<uintptr_t>(g_vol_feat)) & 15) == 0;

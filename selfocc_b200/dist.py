@@ -40,7 +40,7 @@ def all_gather_rays(local, total, group=None):
 def all_gather_planar(tensors, total, group=None):
     """Several per-ray tensors of this rank ([count] or [count, k], same count) -> their full versions ([total, ...]) with ONE
     collective: the payload is packed PLANAR (tensor after tensor, each padded to the common per-rank length -- contiguous
-    copies; an interleaved [count, sum k] pack costs a strided write of every column, ~1 ms for 8.64 M rays x 6 floats)."""
+    copies; an interleaved [count, sum k] pack would cost a strided write of every column)."""
     if not dist.is_available() or not dist.is_initialized() or dist.get_world_size(group) == 1:
         return list(tensors)
     world = dist.get_world_size(group)
@@ -311,9 +311,9 @@ def frame_sharded(model, ms_img_feats, metas, lifter=None, group=None, batch=0):
 
 
 class GraphedFrame:
-    """frame_sharded captured ONCE into a CUDA graph per rank (kernels + the NCCL all_gathers) and replayed per frame: at 8
-    ranks a sharded frame is ~4 ms of GPU work behind ~110 python-issued launches and 7 collectives, i.e. host-bound when run
-    eagerly.  Inputs are static device buffers (copy the frame's FPN features / camera matrices into ``feats`` / ``metas``'
+    """frame_sharded captured ONCE into a CUDA graph per rank (kernels + the NCCL all_gathers) and replayed per frame: at high
+    rank counts a sharded frame is a few ms of GPU work per rank behind ~110 python-issued launches and 7 collectives, i.e.
+    host-bound when run eagerly.  Inputs are static device buffers (copy the frame's FPN features / camera matrices into ``feats`` / ``metas``'
     tensors before ``replay()``); outputs are the static tensors ``self.out``.  ``metas`` must hold DEVICE tensors (a numpy
     matrix list would be uploaded from pageable memory inside the capture).
     STATUS: validated at world size 1 (tests/test_gpu_dist.py, bit-identical to eager).  With torch.distributed's NCCL

@@ -8,7 +8,7 @@ The arithmetic of the hot ops runs in ``libselfocc_b200.so``:
   bilinear gather + head sum (+ camera loop / visible-count average for the image cross-attention),
   no ``nonzero()`` host sync, no padded per-camera rebatch (``ops.tpv_self_attn_forward*`` /
   ``ops.tpv_cross_attn_forward*``); every dense projection (value / offset / weight / output Linear, FFN) runs on
-  the tcgen05 split-precision GEMM (``ops.linear_3xtf32``, fp32-level accuracy), projections of the same input are
+  the wgmma split-precision GEMM (``ops.linear_3xtf32``, fp32-level accuracy), projections of the same input are
   fused into one GEMM; LayerNorm is a warp-per-row kernel (``ops.layer_norm``);
 * training (autograd): the mmcv-contract op ``ops.MultiScaleDeformableAttnFunction`` (forward +
   backward kernels) fed by torch softmax / location arithmetic, visible-query lists compacted on the
@@ -138,7 +138,7 @@ class _DeformBase(nn.Module):
 
 
 def fast_linear(lin, x, relu=False, residual=None, out=None, ln=None):
-    """nn.Linear forward for the inference path: the tcgen05 split-precision GEMM (``so_linear_3xtf32``) when the shape
+    """nn.Linear forward for the inference path: the wgmma split-precision GEMM (``so_linear_3xtf32``) when the shape
     allows it (K % 96 == 0), cuBLAS otherwise.  Split weights are cached per parameter version.
     ``ln``: an nn.LayerNorm applied to the result; folded into the GEMM epilogue when the row fits one tile
     (``so_linear_3xtf32_ln``), a separate ``so_layer_norm`` launch otherwise."""
@@ -186,7 +186,7 @@ def _fast_linear_impl(lin, x, relu, residual, out, ln):
 
 
 def train_linear(lin, x):
-    """nn.Linear inside the autograd (training) path: forward and input gradient on the tcgen05 3xTF32 GEMM
+    """nn.Linear inside the autograd (training) path: forward and input gradient on the wgmma 3xTF32 GEMM
     (ops.TCLinearFunction) when the shape allows it; SELFOCC_B200_TRAIN_LINEAR=cublas keeps the stock nn.Linear."""
     w = lin.weight
     if x.is_cuda and x.dtype == torch.float32 and w.dtype == torch.float32 and x.numel() > 0 \
@@ -201,7 +201,7 @@ def _train_linear_off():
 
 
 def fast_linear_cat(owner, key, lins, x):
-    """Several nn.Linear layers applied to the SAME input as one tcgen05 GEMM (weights concatenated along N, cached on
+    """Several nn.Linear layers applied to the SAME input as one wgmma GEMM (weights concatenated along N, cached on
     ``owner``).  Returns the [M, sum(N_i)] result and the column slices (views, unit column stride) of each layer."""
     ver = tuple((l.weight._version, l.weight.data_ptr(), l.bias._version, l.bias.data_ptr()) for l in lins)
     ent = getattr(owner, key, None)

@@ -2,7 +2,7 @@
 
 The reference head is an adapter over the un-vendored sdfstudio fork; here the same public surface
 (``prepare`` / ``render`` / ``forward_occ`` / ``forward``, constructor kwargs, output dict keys) drives
-the fused sm_100a kernels.  Fork-only knobs whose semantics cannot be recovered from the reference
+the fused sm_90a kernels.  Fork-only knobs whose semantics cannot be recovered from the reference
 (SURVEY.md 8c) are rejected when set to a non-default value instead of being silently ignored.
 """
 import math

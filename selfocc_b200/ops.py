@@ -381,8 +381,8 @@ class FieldSecondGradFunction(torch.autograd.Function):
 
 
 class TPVDecodeFunction(torch.autograd.Function):
-    """Decode with the fused sm_100a forward.  Backward (training only) recomputes the MLP slab by slab -- bounded memory,
-    never the reference's 750 MB intermediate.  Default: the native slab backward (_backward_native: tcgen05 3xTF32 GEMMs
+    """Decode with the fused sm_90a forward.  Backward (training only) recomputes the MLP slab by slab -- bounded memory,
+    never the reference's 750 MB intermediate.  Default: the native slab backward (_backward_native: wgmma 3xTF32 GEMMs
     + the fused element-wise kernels so_tpv_decode_bwd_*); SELFOCC_B200_DECODE_BWD=torch or an unsupported channel count
     takes the torch/cuBLAS autograd restatement of the same slab (_backward_torch), which is also what the tests compare
     the native path with."""
@@ -492,7 +492,7 @@ def linear_ln_supported(N, K):
 
 
 def linear_3xtf32(x, w_hi, w_lo, bias=None, relu=False, residual=None, out=None, ln=None):
-    """y = act(x @ w^T + bias) (+ residual) on tcgen05 tensor cores with fp32-level accuracy.  x [..., K] contiguous.
+    """y = act(x @ w^T + bias) (+ residual) on the Hopper tensor cores (wgmma) with fp32-level accuracy.  x [..., K] contiguous.
     ``out``: optional pre-allocated contiguous [..., N] destination (e.g. a row range of a larger token buffer).
     ``ln`` = (gamma, beta, eps): LayerNorm over the N outputs folded into the epilogue (so_linear_3xtf32_ln)."""
     lib = _lib.load()
@@ -519,13 +519,13 @@ def linear_3xtf32(x, w_hi, w_lo, bias=None, relu=False, residual=None, out=None,
 
 
 def linear_supported(K, N=None):
-    """Shapes so_linear_3xtf32 accepts (gemm.cu): K = 96 or 192, N a multiple of 4 (16-byte TMA store rows).  Anything
+    """Shapes so_linear_3xtf32 accepts (gemm.cu): K = 96 or 192, N even (the epilogue stores column pairs).  Anything
     else takes cuBLAS in the callers instead of raising SO_ERR_UNSUPPORTED."""
-    return K in (96, 192) and (N is None or N % 4 == 0)
+    return K in (96, 192) and (N is None or N % 2 == 0)
 
 
 class TCLinearFunction(torch.autograd.Function):
-    """nn.Linear for the TRAINING path of the lifting encoder: y = x w^T + b and dL/dx = dL/dy w on the tcgen05 3xTF32 GEMM
+    """nn.Linear for the TRAINING path of the lifting encoder: y = x w^T + b and dL/dx = dL/dy w on the wgmma 3xTF32 GEMM
     (fp32-level accuracy, so the step stays an fp32 step: mmcv's Linear layers run cuBLAS fp32 SIMT kernels there); the
     weight gradient is a reduction over the 10^5 token rows (dL/dy^T x, K = rows), which so_linear_3xtf32's tiling does not
     cover, and stays on cuBLAS.  When the contraction of dL/dx (the layer's out_features) is not 96 / 192 it takes cuBLAS too."""

@@ -2,7 +2,7 @@
 frame k's result overlap the compute of the neighbouring frames (two device input buffers, two side streams).
 
 The reference feeds one frame per iteration from a DataLoader with ``pin_memory`` and copies results back with
-``.cpu()`` on the compute stream (eval_depth.py:150-190); on a B200 those copies are ~10 % of a 20 ms frame, so the
+``.cpu()`` on the compute stream (eval_depth.py:150-190); serial copies add their full PCIe time to every frame, so the
 evaluation loop is written as a 3-stage pipeline instead.  Plumbing only: streams, events, pinned copies."""
 import torch
 

@@ -1,7 +1,7 @@
 """Generate golden vectors from the importable pure-torch pieces of the reference.
 
-Run ONCE in the build container (``/root/reference`` is absent on the GPU box):
-    python tests/golden/make_golden.py
+Run once, on a machine with a checkout of huang-yh/SelfOcc (the tests only read the stored vectors):
+    python tests/golden/make_golden.py <path to the SelfOcc checkout>
 Writes ``tests/golden/reference_golden.npz``.  Only reference modules that import without
 mmcv/mmengine/nerfstudio are used (SURVEY.md section 8c); they are loaded by file path and
 executed unmodified.  Inputs are seeded and stored beside the outputs.
@@ -12,7 +12,7 @@ import sys
 import numpy as np
 import torch
 
-REF = '/root/reference'
+REF = next((a for a in sys.argv[1:] if not a.startswith('--')), None)   # the SelfOcc checkout (required)
 HERE = os.path.dirname(os.path.abspath(__file__))
 
 
@@ -128,7 +128,7 @@ def main():
 def dump_reference_model_configs():
     """The lifter / encoder / head config dicts of every shipped TPV experiment config, as the reference's own config
     files define them (plain `exec` of config/<set>/<name>.py: they are self-contained python apart from `_base_`).
-    Written to tests/golden/reference_model_cfgs.json; tests/test_modules_cpu.py builds the B200 modules from them."""
+    Written to tests/golden/reference_model_cfgs.json; tests/test_modules_cpu.py builds the H100 modules from them."""
     import glob
     import json
     out = {}
@@ -223,6 +223,9 @@ def json_dumps(o):
     import json
     return json.dumps(o, sort_keys=True)
 
+
+if __name__ == '__main__' and (REF is None or not os.path.isfile(os.path.join(REF, 'model', 'head', 'nerfacc_head', 'bev_nerf.py'))):
+    sys.exit('usage: python tests/golden/make_golden.py <path to a huang-yh/SelfOcc checkout> [--bevnerf]')
 
 if __name__ == '__main__' and '--bevnerf' in sys.argv:
     bevnerf_golden()

@@ -29,12 +29,12 @@ def test_library_exports_every_declared_symbol():
     assert lib.so_error_string(-1) == b'invalid argument'
 
 
-def test_sm100a_only():
+def test_sm90a_only():
     from selfocc_b200 import _lib, build
     build.build()
     out = subprocess.run(['cuobjdump', '--list-elf', _lib.LIB_PATH], capture_output=True, text=True).stdout
     archs = set(re.findall(r'sm_\d+a?', out))
-    assert archs == {'sm_100a'}, archs
+    assert archs == {'sm_90a'}, archs
 
 
 def test_ops_refuse_cpu_tensors():

@@ -1,6 +1,6 @@
 """GPU: strong-scaling path (selfocc_b200/dist.py).  Single-GPU tests emulate the ranks one after the other (every kernel
 is row-independent, so the sharded result must be BIT-IDENTICAL to the unsharded encoder / decode / render); the torchrun
-test runs the real NCCL path when the box has >= 2 GPUs (`gpurun --gpus N`)."""
+test runs the real NCCL path when the machine has >= 2 GPUs and skips otherwise."""
 import os
 import subprocess
 import sys
@@ -93,9 +93,9 @@ dist.destroy_process_group()
 
 
 def test_frame_sharded_and_lattice_sharded_over_nccl(tmp_path):
-    """BASELINE configs[3] ("4 x B200 ray-sharded") / configs[4]: the real collectives.  Needs >= 2 GPUs."""
+    """BASELINE configs[3] (4-GPU ray-sharded) / configs[4]: the real collectives.  Needs >= 2 GPUs."""
     if not torch.cuda.is_available() or torch.cuda.device_count() < 2:
-        pytest.skip('needs >= 2 GPUs (run under `gpurun --gpus N`)')
+        pytest.skip('needs >= 2 GPUs')
     n = 4 if torch.cuda.device_count() >= 4 else 2
     script = tmp_path / 'worker.py'
     script.write_text(WORKER % (ROOT, ROOT))

@@ -113,7 +113,7 @@ def _fullsize_volume(scene, color_dims, dev):
         vf = synth.pack_feat_volume(feat, desc.feat_pitch).to(dev) if color_dims else None
         vol64 = (sdf[None] if feat is None else torch.cat([sdf[None], feat], 0)).double()
     else:                                      # 'decoded': unit-variance planes (what the encoder's LayerNorm emits) through
-        planes = synth.random_planes(m, 96, scale=1.0, seed=5)     # the tcgen05 decode kernel -- the bench's scene type
+        planes = synth.random_planes(m, 96, scale=1.0, seed=5)     # the tensor-core decode kernel -- the bench's scene type
         w1, b1, w2, b2 = synth.random_mlp(96, 1 + color_dims, seed=2)
         vs, vf = ops.tpv_decode(*[p.to(dev) for p in planes], w1.to(dev), b1.to(dev), w2.to(dev), b2.to(dev), desc)
         vol64 = orender.tpv_decode_ref(*[p.double() for p in planes], (H, W, Z), w1.double(), b1.double(), w2.double(), b2.double())

@@ -1,4 +1,4 @@
-"""GPU parity of the tcgen05 3xTF32 projection GEMM vs an fp64 reference (and vs cuBLAS fp32 for context)."""
+"""GPU parity of the wgmma 3xTF32 projection GEMM vs an fp64 reference (and vs cuBLAS fp32 for context)."""
 import pytest
 import torch
 
@@ -7,7 +7,8 @@ pytestmark = pytest.mark.gpu
 
 @pytest.mark.parametrize('M,N,K,relu,res', [(1000, 96, 96, False, False), (4099, 432, 96, False, False), (257, 192, 96, True, False),
                                             (3000, 96, 192, False, True), (70000, 1152, 96, False, False), (128, 216, 96, False, True),
-                                            (85, 72, 96, False, True), (459, 144, 96, True, False), (50, 24, 192, False, False)])
+                                            (85, 72, 96, False, True), (459, 144, 96, True, False), (50, 24, 192, False, False),
+                                            (301, 50, 96, False, True)])
 def test_linear_3xtf32_matches_fp64(M, N, K, relu, res):
     if not torch.cuda.is_available():
         pytest.skip('needs CUDA')
@@ -34,7 +35,7 @@ def test_linear_3xtf32_matches_fp64(M, N, K, relu, res):
     scale = ref.abs().max().item()
     print('3xTF32 GEMM M=%d N=%d K=%d: max abs err %.3e (cuBLAS fp32 %.3e), |y|max %.2f' % (M, N, K, err, err_cublas, scale))
     assert err < 2e-5 * max(scale, 1.0)
-    # the two pipelines (A operand in tensor memory -- default -- vs both operands in shared memory) compute the same products
+    # the two pipelines (A operand in registers -- default -- vs both operands in shared memory) compute the same products
     # in the same order: identical results
     from selfocc_b200 import _lib
     _lib.load().so_linear_force_ss(1)

@@ -149,7 +149,7 @@ def test_pixel_table_equals_in_kernel_grid():
 @pytest.mark.parametrize('simt', [False, True])
 @pytest.mark.parametrize('C,n_feat,hw,d', [(96, 0, 12, 6), (96, 24, 8, 5), (32, 3, 6, 4), (128, 0, 5, 9)])
 def test_tpv_decode_matches_oracle(C, n_feat, hw, d, simt):
-    """Both decode kernels: tcgen05 3xTF32 (default) and the fp32 SIMT one (forced through the test hook)."""
+    """Both decode kernels: wgmma 3xTF32 (default) and the fp32 SIMT one (forced through the test hook)."""
     dev = _dev()
     from oracle import render as orender
     from selfocc_b200 import ops, _lib
@@ -168,7 +168,7 @@ def test_tpv_decode_matches_oracle(C, n_feat, hw, d, simt):
         _lib.load().so_tpv_decode_force_simt(0)
     assert torch.all(vs[..., m.size_d:] == 0)
     err = (vs[..., :m.size_d] - ref[0]).abs().max().item()
-    print('decode (%s) sdf max abs err %.3e (|sdf| max %.2f)' % ('simt' if simt else 'tcgen05', err, ref[0].abs().max().item()))
+    print('decode (%s) sdf max abs err %.3e (|sdf| max %.2f)' % ('simt' if simt else 'wgmma', err, ref[0].abs().max().item()))
     assert err < 2e-5 * max(1.0, ref[0].abs().max().item())
     if n_feat:
         assert torch.allclose(vf[..., :n_feat], ref[1:].permute(1, 2, 3, 0), atol=5e-5, rtol=1e-5)

@@ -271,7 +271,7 @@ def test_head_forward_with_the_shipped_occ_config_options():
 
 @pytest.mark.parametrize('n_feat,hw,d,slab', [(0, 12, 6, 5), (3, 9, 5, 32), (24, 7, 4, 3)])
 def test_decode_backward_native_matches_oracle_autograd(n_feat, hw, d, slab, monkeypatch):
-    """TPVDecodeFunction.backward, native slab path (tcgen05 GEMMs + so_tpv_decode_bwd_*): gradients of every plane and
+    """TPVDecodeFunction.backward, native slab path (wgmma GEMMs + so_tpv_decode_bwd_*): gradients of every plane and
     MLP parameter vs fp64 autograd through the oracle's decode (oracle/render.py:tpv_decode_ref), with several ragged slabs;
     the torch/cuBLAS restatement of the same slab (SELFOCC_B200_DECODE_BWD=torch) must agree as well."""
     dev = _dev()

@@ -108,7 +108,7 @@ def test_product_mapping_matches_reference_golden(golden):
 
 def test_modules_build_from_the_reference_config_dicts():
     """Drop-in check at the config boundary: the lifter / encoder / head dicts of EVERY shipped TPV experiment config
-    (tests/golden/reference_model_cfgs.json, dumped from the reference's own config files) construct the B200 modules."""
+    (tests/golden/reference_model_cfgs.json, dumped from the reference's own config files) construct the H100 modules."""
     import json, os
     cfgs = json.load(open(os.path.join(os.path.dirname(__file__), 'golden', 'reference_model_cfgs.json')))
     assert sorted(cfgs) == ['kitti/kitti_novel_depth.py', 'kitti/kitti_occ.py', 'kitti_raw/kitti_raw_depth.py',
