@@ -7,26 +7,43 @@
 // operand is split  v = hi + lo,  hi = v rounded to the nearest TF32 number (low 13 mantissa bits zero), lo = v - hi
 // (exact in fp32), and the product is accumulated as  hi*hi + lo*hi + hi*lo  in the fp32 register accumulator
 // ("3xTF32", error ~2^-21).  W is split once on the host side (so_split_tf32); X is split by the consumer warps.
+// Every output element takes the same products in the same order (32-wide k-atoms ascending; per atom hi*hi, lo*hi,
+// hi*lo; per product 4 k-steps of 8), whatever the tile width, M or the CTA: results are bit-reproducible across
+// shardings of the rows.
 //
-// Persistent, warp-specialised pipeline (one CTA per SM, 9 warps):
-//   warp 8      TMA producer   W tile (hi, lo; all K) once per CTA, then X atoms [128 x 32] (128B swizzle) into a ring of stages
-//   warps 0-7   two consumer warpgroups, 64 rows of the 128-row tile each: split the X atom into hi / lo, then
-//               3 products x 4 k-steps of wgmma.m64nBNk8.f32.tf32 into a register accumulator; epilogue (+bias, ReLU,
-//               +residual, optional LayerNorm over the row) straight from the accumulator registers to global memory.
+// Persistent, warp-specialised ping-pong pipeline (one CTA per SM, 9 warps):
+//   warp 8      TMA producer   W tile (hi, lo; all K) once per CTA, then X atoms [64 x 32] (128B swizzle) into a ring of stages
+//   warps 0-7   two consumer warpgroups.  The CTA's m-tiles (64 rows each) alternate between them, so one warpgroup's
+//               epilogue (+bias, ReLU, +residual, optional LayerNorm over the row; registers -> global) runs while the
+//               other issues its MMAs.  Per k-atom: split the X atom into hi / lo, then 3 products x 4 k-steps of
+//               wgmma.m64nBNk8.f32.tf32 into a register accumulator.
 // A CTA owns ONE n-tile (its W tile stays resident in shared memory) and walks m-tiles, so the streamed traffic per
 // output tile is the X tile and the Y tile only.  mbarriers: w_full | full[s] (TMA landed) -> empty[s] (stage consumed).
+// Each warpgroup has its own half of the ring, so every stage has one consumer and each warpgroup waits on consecutive
+// fills of its own stages (with one shared ring, a warpgroup waiting K/32 atoms ahead of the producer could take an
+// older phase of the same parity for its own).
 //
 // The A operand (X hi / lo) comes from REGISTERS by default: each thread loads its wgmma fragment from the swizzled
 // stage and splits it in registers, so the tensor core reads only W from shared memory and the stage is released as
-// soon as it has been loaded.  so_linear_force_ss(1) selects the variant with both operands in shared memory (the X
-// atom is split in place into hi plus a second lo buffer); both issue the same products in the same order.
+// soon as it has been loaded.  Two fragment sets: atom a + 1 is loaded and split while the MMAs of atom a run
+// (wgmma.wait_group 1).  so_linear_force_ss(1) selects the variant with both operands in shared memory (the X atom is
+// split in place into hi plus a second lo buffer); both issue the same products in the same order.
+//
+// Tuning, one H100 80GB HBM3 at a 400 W power limit, the 12 launches of one encoder layer (scripts/bench_gemm.py, sum):
+//   both warpgroups on one 128-row tile, wait_group 0 per atom, BN = fewest padded columns   1.244 ms
+//   ping-pong 64-row tiles, two fragment sets at every BN (before the ring split; spills)    1.027 ms
+//   ping-pong, ring halves per warpgroup, two fragment sets at BN <= 80, BN by bn_cost       1.038 ms  (shipped)
+//   bn_cost picks BN = 80 for N = 3456: 0.138 -> 0.100 ms per zh / wz launch.  The 64-row tiles are slower for
+//   M = 7967 x N = 96 with LayerNorm (0.016 -> 0.031 ms: 125 CTAs with one tile each, one warpgroup busy).
 #include "tc_common.cuh"
 
 namespace so {
 
 constexpr int kGemmConsumers = 256;                 // two warpgroups
 constexpr int kGemmThreads = kGemmConsumers + 32;   // + the TMA producer warp
-constexpr int kMaxStages = 8;
+constexpr int kGemmTileM = kWgRows;                 // rows per m-tile: one warpgroup, one m64 wgmma
+constexpr int kGemmTileBytes = kGemmTileM * 128;    // one X atom of one m-tile
+constexpr int kMaxStages = 12;
 constexpr int kMaxBN = 128;
 
 typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
@@ -63,26 +80,45 @@ struct PipeCfg {
   int stage_bytes;          // raw X atom (A from registers) or raw/hi + lo atoms (A from shared memory)
   int w_bytes;              // resident W bytes = 2 * KA * BN * 128
   int smem;                 // dynamic shared memory request (incl. 1 KB alignment slack)
+  int n_tiles, m_tiles, groups;  // grid = n_tiles x groups CTAs; group g walks m-tiles g, g + groups, ...
 };
 
-// n-tile width: the fewest padded columns, ties to the wider tile (fewer passes over X)
-static int pick_bn(int N) {
-  int best = kMaxBN, best_cols = (int)ceil_div64(N, kMaxBN) * kMaxBN;
-  for (int bn : {96, 64, 32}) {
-    const int cols = (int)ceil_div64(N, bn) * bn;
-    if (cols < best_cols) { best = bn; best_cols = cols; }
+// Per-CTA cost of an n-tile width: the m-tiles of the busiest CTA times (BN + a fixed per-tile cost, in columns, for
+// loading and splitting the X tile).  Balances padding against filling the SMs: N = 3456 at BN = 128 gives 27 n-tiles,
+// 4 CTAs each, 108 of 132 SMs busy; BN = 80 gives 44 n-tiles x 3 = 132.
+static long long bn_cost(int bn, int N, int m_tiles, int sms, int* n_tiles_out, int* groups_out) {
+  const int n_tiles = (int)ceil_div64(N, bn);
+  int groups = sms / n_tiles;
+  if (groups < 1) groups = 1;
+  if (groups > m_tiles) groups = m_tiles;
+  if (n_tiles_out) *n_tiles_out = n_tiles;
+  if (groups_out) *groups_out = groups;
+  constexpr int kTileCostCols = 32;
+  return ceil_div64(m_tiles, groups) * (long long)(bn + kTileCostCols) * ((n_tiles + sms - 1) / sms);
+}
+
+// n-tile width: the lowest bn_cost, ties to the wider tile.  The LayerNorm epilogue needs the whole row in one tile.
+static int pick_bn(int N, int m_tiles, int sms, bool whole_row) {
+  if (whole_row) return N;
+  int best = kMaxBN;
+  long long best_cost = bn_cost(kMaxBN, N, m_tiles, sms, nullptr, nullptr);
+  for (int bn : {96, 80, 64, 32}) {
+    const long long c = bn_cost(bn, N, m_tiles, sms, nullptr, nullptr);
+    if (c < best_cost) { best = bn; best_cost = c; }
   }
   return best;
 }
 
-static PipeCfg make_pipe_cfg(int N, int K, bool reg_a) {
+static PipeCfg make_pipe_cfg(int64_t M, int N, int K, bool reg_a, bool whole_row, int sms) {
   PipeCfg c;
-  c.BN = pick_bn(N);
+  c.m_tiles = (int)ceil_div64(M, kGemmTileM);
+  c.BN = pick_bn(N, c.m_tiles, sms, whole_row);
+  bn_cost(c.BN, N, c.m_tiles, sms, &c.n_tiles, &c.groups);
   c.KA = K / kAtomK;
   c.w_bytes = 2 * c.KA * c.BN * 128;
-  c.stage_bytes = reg_a ? kAtomBytesA : 2 * kAtomBytesA;
+  c.stage_bytes = reg_a ? kGemmTileBytes : 2 * kGemmTileBytes;
   const int fixed = c.w_bytes + 256;                          // + mbarriers
-  c.stages = (227 * 1024 - 1024 - fixed) / c.stage_bytes;
+  c.stages = (227 * 1024 - 1024 - fixed) / c.stage_bytes & ~1;  // even: half of the ring per warpgroup
   if (c.stages > kMaxStages) c.stages = kMaxStages;
   c.smem = fixed + c.stages * c.stage_bytes + 1024;
   return c;
@@ -100,6 +136,50 @@ __device__ __forceinline__ void fence_regs(uint32_t* r) {
   for (int i = 0; i < NR; ++i) asm volatile("" : "+r"(r[i])::"memory");
 }
 
+// next position (stage s, phase ph) in a ring of n stages
+__device__ __forceinline__ void ring_advance(int& s, uint32_t& ph, int n) {
+  if (++s == n) { s = 0; ph ^= 1; }
+}
+
+// register-A fragment of one 64-row X atom: rows frag_row and frag_row + 8, k = 8 kk + t and 8 kk + t + 4, i.e. 16-byte
+// chunks 2 kk and 2 kk + 1; both rows have (row & 7) == g, so the swizzle is the same for the pair.  Split into hi / lo.
+__device__ __forceinline__ void load_split_frag(const uint8_t* stage, int frag_row, int g, int t, uint32_t* ah, uint32_t* al) {
+  const uint8_t* r0 = stage + frag_row * 128 + 4 * t;
+#pragma unroll
+  for (int kk = 0; kk < 4; ++kk) {
+    const float v[4] = {*reinterpret_cast<const float*>(r0 + (((2 * kk) ^ g) << 4)),
+                        *reinterpret_cast<const float*>(r0 + 8 * 128 + (((2 * kk) ^ g) << 4)),
+                        *reinterpret_cast<const float*>(r0 + (((2 * kk + 1) ^ g) << 4)),
+                        *reinterpret_cast<const float*>(r0 + 8 * 128 + (((2 * kk + 1) ^ g) << 4))};
+#pragma unroll
+    for (int i = 0; i < 4; ++i) {
+      const float h = tf32_rn(v[i]);
+      ah[4 * kk + i] = __float_as_uint(h);
+      al[4 * kk + i] = __float_as_uint(v[i] - h);
+    }
+  }
+  fence_regs<16>(ah);
+  fence_regs<16>(al);
+}
+
+// the 12 MMAs of one k-atom, A from registers: hi*hi, lo*hi, hi*lo, 4 k-steps each, as one commit group
+template <int BN>
+__device__ __forceinline__ void mma_atom_rs(float* acc, uint32_t* ah, uint32_t* al, uint32_t bhi, uint32_t blo, uint32_t& accum) {
+  fence_regs<BN / 2>(acc);
+  wg_fence();
+#pragma unroll
+  for (int prod = 0; prod < 3; ++prod) {
+    const uint32_t* af = prod == 1 ? al : ah;
+    const uint32_t bb = prod == 2 ? blo : bhi;
+#pragma unroll
+    for (int kk = 0; kk < kAtomK / 8; ++kk) {
+      Wgmma<BN>::rs(acc, af + 4 * kk, make_desc(bb + kk * 32), accum);
+      accum = 1u;
+    }
+  }
+  wg_commit();
+}
+
 template <int BN, bool kRegA>
 __global__ void __launch_bounds__(kGemmThreads, 1)
 linear_3xtf32_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_constant__ CUtensorMap map_whi,
@@ -107,7 +187,7 @@ linear_3xtf32_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_con
                      const float* __restrict__ residual, float* __restrict__ y, long long M, int N, int KA, int stages,
                      int n_tiles, int m_tiles, int relu, const float* __restrict__ ln_gamma, const float* __restrict__ ln_beta,
                      float ln_eps) {
-  constexpr int kStageBytes = kRegA ? kAtomBytesA : 2 * kAtomBytesA;
+  constexpr int kStageBytes = kRegA ? kGemmTileBytes : 2 * kGemmTileBytes;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* sm = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
   const int w_bytes = 2 * KA * BN * 128;
@@ -118,6 +198,7 @@ linear_3xtf32_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_con
   uint64_t* w_full = bars;
   uint64_t* full = bars + 1;
   uint64_t* empty = full + kMaxStages;
+  const int half = stages / 2;                                    // ring stages per warpgroup
 
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int n_tile = blockIdx.x % n_tiles;
@@ -126,101 +207,103 @@ linear_3xtf32_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_con
 
   if (tid == 0) {
     mbar_init(w_full, 1);
-    for (int s = 0; s < kMaxStages; ++s) { mbar_init(full + s, 1); mbar_init(empty + s, kGemmConsumers / 32); }
+    for (int s = 0; s < kMaxStages; ++s) { mbar_init(full + s, 1); mbar_init(empty + s, kGemmConsumers / 2 / 32); }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
   __syncthreads();
 
   if (warp == kGemmConsumers / 32) {
-    // ===== TMA producer =====
+    // ===== TMA producer: the CTA's m-tiles in order, KA atoms each =====
     if (lane == 0) {
       mbar_expect_tx(w_full, (uint32_t)w_bytes);
       for (int a = 0; a < KA; ++a) {
         tma_load_2d(w_hi + a * BN * 128, &map_whi, a * kAtomK, n0, w_full);
         tma_load_2d(w_lo + a * BN * 128, &map_wlo, a * kAtomK, n0, w_full);
       }
-      int s = 0; uint32_t ph = 0;
-      constexpr int kPrefetchTiles = 4;                 // X tiles requested into L2 ahead of the smem ring
+      int s0 = 0, s1 = 0; uint32_t ph0 = 0, ph1 = 0;   // position in each warpgroup's half of the ring
+      constexpr int kPrefetchTiles = 8;                 // X tiles requested into L2 ahead of the smem ring
       for (int p = 0; p < kPrefetchTiles; ++p) {
         int mt = group + p * n_groups;
         if (mt < m_tiles)
-          for (int a = 0; a < KA; ++a) tma_prefetch_l2_2d(&map_x, a * kAtomK, mt * kBM);
+          for (int a = 0; a < KA; ++a) tma_prefetch_l2_2d(&map_x, a * kAtomK, mt * kGemmTileM);
       }
-      for (int mt = group; mt < m_tiles; mt += n_groups) {
+      int w = 0;                                        // warpgroup of the current tile
+      for (int mt = group; mt < m_tiles; mt += n_groups, w ^= 1) {
         const int mt_pf = mt + kPrefetchTiles * n_groups;
         if (mt_pf < m_tiles)
-          for (int a = 0; a < KA; ++a) tma_prefetch_l2_2d(&map_x, a * kAtomK, mt_pf * kBM);
+          for (int a = 0; a < KA; ++a) tma_prefetch_l2_2d(&map_x, a * kAtomK, mt_pf * kGemmTileM);
         for (int a = 0; a < KA; ++a) {
-          mbar_wait(empty + s, ph ^ 1);
-          mbar_expect_tx(full + s, (uint32_t)kAtomBytesA);
-          tma_load_2d(ring + s * kStageBytes, &map_x, a * kAtomK, mt * kBM, full + s);
-          if (++s == stages) { s = 0; ph ^= 1; }
+          const int slot = w ? half + s1 : s0;
+          mbar_wait(empty + slot, (w ? ph1 : ph0) ^ 1);
+          mbar_expect_tx(full + slot, (uint32_t)kGemmTileBytes);
+          tma_load_2d(ring + slot * kStageBytes, &map_x, a * kAtomK, mt * kGemmTileM, full + slot);
+          if (w) ring_advance(s1, ph1, half); else ring_advance(s0, ph0, half);
         }
       }
     }
     return;
   }
 
-  // ===== consumers: warpgroup wg owns rows 64 wg .. 64 wg + 63 of every m-tile =====
+  // ===== consumers: warpgroup wg takes the CTA's m-tiles j = wg, wg + 2, ... (64 rows each) =====
   const int wg = warp >> 2, wl = warp & 3, g = lane >> 2, t = lane & 3;
-  const int frag_row = wg * kWgRows + wl * 16 + g;                // this thread's rows: frag_row and frag_row + 8
+  const int frag_row = wl * 16 + g;                               // this thread's rows: frag_row and frag_row + 8
   float acc[BN / 2];
 #pragma unroll
   for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
   const uint32_t whi = smem_u32(w_hi), wlo = smem_u32(w_lo);
   mbar_wait(w_full, 0);
+  uint8_t* my_ring = ring + wg * half * kStageBytes;              // this warpgroup's half of the ring
+  uint64_t* my_full = full + wg * half;
+  uint64_t* my_empty = empty + wg * half;
   int s = 0; uint32_t ph = 0;
-  for (int mt = group; mt < m_tiles; mt += n_groups) {
+  for (int mt = group + wg * n_groups; mt < m_tiles; mt += 2 * n_groups) {
     uint32_t accum = 0;
-    for (int a = 0; a < KA; ++a) {
-      mbar_wait(full + s, ph);
-      uint8_t* stage = ring + s * kStageBytes;
-      const uint32_t bhi = whi + a * BN * 128, blo = wlo + a * BN * 128;
-      if constexpr (kRegA) {
-        // fragment of k-step kk: rows frag_row (+8), k = 8 kk + t and 8 kk + t + 4, i.e. 16-byte chunks 2 kk and 2 kk + 1;
-        // both rows have (row & 7) == g, so the swizzle is the same for the pair
-        const uint8_t* r0 = stage + frag_row * 128 + 4 * t;
-        uint32_t ah[16], al[16];
-#pragma unroll
-        for (int kk = 0; kk < 4; ++kk) {
-          const float v[4] = {*reinterpret_cast<const float*>(r0 + (((2 * kk) ^ g) << 4)),
-                              *reinterpret_cast<const float*>(r0 + 8 * 128 + (((2 * kk) ^ g) << 4)),
-                              *reinterpret_cast<const float*>(r0 + (((2 * kk + 1) ^ g) << 4)),
-                              *reinterpret_cast<const float*>(r0 + 8 * 128 + (((2 * kk + 1) ^ g) << 4))};
-#pragma unroll
-          for (int i = 0; i < 4; ++i) {
-            const float h = tf32_rn(v[i]);
-            ah[4 * kk + i] = __float_as_uint(h);
-            al[4 * kk + i] = __float_as_uint(v[i] - h);
+    if constexpr (kRegA) {
+      // two fragment sets: atom a + 1 is loaded and split while the MMAs of atom a run.  At BN >= 96 the second set
+      // does not fit in the 168 registers a thread gets: one set, and each atom's MMAs complete before the next load.
+      constexpr bool kTwoSets = BN <= 80;
+      uint32_t ah0[16], al0[16], ah1_[kTwoSets ? 16 : 1], al1_[kTwoSets ? 16 : 1];
+      uint32_t* ah1 = kTwoSets ? ah1_ : ah0;
+      uint32_t* al1 = kTwoSets ? al1_ : al0;
+      mbar_wait(my_full + s, ph);
+      load_split_frag(my_ring + s * kStageBytes, frag_row, g, t, ah0, al0);
+      __syncwarp();
+      if (lane == 0) mbar_arrive(my_empty + s);            // the stage is in registers: the producer may refill it
+      ring_advance(s, ph, half);
+      for (int a = 0; a < KA; a += 2) {
+        mma_atom_rs<BN>(acc, ah0, al0, whi + a * BN * 128, wlo + a * BN * 128, accum);
+        if constexpr (kTwoSets) wg_wait1(); else wg_wait0();   // atom a - 1 is done: set 1 is free
+        if (a + 1 < KA) {
+          mbar_wait(my_full + s, ph);
+          load_split_frag(my_ring + s * kStageBytes, frag_row, g, t, ah1, al1);
+          __syncwarp();
+          if (lane == 0) mbar_arrive(my_empty + s);
+          ring_advance(s, ph, half);
+          mma_atom_rs<BN>(acc, ah1, al1, whi + (a + 1) * BN * 128, wlo + (a + 1) * BN * 128, accum);
+          if constexpr (kTwoSets) wg_wait1(); else wg_wait0();  // atom a is done: set 0 is free
+          if (a + 2 < KA) {
+            mbar_wait(my_full + s, ph);
+            load_split_frag(my_ring + s * kStageBytes, frag_row, g, t, ah0, al0);
+            __syncwarp();
+            if (lane == 0) mbar_arrive(my_empty + s);
+            ring_advance(s, ph, half);
           }
         }
-        fence_regs<16>(ah);
-        fence_regs<16>(al);
-        __syncwarp();
-        if (lane == 0) mbar_arrive(empty + s);          // the stage is in registers: the producer may refill it
-        fence_regs<BN / 2>(acc);
-        wg_fence();
-#pragma unroll
-        for (int prod = 0; prod < 3; ++prod) {
-          const uint32_t* af = prod == 1 ? al : ah;
-          const uint32_t bb = prod == 2 ? blo : bhi;
-#pragma unroll
-          for (int kk = 0; kk < kAtomK / 8; ++kk) {
-            Wgmma<BN>::rs(acc, af + 4 * kk, make_desc(bb + kk * 32), accum);
-            accum = 1u;
-          }
-        }
-        wg_commit();
-        wg_wait0();
-        fence_regs<BN / 2>(acc);
-      } else {
-        // split this warpgroup's 64 rows in place: raw -> hi, lo into the second half of the stage.  Element-wise, so the
+      }
+      wg_wait0();
+      fence_regs<BN / 2>(acc);
+    } else {
+      for (int a = 0; a < KA; ++a) {
+        mbar_wait(my_full + s, ph);
+        uint8_t* stage = my_ring + s * kStageBytes;
+        const uint32_t bhi = whi + a * BN * 128, blo = wlo + a * BN * 128;
+        // split the 64-row atom in place: raw -> hi, lo into the second half of the stage.  Element-wise, so the
         // swizzle is irrelevant.
-        float4* hi = reinterpret_cast<float4*>(stage + wg * kWgRows * 128);
-        float4* lo = reinterpret_cast<float4*>(stage + kAtomBytesA + wg * kWgRows * 128);
+        float4* hi = reinterpret_cast<float4*>(stage);
+        float4* lo = reinterpret_cast<float4*>(stage + kGemmTileBytes);
         const int wt = tid & 127;
 #pragma unroll
-        for (int i = 0; i < kWgRows * 128 / 16 / 128; ++i) {
+        for (int i = 0; i < kGemmTileBytes / 16 / 128; ++i) {
           float4 v = hi[wt + i * 128], h, l;
           h.x = tf32_rn(v.x); l.x = v.x - h.x;
           h.y = tf32_rn(v.y); l.y = v.y - h.y;
@@ -231,7 +314,7 @@ linear_3xtf32_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_con
         }
         asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // generic-proxy smem writes -> visible to wgmma
         wg_sync(1 + wg);
-        const uint32_t ahi = smem_u32(stage + wg * kWgRows * 128), alo = ahi + kAtomBytesA;
+        const uint32_t ahi = smem_u32(stage), alo = ahi + kGemmTileBytes;
         fence_regs<BN / 2>(acc);
         wg_fence();
 #pragma unroll
@@ -248,13 +331,13 @@ linear_3xtf32_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_con
         wg_wait0();
         fence_regs<BN / 2>(acc);
         __syncwarp();
-        if (lane == 0) mbar_arrive(empty + s);          // this warpgroup's MMAs have finished reading the stage
+        if (lane == 0) mbar_arrive(my_empty + s);          // this warpgroup's MMAs have finished reading the stage
+        ring_advance(s, ph, half);
       }
-      if (++s == stages) { s = 0; ph ^= 1; }
     }
 
     // ===== epilogue: accumulator registers -> (+bias, ReLU, +residual [, LayerNorm]) -> global =====
-    const long long row[2] = {(long long)mt * kBM + frag_row, (long long)mt * kBM + frag_row + 8};
+    const long long row[2] = {(long long)mt * kGemmTileM + frag_row, (long long)mt * kGemmTileM + frag_row + 8};
 #pragma unroll
     for (int j = 0; j < BN / 8; ++j) {
       const int gc = n0 + 8 * j + 2 * t;                // N is even: the column pair is in range or out of range together
@@ -376,41 +459,39 @@ static int linear_impl(const float* x, const float* w_hi, const float* w_lo, con
   // the epilogue stores Y and reads the residual as column pairs (float2)
   if ((reinterpret_cast<uintptr_t>(y) & 7) || (reinterpret_cast<uintptr_t>(residual) & 7) || (N % 2)) return SO_ERR_UNSUPPORTED;
   const bool reg_a = !g_linear_force_ss;
-  PipeCfg cfg = make_pipe_cfg(N, K, reg_a);
+  PipeCfg cfg = make_pipe_cfg(M, N, K, reg_a, ln_gamma != nullptr, num_sms());
   if (cfg.stages < 2) return SO_ERR_UNSUPPORTED;
-  if (ln_gamma && cfg.BN != N) return SO_ERR_UNSUPPORTED;
   CUtensorMap mx, mhi, mlo;
   int rc;
-  if ((rc = make_tmap(&mx, x, M, K, kBM))) return rc;
+  if ((rc = make_tmap(&mx, x, M, K, kGemmTileM))) return rc;
   if ((rc = make_tmap(&mhi, w_hi, N, K, cfg.BN))) return rc;
   if ((rc = make_tmap(&mlo, w_lo, N, K, cfg.BN))) return rc;
   static PerDeviceOnce smem_attr;
   if ((rc = smem_attr.run([] {
          int r;
-         if ((r = set_smem_attr<32, true>()) || (r = set_smem_attr<64, true>()) || (r = set_smem_attr<96, true>()) ||
-             (r = set_smem_attr<128, true>()) || (r = set_smem_attr<32, false>()) || (r = set_smem_attr<64, false>()) ||
-             (r = set_smem_attr<96, false>()) || (r = set_smem_attr<128, false>()))
+         if ((r = set_smem_attr<32, true>()) || (r = set_smem_attr<64, true>()) || (r = set_smem_attr<80, true>()) ||
+             (r = set_smem_attr<96, true>()) || (r = set_smem_attr<128, true>()) || (r = set_smem_attr<32, false>()) ||
+             (r = set_smem_attr<64, false>()) || (r = set_smem_attr<80, false>()) || (r = set_smem_attr<96, false>()) ||
+             (r = set_smem_attr<128, false>()))
            return r;
          return SO_OK;
        })))
     return rc;
   cudaStream_t st = (cudaStream_t)stream;
-  const int n_tiles = (int)ceil_div64(N, cfg.BN), m_tiles = (int)ceil_div64(M, kBM);
-  int groups = num_sms() / n_tiles;
-  if (groups < 1) groups = 1;
-  if (groups > m_tiles) groups = m_tiles;
   ProfScope prof(8, st);
-#define SO_GEMM(BN_, REGA)                                                                                                     \
-  linear_3xtf32_kernel<BN_, REGA><<<n_tiles * groups, kGemmThreads, cfg.smem, st>>>(mx, mhi, mlo, bias, residual, y, (long long)M, \
-                                                                                   N, cfg.KA, cfg.stages, n_tiles, m_tiles, relu,  \
-                                                                                   ln_gamma, ln_beta, ln_eps)
+#define SO_GEMM(BN_, REGA)                                                                                                   \
+  linear_3xtf32_kernel<BN_, REGA><<<cfg.n_tiles * cfg.groups, kGemmThreads, cfg.smem, st>>>(                                \
+      mx, mhi, mlo, bias, residual, y, (long long)M, N, cfg.KA, cfg.stages, cfg.n_tiles, cfg.m_tiles, relu, ln_gamma, ln_beta, \
+      ln_eps)
   switch (cfg.BN * 2 + (reg_a ? 1 : 0)) {
     case 32 * 2 + 1: SO_GEMM(32, true); break;
     case 64 * 2 + 1: SO_GEMM(64, true); break;
+    case 80 * 2 + 1: SO_GEMM(80, true); break;
     case 96 * 2 + 1: SO_GEMM(96, true); break;
     case 128 * 2 + 1: SO_GEMM(128, true); break;
     case 32 * 2: SO_GEMM(32, false); break;
     case 64 * 2: SO_GEMM(64, false); break;
+    case 80 * 2: SO_GEMM(80, false); break;
     case 96 * 2: SO_GEMM(96, false); break;
     default: SO_GEMM(128, false); break;
   }
