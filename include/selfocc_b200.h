@@ -28,7 +28,8 @@ extern "C" {
 #define SO_ERR_CUDA (-3)          /* a CUDA runtime call or launch failed; see so_last_cuda_error */
 #define SO_ERR_NO_DEVICE (-4)
 
-#define SO_ABI_VERSION 3   /* 2: so_render_train_forward gained pair_workspace; 3: packed render volume entry points */
+#define SO_ABI_VERSION 4   /* 2: so_render_train_forward gained pair_workspace; 3: packed render volume entry points;
+                              4: backward of the fused attention cores */
 
 /* ABI version of the loaded library (compare with SO_ABI_VERSION). */
 int so_abi_version(void);
@@ -363,6 +364,32 @@ int so_tpv_self_attn_forward_strided(const float* value, const int64_t* spatial_
                                      const float* offsets, const float* logits, const float* ref, float* out, int32_t Nv,
                                      int32_t Hd, int32_t Dh, int32_t Q, int32_t L, int32_t P, int32_t value_ld,
                                      int32_t offsets_ld, int32_t logits_ld, void* stream);
+
+/* Backward of so_tpv_cross_attn_forward (training).  Takes the forward's operands (contiguous, no strided form) plus
+ *   count int32 [Q]       the forward's per-query visible-camera count (so_tpv_cross_attn_forward's `count` output)
+ *   grad_slots [Q, Hd*Dh] the gradient of `slots`
+ * and writes
+ *   grad_value [N, Nv, Hd, Dh]      ACCUMULATED with atomics: the caller zero-fills it
+ *   grad_offsets [Q, Hd, L, D, 2]   summed over the visible cameras; overwritten
+ *   grad_logits [Q, Hd, L, D]       softmax backward over the (L, D) samples of each (query, head); overwritten
+ * Each sample's softmax weight and location are recomputed with the forward's arithmetic (nothing else is saved), so
+ * this is the adjoint of the function the forward evaluated.  A query visible in no camera gets zero gradients.
+ * grad_offsets and grad_logits are deterministic (fixed loop and shuffle order, no atomics); grad_value is not.
+ * value, grad_value and grad_slots 16-byte aligned, offsets and grad_offsets 8-byte aligned.  Dh must be 16 or 32. */
+int so_tpv_cross_attn_backward(const float* value, const int64_t* spatial_shapes, const int64_t* level_start_index,
+                               const float* offsets, const float* logits, const float* uv, const uint8_t* vis,
+                               const int32_t* count, const float* grad_slots, float* grad_value, float* grad_offsets,
+                               float* grad_logits, int32_t N, int32_t Nv, int32_t Hd, int32_t Dh, int32_t Q, int32_t L,
+                               int32_t D, void* stream);
+
+/* Backward of so_tpv_self_attn_forward (training): grad_out [Q, Hd*Dh] ->
+ *   grad_value [Nv, Hd, Dh] (ACCUMULATED with atomics: the caller zero-fills it), grad_offsets [Q, Hd, L, P, 2],
+ *   grad_logits [Q, Hd, L, P] (both overwritten, deterministic).
+ * Same recomputation, alignment and Dh rules as so_tpv_cross_attn_backward; ref is a constant (no gradient). */
+int so_tpv_self_attn_backward(const float* value, const int64_t* spatial_shapes, const int64_t* level_start_index,
+                              const float* offsets, const float* logits, const float* ref, const float* grad_out,
+                              float* grad_value, float* grad_offsets, float* grad_logits, int32_t Nv, int32_t Hd, int32_t Dh,
+                              int32_t Q, int32_t L, int32_t P, void* stream);
 
 #ifdef __cplusplus
 }

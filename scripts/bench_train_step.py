@@ -3,9 +3,11 @@ every rank lifts the same frame, renders its slice of each camera's rays (head.r
     python scripts/bench_train_step.py [--profile]
     python -m torch.distributed.run --nproc-per-node N --master-addr 127.0.0.1 scripts/bench_train_step.py
 Single GPU:
-lifter -> encoder (autograd path: mmcv-contract MSDA op forward/backward kernels + cuBLAS projections) -> NeuSHead.forward
-(fused decode forward, training-form render kernels) -> toy loss on depth / weights / eik_grad / rgb -> backward to every
-parameter.  Prints one JSON line (ms per step, device timed).  nuScenes_occ geometry: TPV 257x257x25, 6 cams x 48x100 rays."""
+lifter -> encoder (autograd path: the fused self- and image cross-attention cores with their backward kernels, projections
+forward and input gradient on the wgmma GEMM, weight gradients on cuBLAS) -> NeuSHead.forward (fused decode forward,
+training-form render kernels) -> toy loss on depth / weights / eik_grad / rgb -> backward to every parameter.  Prints one
+JSON line (ms per step, device timed; peak device memory of the timed steps).  nuScenes_occ geometry: TPV 257x257x25,
+6 cams x 48x100 rays."""
 import json, os, sys, time
 import numpy as np
 import torch
@@ -68,6 +70,7 @@ def step():
 for _ in range(2):
     step()
 torch.cuda.synchronize()
+torch.cuda.reset_peak_memory_stats()
 K = 5
 a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
 l0 = _lib.launch_count()
@@ -77,6 +80,7 @@ for _ in range(K):
 b.record()
 torch.cuda.synchronize()
 ms = a.elapsed_time(b) / K
+peak_gb = torch.cuda.max_memory_allocated() / 2 ** 30
 if world > 1:
     t = torch.tensor([ms], device=dev)
     dist.all_reduce(t, op=dist.ReduceOp.MAX)
@@ -89,7 +93,7 @@ if '--profile' in sys.argv and world == 1:
     print(prof.key_averages().table(sort_by='cuda_time_total', row_limit=25))
 if rank == 0:
   print(json.dumps({'workload': 'nuscenes_occ-like training step, %d GPU(s)%s, fp32, 6x48x100 rays x 256, TPV 257x257x25, colour' % (world, ' ray-sharded + DDP' if world > 1 else ''), 'ms_per_step': ms,
-                  'rays_per_s': 28800 / (ms * 1e-3), 'library_launches_per_step': (_lib.launch_count() - l0) / K,
+                  'rays_per_s': 28800 / (ms * 1e-3), 'library_launches_per_step': (_lib.launch_count() - l0) / K, 'peak_mem_gb': peak_gb,
                   'loss': float(last), 'finite': bool(torch.isfinite(last))}))
 if world > 1:
     dist.destroy_process_group()

@@ -8,7 +8,7 @@ import os
 
 _PKG = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.environ.get('SELFOCC_B200_LIB') or os.path.join(_PKG, 'lib', 'libselfocc_b200.so')   # env: experimental variant
-ABI_VERSION = 3
+ABI_VERSION = 4
 
 
 class AxisMap(C.Structure):
@@ -88,6 +88,8 @@ SIGNATURES = {
     'so_attn_force_v1': (C.c_int, [C.c_int]),
     'so_visible_index_lists': (C.c_int, [_P, _I, _I, _I, _P, _P, _P]),
     'so_tpv_self_attn_forward': (C.c_int, [_P, _P, _P, _P, _P, _P, _P, _I, _I, _I, _I, _I, _I, _P]),
+    'so_tpv_cross_attn_backward': (C.c_int, [_P] * 12 + [_I] * 7 + [_P]),
+    'so_tpv_self_attn_backward': (C.c_int, [_P] * 10 + [_I] * 6 + [_P]),
 }
 
 _lib = None

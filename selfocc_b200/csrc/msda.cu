@@ -490,6 +490,194 @@ __global__ void __launch_bounds__(256, SO_ATTN2_MIN_CTAS) tpv_self_attn2_kernel(
   if (live) *reinterpret_cast<float4*>(out + item * DH + lc * 4) = acc;
 }
 
+// ======================================================================================================================
+// Backward of the two fused attention cores (training).  Same lane mapping as the first-generation forwards: LPI = DH/4
+// lanes own one (query, head), each one float4 of channels; the cross-attention's SPLIT sample groups take pillar points
+// d = g, g + SPLIT, ...  Nothing from the forward is stored: each sample's softmax weight and location are recomputed with
+// the forward's arithmetic (softmax_stats, __expf, fmaf(o, 1/W_l, r)), so the gradients are those of the function the
+// forward evaluated.  Per sample, the cross-attention loops over the visible cameras in camera order inside the sample
+// loop, so the per-sample results (location gradient, attention-weight gradient) are complete before they are reduced.
+//   grad_value   += a * corner weight * g           128-bit vector atomics (the only atomics)
+//   grad_offsets  = a * <g, d bilinear / d loc> / (W_l, H_l)     summed over the cameras, reduced over the item's lanes
+//   grad_logits   = a_i (g_a_i - sum_j a_j g_a_j),  g_a_i = <g, bilinear_i> summed over the cameras
+// g_a_i is parked in grad_logits by the lane that owns sample i and rewritten by the same lane once sum_j a_j g_a_j is
+// known (shuffle fold over the sample groups): fixed loop and shuffle order, so grad_offsets / grad_logits are
+// deterministic.
+
+// Adjoint of bilinear4 for one lane's 4 channels: accumulates <g, s> into ga and <g, ds/dlx>, <g, ds/dly> into gx, gy
+// (normalised-location derivatives, still to be multiplied by the attention weight), and scatters aw * w_corner * g into
+// grad_value.  vofs: offset of this lane's channel 0 in pixel 0 of the level (same for value and grad_value).
+__device__ __forceinline__ void bilinear4_adjoint(const float* __restrict__ value, float* __restrict__ gvalue, long long vofs,
+                                                  int pstride, int Hl, int Wl, float lx, float ly, float4 g, float aw, bool live,
+                                                  float& ga, float& gx, float& gy) {
+  float x = lx * (float)Wl - 0.5f, y = ly * (float)Hl - 0.5f;
+  if (!(y > -1.f && x > -1.f && y < (float)Hl && x < (float)Wl)) return;
+  float xf = floorf(x), yf = floorf(y);
+  int x0 = (int)xf, y0 = (int)yf;
+  float fx = x - xf, fy = y - yf;
+  bool xa = x0 >= 0, xb = x0 + 1 < Wl, ya = y0 >= 0, yb = y0 + 1 < Hl;
+  long long o00 = vofs + ((long long)y0 * Wl + x0) * pstride;
+  long long o01 = o00 + pstride, o10 = o00 + (long long)Wl * pstride, o11 = o10 + pstride;
+  float4 z = make_float4(0.f, 0.f, 0.f, 0.f);
+  float4 v00 = (ya && xa) ? __ldg(reinterpret_cast<const float4*>(value + o00)) : z;
+  float4 v01 = (ya && xb) ? __ldg(reinterpret_cast<const float4*>(value + o01)) : z;
+  float4 v10 = (yb && xa) ? __ldg(reinterpret_cast<const float4*>(value + o10)) : z;
+  float4 v11 = (yb && xb) ? __ldg(reinterpret_cast<const float4*>(value + o11)) : z;
+  float w00 = (1.f - fy) * (1.f - fx), w01 = (1.f - fy) * fx, w10 = fy * (1.f - fx), w11 = fy * fx;
+  float d00 = g.x * v00.x + g.y * v00.y + g.z * v00.z + g.w * v00.w;
+  float d01 = g.x * v01.x + g.y * v01.y + g.z * v01.z + g.w * v01.w;
+  float d10 = g.x * v10.x + g.y * v10.y + g.z * v10.z + g.w * v10.w;
+  float d11 = g.x * v11.x + g.y * v11.y + g.z * v11.z + g.w * v11.w;
+  ga += w00 * d00 + w01 * d01 + w10 * d10 + w11 * d11;
+  gx += (float)Wl * ((1.f - fy) * (d01 - d00) + fy * (d11 - d10));
+  gy += (float)Hl * ((1.f - fx) * (d10 - d00) + fx * (d11 - d01));
+  if (!live) return;
+  if (ya && xa) { float s = aw * w00; atomicAdd(reinterpret_cast<float4*>(gvalue + o00), make_float4(s * g.x, s * g.y, s * g.z, s * g.w)); }
+  if (ya && xb) { float s = aw * w01; atomicAdd(reinterpret_cast<float4*>(gvalue + o01), make_float4(s * g.x, s * g.y, s * g.z, s * g.w)); }
+  if (yb && xa) { float s = aw * w10; atomicAdd(reinterpret_cast<float4*>(gvalue + o10), make_float4(s * g.x, s * g.y, s * g.z, s * g.w)); }
+  if (yb && xb) { float s = aw * w11; atomicAdd(reinterpret_cast<float4*>(gvalue + o11), make_float4(s * g.x, s * g.y, s * g.z, s * g.w)); }
+}
+
+// Reduce one sample's three partial sums over the LPI lanes of a sample group (xor butterfly: every lane ends with the
+// same bits).
+template <int LPI>
+__device__ __forceinline__ void reduce_sample(float& ga, float& gx, float& gy) {
+#pragma unroll
+  for (int s = LPI / 2; s > 0; s >>= 1) {
+    ga += __shfl_xor_sync(0xffffffffu, ga, s);
+    gx += __shfl_xor_sync(0xffffffffu, gx, s);
+    gy += __shfl_xor_sync(0xffffffffu, gy, s);
+  }
+}
+
+// Softmax backward, second pass: the lane that parked g_a_i for its samples (i = l * n + j, j = first, first + step, ...)
+// rewrites them as a_i (g_a_i - sdot).
+__device__ __forceinline__ void softmax_backward_rewrite(const float* __restrict__ lg, float* __restrict__ gl, int L, int n,
+                                                         int first, int step, float mx, float inv_sum, float sdot) {
+  for (int l = 0; l < L; ++l)
+    for (int j = first; j < n; j += step) {
+      const int i = l * n + j;
+      const float a = __expf(__ldg(lg + i) - mx) * inv_sum;
+      gl[i] = a * (gl[i] - sdot);
+    }
+}
+
+template <int DH, int SPLIT>
+__global__ void __launch_bounds__(256) tpv_cross_attn_backward_kernel(
+    const float* __restrict__ value, const long long* __restrict__ shapes, const long long* __restrict__ lsi,
+    const float* __restrict__ offsets, const float* __restrict__ logits, const float* __restrict__ uv,
+    const unsigned char* __restrict__ vis, const int* __restrict__ count, const float* __restrict__ gslots,
+    float* __restrict__ gvalue, float* __restrict__ goffsets, float* __restrict__ glogits, int N, int Nv, int Hd, int Q, int L,
+    int D) {
+  constexpr int LPI = DH / 4;
+  constexpr int LANES = LPI * SPLIT;
+  __shared__ Levels lv;
+  load_levels(lv, shapes, lsi, L);
+  long long t = blockIdx.x * (long long)blockDim.x + threadIdx.x;
+  long long item = t / LANES;
+  const int li = (int)(t % LANES);
+  const int lc = li % LPI, sg = li / LPI;
+  const long long n_items = (long long)Q * Hd;
+  const bool live = item < n_items;
+  if (!live) item = n_items - 1;   // keep the warp converged for the shuffles
+  const int h = (int)(item % Hd);
+  const int q = (int)(item / Hd);
+  const int pstride = Hd * DH;
+  const int LD = L * D;
+  const float* op = offsets + item * (long long)LD * 2;
+  const float* lg = logits + item * (long long)LD;
+  float* gop = goffsets + item * (long long)LD * 2;
+  float* glp = glogits + item * (long long)LD;
+  float mx, inv_sum;
+  softmax_stats<LANES>(lg, LD, li, mx, inv_sum);
+  // forward: slots = acc / max(cnt, 1)  ->  every camera's sample sees g / max(cnt, 1)
+  const float c = (float)max(__ldg(count + q), 1);
+  float4 g = __ldg(reinterpret_cast<const float4*>(gslots + item * DH + lc * 4));
+  g.x /= c; g.y /= c; g.z /= c; g.w /= c;
+  const long long vlane = (long long)h * DH + lc * 4;
+  float sdot = 0.f;   // sum over this sample group's samples of a_i g_a_i
+  for (int l = 0; l < L; ++l) {
+    const int Hl = lv.h[l], Wl = lv.w[l];
+    const float rw = 1.0f / (float)Wl, rh = 1.0f / (float)Hl;
+    const long long lstart = lv.start[l];
+    for (int d0 = 0; d0 < D; d0 += SPLIT) {   // uniform trip count over the warp: the shuffles below need every lane
+      const int d = d0 + sg;
+      float ga = 0.f, gx = 0.f, gy = 0.f, aw = 0.f;
+      if (d < D) {
+        const float2 o = __ldg(reinterpret_cast<const float2*>(op) + l * D + d);
+        aw = __expf(__ldg(lg + l * D + d) - mx) * inv_sum;
+        for (int cam = 0; cam < N; ++cam) {
+          if (!__ldg(vis + (long long)cam * Q + q)) continue;
+          const float2 r = __ldg(reinterpret_cast<const float2*>(uv + ((long long)cam * Q + q) * D * 2) + d);
+          bilinear4_adjoint(value, gvalue, ((long long)cam * Nv + lstart) * pstride + vlane, pstride, Hl, Wl, fmaf(o.x, rw, r.x),
+                            fmaf(o.y, rh, r.y), g, aw, live, ga, gx, gy);
+        }
+      }
+      reduce_sample<LPI>(ga, gx, gy);
+      if (d < D) {
+        sdot = fmaf(aw, ga, sdot);
+        if (live && lc == 0) {
+          reinterpret_cast<float2*>(gop)[l * D + d] = make_float2(aw * gx * rw, aw * gy * rh);
+          glp[l * D + d] = ga;
+        }
+      }
+    }
+  }
+#pragma unroll
+  for (int s = LPI; s < LANES; s <<= 1) sdot += __shfl_xor_sync(0xffffffffu, sdot, s);   // fold the sample groups
+  if (live && lc == 0) softmax_backward_rewrite(lg, glp, L, D, sg, SPLIT, mx, inv_sum, sdot);
+}
+
+template <int DH>
+__global__ void __launch_bounds__(256) tpv_self_attn_backward_kernel(
+    const float* __restrict__ value, const long long* __restrict__ shapes, const long long* __restrict__ lsi,
+    const float* __restrict__ offsets, const float* __restrict__ logits, const float* __restrict__ ref,
+    const float* __restrict__ gout, float* __restrict__ gvalue, float* __restrict__ goffsets, float* __restrict__ glogits, int Nv,
+    int Hd, int Q, int L, int P) {
+  constexpr int LPI = DH / 4;
+  __shared__ Levels lv;
+  load_levels(lv, shapes, lsi, L);
+  long long t = blockIdx.x * (long long)blockDim.x + threadIdx.x;
+  long long item = t / LPI;
+  const int lc = (int)(t % LPI);
+  const long long n_items = (long long)Q * Hd;
+  const bool live = item < n_items;
+  if (!live) item = n_items - 1;
+  const int h = (int)(item % Hd);
+  const int q = (int)(item / Hd);
+  const int pstride = Hd * DH;
+  const int LP = L * P;
+  const float* op = offsets + item * (long long)LP * 2;
+  const float* lg = logits + item * (long long)LP;
+  const float* rp = ref + (long long)q * LP * 2;
+  float* gop = goffsets + item * (long long)LP * 2;
+  float* glp = glogits + item * (long long)LP;
+  float mx, inv_sum;
+  softmax_stats<LPI>(lg, LP, lc, mx, inv_sum);
+  const float4 g = __ldg(reinterpret_cast<const float4*>(gout + item * DH + lc * 4));
+  const long long vlane = (long long)h * DH + lc * 4;
+  float sdot = 0.f;
+  for (int l = 0; l < L; ++l) {
+    const int Hl = lv.h[l], Wl = lv.w[l];
+    const float rw = 1.0f / (float)Wl, rh = 1.0f / (float)Hl;
+    const long long vofs = (long long)lv.start[l] * pstride + vlane;
+    for (int p = 0; p < P; ++p) {
+      const float2 r = __ldg(reinterpret_cast<const float2*>(rp) + l * P + p);
+      const float2 o = __ldg(reinterpret_cast<const float2*>(op) + l * P + p);
+      const float aw = __expf(__ldg(lg + l * P + p) - mx) * inv_sum;
+      float ga = 0.f, gx = 0.f, gy = 0.f;
+      bilinear4_adjoint(value, gvalue, vofs, pstride, Hl, Wl, fmaf(o.x, rw, r.x), fmaf(o.y, rh, r.y), g, aw, live, ga, gx, gy);
+      reduce_sample<LPI>(ga, gx, gy);
+      sdot = fmaf(aw, ga, sdot);
+      if (live && lc == 0) {
+        reinterpret_cast<float2*>(gop)[l * P + p] = make_float2(aw * gx * rw, aw * gy * rh);
+        glp[l * P + p] = ga;
+      }
+    }
+  }
+  if (live && lc == 0) softmax_backward_rewrite(lg, glp, L, P, 0, 1, mx, inv_sum, sdot);
+}
+
 // ---- A4 point_sampling (bevformer/utils.py:116-206) ---------------------------------------------------------
 // One thread per (camera, query, pillar point): fully coalesced uv / mask stores.  The projection uses plain fp32
 // mul/add in a fixed left-to-right order (no FMA contraction): `mask` generates index lists.  `vis` (any over the
@@ -704,6 +892,61 @@ extern "C" int so_tpv_self_attn_forward(const float* value, const int64_t* spati
                                         int32_t Hd, int32_t Dh, int32_t Q, int32_t L, int32_t P, void* stream) {
   return so_tpv_self_attn_forward_strided(value, spatial_shapes, level_start_index, offsets, logits, ref, out, Nv, Hd, Dh, Q, L, P,
                                           Hd * Dh, Hd * L * P * 2, Hd * L * P, stream);
+}
+
+// float4 rows of value / grad_value / the incoming gradient, float2 (x, y) pairs of offsets / grad_offsets
+static bool attn_backward_misaligned(const float* value, const float* offsets, const float* grad_in, const float* grad_value,
+                                     const float* grad_offsets) {
+  return ((reinterpret_cast<uintptr_t>(value) | reinterpret_cast<uintptr_t>(grad_in) | reinterpret_cast<uintptr_t>(grad_value)) & 15) ||
+         ((reinterpret_cast<uintptr_t>(offsets) | reinterpret_cast<uintptr_t>(grad_offsets)) & 7);
+}
+
+extern "C" int so_tpv_cross_attn_backward(const float* value, const int64_t* spatial_shapes, const int64_t* level_start_index,
+                                          const float* offsets, const float* logits, const float* uv, const uint8_t* vis,
+                                          const int32_t* count, const float* grad_slots, float* grad_value, float* grad_offsets,
+                                          float* grad_logits, int32_t N, int32_t Nv, int32_t Hd, int32_t Dh, int32_t Q, int32_t L,
+                                          int32_t D, void* stream) {
+  if (!value || !spatial_shapes || !level_start_index || !offsets || !logits || !uv || !vis || !count || !grad_slots ||
+      !grad_value || !grad_offsets || !grad_logits)
+    return SO_ERR_INVALID_ARG;
+  if (N < 1 || Nv < 1 || Hd < 1 || Q < 1 || L < 1 || D < 1) return SO_ERR_INVALID_ARG;
+  if (Dh != 16 && Dh != 32) return SO_ERR_UNSUPPORTED;
+  if (attn_backward_misaligned(value, offsets, grad_slots, grad_value, grad_offsets)) return SO_ERR_INVALID_ARG;
+  if (L > kMaxLevels) return SO_ERR_UNSUPPORTED;
+  cudaStream_t st = (cudaStream_t)stream;
+  const long long* shp = reinterpret_cast<const long long*>(spatial_shapes);
+  const long long* lsi = reinterpret_cast<const long long*>(level_start_index);
+  const int split = D >= 32 ? 4 : (D >= 16 ? 2 : 1);   // the forward's sample groups
+  long long threads = (long long)Q * Hd * (Dh / 4) * split;
+  unsigned grid = (unsigned)ceil_div64(threads, 256);
+#define SO_CROSS_BWD(DHV, SP) tpv_cross_attn_backward_kernel<DHV, SP><<<grid, 256, 0, st>>>(value, shp, lsi, offsets, logits, uv, vis, count, grad_slots, grad_value, grad_offsets, grad_logits, N, Nv, Hd, Q, L, D)
+  if (Dh == 16) { if (split == 4) SO_CROSS_BWD(16, 4); else if (split == 2) SO_CROSS_BWD(16, 2); else SO_CROSS_BWD(16, 1); }
+  else { if (split == 4) SO_CROSS_BWD(32, 4); else if (split == 2) SO_CROSS_BWD(32, 2); else SO_CROSS_BWD(32, 1); }
+#undef SO_CROSS_BWD
+  note_launch(1);
+  return check_launch();
+}
+
+extern "C" int so_tpv_self_attn_backward(const float* value, const int64_t* spatial_shapes, const int64_t* level_start_index,
+                                         const float* offsets, const float* logits, const float* ref, const float* grad_out,
+                                         float* grad_value, float* grad_offsets, float* grad_logits, int32_t Nv, int32_t Hd,
+                                         int32_t Dh, int32_t Q, int32_t L, int32_t P, void* stream) {
+  if (!value || !spatial_shapes || !level_start_index || !offsets || !logits || !ref || !grad_out || !grad_value ||
+      !grad_offsets || !grad_logits)
+    return SO_ERR_INVALID_ARG;
+  if (Nv < 1 || Hd < 1 || Q < 1 || L < 1 || P < 1) return SO_ERR_INVALID_ARG;
+  if (Dh != 16 && Dh != 32) return SO_ERR_UNSUPPORTED;
+  if (attn_backward_misaligned(value, offsets, grad_out, grad_value, grad_offsets)) return SO_ERR_INVALID_ARG;
+  if (L > kMaxLevels) return SO_ERR_UNSUPPORTED;
+  cudaStream_t st = (cudaStream_t)stream;
+  const long long* shp = reinterpret_cast<const long long*>(spatial_shapes);
+  const long long* lsi = reinterpret_cast<const long long*>(level_start_index);
+  long long threads = (long long)Q * Hd * (Dh / 4);
+  unsigned grid = (unsigned)ceil_div64(threads, 256);
+  SO_DISPATCH_DH(Dh, (tpv_self_attn_backward_kernel<16><<<grid, 256, 0, st>>>(value, shp, lsi, offsets, logits, ref, grad_out, grad_value, grad_offsets, grad_logits, Nv, Hd, Q, L, P)),
+                 (tpv_self_attn_backward_kernel<32><<<grid, 256, 0, st>>>(value, shp, lsi, offsets, logits, ref, grad_out, grad_value, grad_offsets, grad_logits, Nv, Hd, Q, L, P)));
+  note_launch(1);
+  return check_launch();
 }
 
 extern "C" int so_visible_index_lists(const uint8_t* mask, int32_t N, int32_t Q, int32_t D, int64_t* index_lists, int32_t* lens,

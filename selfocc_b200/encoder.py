@@ -10,9 +10,13 @@ The arithmetic of the hot ops runs in ``libselfocc_b200.so``:
   ``ops.tpv_cross_attn_forward*``); every dense projection (value / offset / weight / output Linear, FFN) runs on
   the wgmma split-precision GEMM (``ops.linear_3xtf32``, fp32-level accuracy), projections of the same input are
   fused into one GEMM; LayerNorm is a warp-per-row kernel (``ops.layer_norm``);
-* training (autograd): the mmcv-contract op ``ops.MultiScaleDeformableAttnFunction`` (forward +
-  backward kernels) fed by torch softmax / location arithmetic, visible-query lists compacted on the
-  device (``ops.visible_index_lists``); the projections stay ``nn.Linear`` (cuBLAS) on this path.
+* training (autograd), batch 1: the same fused attention cores with their backward kernels
+  (``ops.TPVSelfAttnFunction`` / ``ops.TPVCrossAttnFunction``: no host sync, no padded rebatch, no
+  sampling-location tensor); the projections run forward and input gradient on the wgmma GEMM
+  (``train_linear``), the weight gradients on cuBLAS;
+* batch > 1 or a ``key_padding_mask``: the reference's formulation, the mmcv-contract op
+  ``ops.MultiScaleDeformableAttnFunction`` fed by torch softmax / location arithmetic, with the image
+  cross-attention's rebatch built from device-compacted index lists (``ops.visible_index_lists``).
 """
 import copy
 import math
@@ -228,6 +232,10 @@ def _needs_grad(*tensors):
     return torch.is_grad_enabled() and any(t is not None and t.requires_grad for t in tensors)
 
 
+def _cuda_fp32(*tensors):
+    return all(t.is_cuda and t.dtype == torch.float32 for t in tensors)
+
+
 @MODELS.register_module()
 class CrossViewHybridAttention(_DeformBase):
     """A8.  cross_view_hybrid_attention.py:11-124 (subclass of mmcv MultiScaleDeformableAttention whose
@@ -285,6 +293,16 @@ class CrossViewHybridAttention(_DeformBase):
                 out = fast_linear(self.output_proj, out, residual=idt, ln=fuse_norm)
                 self.fused_norm_applied = fuse_norm is not None
             return out[None] if self.batch_first else out[:, None]
+        if bs == 1 and key_padding_mask is None and _cuda_fp32(query, value):
+            # training: the same fused core with its backward kernel; projections on the autograd GEMM
+            v = train_linear(self.value_proj, value[0]).view(num_value, Hd, -1)
+            offsets = train_linear(self.sampling_offsets, query[0]).view(num_query, Hd, L, P, 2)
+            logits = train_linear(self.attention_weights, query[0]).view(num_query, Hd, L, P)
+            ref = reference_points[0] if reference_points.dim() == 5 else reference_points
+            out = ops.TPVSelfAttnFunction.apply(v, spatial_shapes, level_start_index, offsets, logits, ref)
+            out = train_linear(self.output_proj, out)
+            out = out[None] if self.batch_first else out[:, None]
+            return self.dropout(out) + identity
         value = train_linear(self.value_proj, value)
         if key_padding_mask is not None:
             value = value.masked_fill(key_padding_mask[..., None], 0.0)
@@ -346,8 +364,9 @@ class BEVDeformableAttention(_DeformBase):
 
 @MODELS.register_module()
 class BEVCrossAttention(nn.Module):
-    """A5.  image_cross_attention.py:11-139.  Inference runs the rebatch-free fused core; with autograd
-    the reference's rebatch is reproduced with device-compacted index lists."""
+    """A5.  image_cross_attention.py:11-139.  Batch 1 runs the rebatch-free fused core, with autograd through
+    its backward kernel; batch > 1 or a key_padding_mask reproduce the reference's rebatch with
+    device-compacted index lists."""
 
     def __init__(self, embed_dims=256, num_cams=6, dropout=0.1, init_cfg=None, batch_first=True,
                  deformable_attention=dict(type='BEVDeformableAttention', embed_dims=256, num_levels=4), **kwargs):
@@ -400,6 +419,18 @@ class BEVCrossAttention(nn.Module):
             self.fused_norm_applied = fuse_norm is not None
             return fast_linear(self.output_proj, slots, residual=residual[0], out=out_rows, ln=fuse_norm)[None]
         self.fused_norm_applied = False
+        if bs == 1 and kwargs.get('key_padding_mask') is None and _cuda_fp32(query, value):
+            # training: the rebatch-free core with its backward kernel (no host sync, no padded per-camera copies)
+            n_cam, nv = value.shape[0], value.shape[1]
+            if bev_vis is None:
+                bev_vis = (bev_masks[:, 0].sum(-1) > 0).to(torch.uint8)
+            v = train_linear(da.value_proj, value[:, :, 0]).view(n_cam, nv, Hd, -1)
+            offsets = train_linear(da.sampling_offsets, query[0]).view(num_query, Hd, L, D, 2)
+            logits = train_linear(da.attention_weights, query[0]).view(num_query, Hd, L, D)
+            slots = ops.TPVCrossAttnFunction.apply(v, spatial_shapes, level_start_index, offsets, logits,
+                                                   reference_points_cams[:, 0], bev_vis)
+            slots = train_linear(self.output_proj, slots)
+            return self.dropout(slots)[None] + residual
         slots = self._rebatch_forward(query, value, spatial_shapes, reference_points_cams, bev_masks, level_start_index)
         slots = train_linear(self.output_proj, slots)
         return self.dropout(slots) + residual

@@ -260,6 +260,82 @@ def tpv_self_attn_forward(value, spatial_shapes, level_start_index, offsets, log
     return out
 
 
+def tpv_cross_attn_backward(value, spatial_shapes, level_start_index, offsets, logits, uv, vis, count, grad_slots):
+    """Backward of tpv_cross_attn_forward: grad_slots [Q,Hd*Dh] -> (grad_value, grad_offsets, grad_logits), shaped like
+    value, offsets, logits.  count: the forward's int32 [Q] visible-camera count."""
+    lib = _lib.load()
+    for n, t in (('value', value), ('offsets', offsets), ('logits', logits), ('uv', uv), ('grad_slots', grad_slots)):
+        _chk(t, name=n)
+    _chk(vis, torch.uint8, 'vis'); _chk(count, torch.int32, 'count')
+    _chk(spatial_shapes, torch.int64, 'spatial_shapes'); _chk(level_start_index, torch.int64, 'level_start_index')
+    N, Nv, Hd, Dh = value.shape
+    Q, _, L, D, _ = offsets.shape
+    gv = torch.zeros_like(value)
+    go = torch.empty_like(offsets)
+    gl = torch.empty_like(logits)
+    _lib.check(lib.so_tpv_cross_attn_backward(_p(value), _p(spatial_shapes), _p(level_start_index), _p(offsets), _p(logits), _p(uv),
+                                              _p(vis), _p(count), _p(grad_slots), _p(gv), _p(go), _p(gl), N, Nv, Hd, Dh, Q, L, D,
+                                              _stream()), 'so_tpv_cross_attn_backward')
+    return gv, go, gl
+
+
+def tpv_self_attn_backward(value, spatial_shapes, level_start_index, offsets, logits, ref, grad_out):
+    """Backward of tpv_self_attn_forward: grad_out [Q,Hd*Dh] -> (grad_value, grad_offsets, grad_logits)."""
+    lib = _lib.load()
+    for n, t in (('value', value), ('offsets', offsets), ('logits', logits), ('ref', ref), ('grad_out', grad_out)):
+        _chk(t, name=n)
+    _chk(spatial_shapes, torch.int64, 'spatial_shapes'); _chk(level_start_index, torch.int64, 'level_start_index')
+    Nv, Hd, Dh = value.shape
+    Q, _, L, P, _ = offsets.shape
+    gv = torch.zeros_like(value)
+    go = torch.empty_like(offsets)
+    gl = torch.empty_like(logits)
+    _lib.check(lib.so_tpv_self_attn_backward(_p(value), _p(spatial_shapes), _p(level_start_index), _p(offsets), _p(logits), _p(ref),
+                                             _p(grad_out), _p(gv), _p(go), _p(gl), Nv, Hd, Dh, Q, L, P, _stream()),
+               'so_tpv_self_attn_backward')
+    return gv, go, gl
+
+
+class TPVCrossAttnFunction(torch.autograd.Function):
+    """The rebatch-free image cross-attention core with autograd: (value [N,Nv,Hd,Dh], spatial_shapes, level_start_index,
+    offsets [Q,Hd,L,D,2], logits [Q,Hd,L,D], uv [N,Q,D,2], vis uint8 [N,Q]) -> slots [Q,Hd*Dh].  Forward is the inference
+    kernel; backward recomputes the sampling set-up.  uv, vis and the level tables are constants (the reference projects the
+    pillars with fixed tables and numpy metas), so they get no gradient."""
+
+    @staticmethod
+    def forward(ctx, value, spatial_shapes, level_start_index, offsets, logits, uv, vis):
+        value, offsets, logits, uv, vis = (t.contiguous() for t in (value, offsets, logits, uv, vis))
+        slots, count = tpv_cross_attn_forward(value, spatial_shapes, level_start_index, offsets, logits, uv, vis, want_count=True)
+        ctx.save_for_backward(value, spatial_shapes, level_start_index, offsets, logits, uv, vis, count)
+        return slots
+
+    @staticmethod
+    @torch.autograd.function.once_differentiable
+    def backward(ctx, grad_slots):
+        value, ss, lsi, offsets, logits, uv, vis, count = ctx.saved_tensors
+        gv, go, gl = tpv_cross_attn_backward(value, ss, lsi, offsets, logits, uv, vis, count, grad_slots.contiguous())
+        return gv, None, None, go, gl, None, None
+
+
+class TPVSelfAttnFunction(torch.autograd.Function):
+    """The fused cross-view hybrid (self) attention core with autograd: (value [Nv,Hd,Dh], spatial_shapes, level_start_index,
+    offsets [Q,Hd,L,P,2], logits [Q,Hd,L,P], ref [Q,L,P,2]) -> out [Q,Hd*Dh].  ref and the level tables get no gradient."""
+
+    @staticmethod
+    def forward(ctx, value, spatial_shapes, level_start_index, offsets, logits, ref):
+        value, offsets, logits, ref = (t.contiguous() for t in (value, offsets, logits, ref))
+        out = tpv_self_attn_forward(value, spatial_shapes, level_start_index, offsets, logits, ref)
+        ctx.save_for_backward(value, spatial_shapes, level_start_index, offsets, logits, ref)
+        return out
+
+    @staticmethod
+    @torch.autograd.function.once_differentiable
+    def backward(ctx, grad_out):
+        value, ss, lsi, offsets, logits, ref = ctx.saved_tensors
+        gv, go, gl = tpv_self_attn_backward(value, ss, lsi, offsets, logits, ref, grad_out.contiguous())
+        return gv, None, None, go, gl, None
+
+
 # --------------------------------------------------------------------------------------- training form (B6-B10, B13)
 def _render_ws(lib, rays, dev):
     total = rays.n_cam * rays.rays_per_cam
