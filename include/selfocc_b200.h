@@ -28,8 +28,8 @@ extern "C" {
 #define SO_ERR_CUDA (-3)          /* a CUDA runtime call or launch failed; see so_last_cuda_error */
 #define SO_ERR_NO_DEVICE (-4)
 
-#define SO_ABI_VERSION 4   /* 2: so_render_train_forward gained pair_workspace; 3: packed render volume entry points;
-                              4: backward of the fused attention cores */
+#define SO_ABI_VERSION 5   /* 2: so_render_train_forward gained pair_workspace; 3: packed render volume entry points;
+                              4: backward of the fused attention cores; 5: the colour pack holds the SH-0 colour */
 
 /* ABI version of the loaded library (compare with SO_ABI_VERSION). */
 int so_abi_version(void);
@@ -161,7 +161,10 @@ int so_render_infer(const float* vol_sdf, const float* vol_feat, const so_volume
  * render wants (built by NeuSHead.prepare, reused by every render of the frame -- eval_novel_depth.py:143-172 renders
  * several poses per prepare):
  *   n_feat == 0 : float2 [H][W][zpitch] {sdf[z], sdf[z+1]}  -- the 8 trilinear taps become 4 aligned 64-bit loads
- *   n_feat == 3 : float4 [H][W][Z]      {r, g, b, sdf}       -- 8 aligned 128-bit loads fetch sdf and colour together
+ *   n_feat == 3 : float4 [H][W][Z]      {C0 r + 0.5, C0 g + 0.5, C0 b + 0.5, sdf}, C0 = 0.28209479177387814 (SH degree 0)
+ *                 -- 8 aligned 128-bit loads fetch sdf and colour together.  The colour lanes hold the SH-0 colour before
+ *                 its relu (one fmaf per channel), not the decoded features: trilinear weights sum to one, so the map
+ *                 commutes with the interpolation and the render applies only the relu.  The sdf lane is the decoded sdf.
  * so_render_pack_floats: floats needed (0: this channel count has no packed form).  pack must be 16-byte aligned. */
 int64_t so_render_pack_floats(const so_volume_desc* vol_host);
 int so_render_pack(const float* vol_sdf, const float* vol_feat, const so_volume_desc* vol_host, float* pack, void* stream);

@@ -4,23 +4,32 @@
 //
 //  * the decoded volume is first repacked once per frame (so_render_pack) into the layout the gather wants:
 //      n_feat == 0 : float2 [H][W][zpitch]  {sdf[z], sdf[z+1]}     -> the 8 trilinear taps are 4 aligned 64-bit loads
-//      n_feat == 3 : float4 [H][W][Z]       {r, g, b, sdf}          -> 8 aligned 128-bit loads fetch sdf AND colour
-//    (the reference gathers 8 + 24 scalars per sample for colour, bev_nerf.py:99-117);
-//  * the trilinear interpolation works on register pairs: the two lanes of a loaded pair are lerped together, the sdf
-//    gradient falls out of the lerp differences;
+//      n_feat == 3 : float4 [H][W][Z]       {C0 r + 1/2, C0 g + 1/2, C0 b + 1/2, sdf}
+//                                                                   -> 8 aligned 128-bit loads fetch sdf AND colour
+//    (the reference gathers 8 + 24 scalars per sample for colour, bev_nerf.py:99-117; the SH-0 colour map is affine, so
+//    it is applied once per voxel in the pack and the loop keeps only the relu);
+//  * the interior loop is scalar FP32 (sm_90 has no packed fp32x2 pipe): only the sdf is lerped with its gradient terms
+//    (the gradient falls out of the lerp differences); r, g, b take one shared set of 8 trilinear weights;
 //  * "all 8 corners inside the volume" is decided ONCE per ray: for the affine metre->grid map g(t) = g0 + gd * t is
 //    monotone along the ray (so is its fp32 evaluation fma(gd, t, g0)), so if the first and the last sample are interior,
 //    every sample is; warps with a non-interior ray take the general zero-padding loop;
 //  * NeuS alpha with ONE reciprocal:  alpha = (omen + c (1 + B)) / ((1 + B) (1 + c)),  A = e^-(s-h), B = e^(s+h),
-//    c = 1e-5 (1 + A)  (algebraically equal to (Phi(prev) - Phi(next) + 1e-5) / (Phi(prev) + 1e-5), no cancellation);
+//    c = 1e-5 (1 + A)  (algebraically equal to (Phi(prev) - Phi(next) + 1e-5) / (Phi(prev) + 1e-5), no cancellation),
+//    and in the interior loop two exponentials: omen = 1 - e^-x = 1 - A B;
+//  * with colour, a lane keeps its last cell's corners in registers and reloads only when its cell changes;
 //  * cell indices come from the float floor through the 2^23 magic add (integer pipe) instead of F2I (XU pipe);
 //  * a warp stops marching once every ray's transmittance is below 1e-9: the dropped tail changes acc / depth / rgb by
 //    < 1e-9 relative and cannot hold the max-depth argmax (a later w is <= T < 1e-9 <= max_s w_s since sum_s w_s >= 1 - T).
 #include "render_common.cuh"
 
-// Tuning knobs, timed on an H100 SXM (400 W) with scripts/bench_render.py, analytic scene, 8.64 M rays, depth-only / colour
-// ms: defaults (unroll 4; 6 / 4 CTAs per SM) 6.93-7.18 / 12.06-12.12 over two runs; unroll 1 7.27 / 12.08, unroll 2
-// 7.04 / 12.18; 4 / 3 CTAs 6.98 / 12.14; 8 / 5 CTAs 6.92 / 12.12.  No alternative beats the run-to-run spread.
+// Tuning knobs, timed on an H100 80GB HBM3 (400 W) with scripts/bench_render.py, analytic scene, 8.64 M rays, depth-only /
+// colour ms, before the scalar rewrite: defaults (unroll 4; 6 / 4 CTAs per SM) 6.93-7.18 / 12.06-12.12 over two runs;
+// unroll 1 7.27 / 12.08, unroll 2 7.04 / 12.18; 4 / 3 CTAs 6.98 / 12.14; 8 / 5 CTAs 6.92 / 12.12.  After it (same card and
+// limit, one session): previous kernel 6.94 / 12.10; cell cache in both kernels 6.74 / 10.81; in neither 6.54 / 11.51.
+// bench.py render per step agrees: with the cache depth-only 9.84 / 9.70 vs 9.40 / 9.28 without, colour 15.35 / 15.33 vs
+// 16.04 / 15.95 (previous kernel 10.13 / 10.16 and 16.60 / 16.53).  So the cache is on for the colour kernel, whose 8
+// 128-bit corner loads it saves, and off for the depth-only one, whose 4 64-bit loads cost less than the vote and the
+// register-held corners.  Unroll, CTAs per SM and the exit period were not re-timed after the rewrite.
 #ifndef SO_RF_BLOCK
 #define SO_RF_BLOCK 128
 #endif
@@ -32,6 +41,12 @@
 #endif
 #ifndef SO_RF_UNROLL
 #define SO_RF_UNROLL 4
+#endif
+#ifndef SO_RF_CELL_CACHE
+#define SO_RF_CELL_CACHE 0      // depth-only: keep the last cell's corners in registers (0: load them every sample)
+#endif
+#ifndef SO_RF_CELL_CACHE_RGB
+#define SO_RF_CELL_CACHE_RGB 1  // the same for the colour kernel
 #endif
 #ifndef SO_RF_EXIT_T
 #define SO_RF_EXIT_T 1e-9f
@@ -56,16 +71,13 @@ struct RayGeo {        // per-ray constants of the affine march (grid units)
   float k_log2;
 };
 
-__device__ __forceinline__ float2 f2(float a, float b) { return make_float2(a, b); }
-__device__ __forceinline__ float2 bc2(float a) { return make_float2(a, a); }
-// two-lane helpers: one rounded fmaf / add per lane (sm_90 has no packed fp32x2 pipe; the results are the same)
-__device__ __forceinline__ float2 fma2(float2 a, float2 b, float2 c) { return make_float2(fmaf(a.x, b.x, c.x), fmaf(a.y, b.y, c.y)); }
-__device__ __forceinline__ float2 add2(float2 a, float2 b) { return make_float2(a.x + b.x, a.y + b.y); }
-__device__ __forceinline__ float2 sub2(float2 a, float2 b) { return fma2(b, make_float2(-1.f, -1.f), a); }   // a - b, exact
-__device__ __forceinline__ float2 lerp2(float2 t, float2 d, float2 a) { return fma2(t, d, a); }               // a + t * d
-
 // NeuS alpha, one-reciprocal form (see the file header).  s2 = sdf * inv_s * log2(e), h2 = half * inv_s * log2(e) <= 0.
 // The exponents are clamped at 64: beyond that alpha is 1 (A huge) or the 1e-5 floor (B huge) to within 2^-40.
+// kTwoExp (interior loop): e^-x = 2^(2 h2) = A B whenever neither exponent is clamped, so omen needs no third
+// exponential.  A clamped A or B makes A B smaller than e^-x, but then alpha is 1 (resp. the 1e-5 floor) to within 2^-40
+// whatever omen is; A B <= 1 always (the exponents sum to 2 h2 <= 0 and cannot both exceed 64), so omen stays in [0, 1].
+// A flushed A or B means e^-x < 2^-62, where 1 - e^-x rounds to 1 anyway.
+template <bool kTwoExp>
 __device__ __forceinline__ float neus_alpha_rcp1(float s2, float h2) {
   float A = exp2f(fminf(h2 - s2, 64.f));
   float B = exp2f(fminf(s2 + h2, 64.f));
@@ -73,7 +85,7 @@ __device__ __forceinline__ float neus_alpha_rcp1(float s2, float h2) {
   float c = fmaf(A, 1e-5f, 1e-5f);                               // 1e-5 (1 + A)
   float x = h2 * (-2.0f * 0.6931471805599453f);                  // (s - h) - (s + h) in natural units, >= 0
   float ser = x * fmaf(x, fmaf(x, fmaf(x, fmaf(x, 1.0f / 120.0f, -1.0f / 24.0f), 1.0f / 6.0f), -0.5f), 1.0f);
-  float omen = x < 0.125f ? ser : 1.0f - exp2f(h2 + h2);         // 1 - e^-x
+  float omen = x < 0.125f ? ser : (kTwoExp ? fmaf(-A, B, 1.0f) : 1.0f - exp2f(h2 + h2));   // 1 - e^-x
   float num = fmaf(c, pB, omen);
   float den = fmaf(pB, c, pB);
   return __saturatef(__fdividef(num, den));
@@ -104,7 +116,7 @@ __device__ __noinline__ void march_padded(const VolumeDev& V, const RayGeo& G, i
     float sdf, dgh, dgw, dgd;
     gather_sdf(V, t, sdf, dgh, dgw, dgd);
     float tc = fmaf(G.gdh, dgh, fmaf(G.gdw, dgw, G.gdd * dgd));
-    float alpha = neus_alpha_rcp1(sdf * G.k_log2, fminf(tc, 0.f) * G.h_const);
+    float alpha = neus_alpha_rcp1<false>(sdf * G.k_log2, fminf(tc, 0.f) * G.h_const);
     float w;
     composite(a, alpha, mid, dgw * G.kw, dgh * G.kh, dgd * G.kd, s, w);
     if (RGB) {
@@ -173,81 +185,97 @@ render_packed_kernel(VolumeDev V, const void* __restrict__ pack, RayDev R, Rende
   if (!__all_sync(kFull, inside)) {
     march_padded<RGB>(V, G, S, P.sh_act, valid ? dbg_ray : nullptr, a);
   } else {
-    const float2 span2 = bc2(G.span), tn2 = bc2(tn), step2 = bc2(G.step);
-    const float2 gdhw = f2(G.gdh, G.gdw), ghw0 = f2(G.gh0, G.gw0), magic2 = bc2(kMagic);
-    float2 bm2 = bc2(bm_first);
     const unsigned zp = ZP ? ZP : (RGB ? V.Z : V.zpitch), wz = WZ ? WZ : V.W * zp;
+    // Address of the cell's (h0, w0, z0) corner.  With compile-time pitches the element index goes through fp32: every
+    // partial sum is an integer below 2^24 (the launcher checks H * W * Z <= 2^23), so both FFMAs are exact and the float's
+    // bits are 0x4B000000 + index.  Otherwise the index is formed on the integer
+    // pipe from the magic-added floors (kcorr removes their 0x4B000000s, modulo 2^32).
+    const unsigned kIdx0 = ZP ? kMagicBits : 0u;
     const unsigned kcorr = 0u - kMagicBits * (wz + zp + 1u);
+    // The last cell's corners (and the differences that depend on the cell only) stay in registers: a lane reloads
+    // when its cell changes, the warp branches over the reload when no lane's cell did.  `cell` starts at a key no
+    // cell has (0x4B000000 + index < 0x4C000000 on the fp32 path; the pack holds fewer than 2^32 - 1 elements).
+    constexpr bool kCache = (RGB ? SO_RF_CELL_CACHE_RGB : SO_RF_CELL_CACHE) != 0;
+    unsigned cell = 0xffffffffu;
+    float4 k[8];                         // RGB: corners {r, g, b, sdf}, order (h, w, z) = 000 001 010 011 100 101 110 111
+    float dz[4] = {}, ddz0 = 0.f, ddz1 = 0.f;   // RGB: sdf differences along z per (h, w) column, and their w-differences
+    float2 a00, a10, e0, e1, ee;         // depth-only: z-pairs at (h0, w0) / (h1, w0), their w-differences, e1 - e0
+#pragma unroll
+    for (int i = 0; i < 8; ++i) k[i] = make_float4(0.f, 0.f, 0.f, 0.f);
+    a00 = a10 = e0 = e1 = ee = make_float2(0.f, 0.f);
+    float bm = bm_first;
     constexpr int kUnroll = SO_RF_UNROLL;
 #pragma unroll kUnroll
     for (int s = 0; s < S; ++s) {
-      const float2 mid2 = fma2(bm2, span2, tn2);
-      bm2 = add2(bm2, step2);
-      const float mid = mid2.x;
-      const float2 ghw = fma2(gdhw, mid2, ghw0);
-      const float gd = fmaf(G.gdd, mid, G.gd0);
-      if (DBG) { dbg_ray[3 * s] = ghw.x; dbg_ray[3 * s + 1] = ghw.y; dbg_ray[3 * s + 2] = gd; }
-      const float flh = floorf(ghw.x), flw = floorf(ghw.y), flz = floorf(gd);
-      const float2 fhw = sub2(ghw, f2(flh, flw));
-      const float fz = gd - flz;
-      const float2 rhw = add2(f2(flh, flw), magic2);
+      const float mid = fmaf(bm, G.span, tn);
+      bm += G.step;
+      const float gh = fmaf(G.gdh, mid, G.gh0), gw = fmaf(G.gdw, mid, G.gw0), gd = fmaf(G.gdd, mid, G.gd0);
+      if (DBG) { dbg_ray[3 * s] = gh; dbg_ray[3 * s + 1] = gw; dbg_ray[3 * s + 2] = gd; }
+      const float flh = floorf(gh), flw = floorf(gw), flz = floorf(gd);
+      const float fh = gh - flh, fw = gw - flw, fz = gd - flz;
       const float rz = flz + kMagic;
-      const unsigned idx = __float_as_uint(rhw.x) * wz + (__float_as_uint(rhw.y) * zp + (__float_as_uint(rz) + kcorr));
-      const float2 fh2 = bc2(fhw.x), fw2 = bc2(fhw.y);
+      unsigned idx;
+      if (ZP) idx = __float_as_uint(fmaf(flh, (float)WZ, fmaf(flw, (float)ZP, rz)));
+      else idx = __float_as_uint(flh + kMagic) * wz + (__float_as_uint(flw + kMagic) * zp + (__float_as_uint(rz) + kcorr));
+      if (!kCache || __any_sync(kFull, idx != cell)) {
+        if (!kCache || idx != cell) {
+          cell = idx;
+          if (!RGB) {
+            const float2* p = reinterpret_cast<const float2*>(pack) + (idx - kIdx0);
+            a00 = __ldg(p); a10 = __ldg(p + wz);
+            const float2 a01 = __ldg(p + zp), a11 = __ldg(p + wz + zp);
+            e0 = make_float2(a01.x - a00.x, a01.y - a00.y);
+            e1 = make_float2(a11.x - a10.x, a11.y - a10.y);
+            ee = make_float2(e1.x - e0.x, e1.y - e0.y);
+          } else {
+            const float4* p = reinterpret_cast<const float4*>(pack) + (idx - kIdx0);
+            k[0] = __ldg(p); k[1] = __ldg(p + 1); k[2] = __ldg(p + zp); k[3] = __ldg(p + zp + 1);
+            k[4] = __ldg(p + wz); k[5] = __ldg(p + wz + 1); k[6] = __ldg(p + wz + zp); k[7] = __ldg(p + wz + zp + 1);
+#pragma unroll
+            for (int j = 0; j < 4; ++j) dz[j] = k[2 * j + 1].w - k[2 * j].w;
+            ddz0 = dz[1] - dz[0]; ddz1 = dz[3] - dz[2];
+          }
+        }
+      }
       float sdf, dgh, dgw, dgd;
-      float2 rg;
-      float bl;
       if (!RGB) {
-        const float2* p = reinterpret_cast<const float2*>(pack) + idx;
-        const float2 a00 = __ldg(p), a01 = __ldg(p + zp), a10 = __ldg(p + wz), a11 = __ldg(p + wz + zp);
-        // lanes = (z0, z1): lerp along w, then h, with both lanes at once; z last
-        const float2 e0 = sub2(a01, a00), e1 = sub2(a11, a10);
-        const float2 c0 = lerp2(fw2, e0, a00), c1 = lerp2(fw2, e1, a10);
-        const float2 dh = sub2(c1, c0);
-        const float2 c = lerp2(fh2, dh, c0);
-        const float2 e = lerp2(fh2, sub2(e1, e0), e0);
-        dgd = c.y - c.x;
-        sdf = fmaf(fz, dgd, c.x);
+        // lanes = (z0, z1): lerp along w, then h, both lanes; z last
+        const float2 c0 = make_float2(fmaf(fw, e0.x, a00.x), fmaf(fw, e0.y, a00.y));
+        const float2 c1 = make_float2(fmaf(fw, e1.x, a10.x), fmaf(fw, e1.y, a10.y));
+        const float2 dh = make_float2(c1.x - c0.x, c1.y - c0.y);
+        const float c_x = fmaf(fh, dh.x, c0.x), c_y = fmaf(fh, dh.y, c0.y);
+        const float e_x = fmaf(fh, ee.x, e0.x), e_y = fmaf(fh, ee.y, e0.y);
+        dgd = c_y - c_x;
+        sdf = fmaf(fz, dgd, c_x);
         dgh = fmaf(fz, dh.y - dh.x, dh.x);
-        dgw = fmaf(fz, e.y - e.x, e.x);
+        dgw = fmaf(fz, e_y - e_x, e_x);
       } else {
-        const float4* p = reinterpret_cast<const float4*>(pack) + idx;
-        const float4 q000 = __ldg(p), q001 = __ldg(p + 1), q010 = __ldg(p + zp), q011 = __ldg(p + zp + 1);
-        const float4 q100 = __ldg(p + wz), q101 = __ldg(p + wz + 1), q110 = __ldg(p + wz + zp), q111 = __ldg(p + wz + zp + 1);
-        const float2 fz2 = bc2(fz);
-        // lanes lo = (r, g), hi = (b, sdf): lerp along z, w, h
-#define SO_LO(q) f2((q).x, (q).y)
-#define SO_HI(q) f2((q).z, (q).w)
-        const float2 dz00l = sub2(SO_LO(q001), SO_LO(q000)), dz00h = sub2(SO_HI(q001), SO_HI(q000));
-        const float2 dz01l = sub2(SO_LO(q011), SO_LO(q010)), dz01h = sub2(SO_HI(q011), SO_HI(q010));
-        const float2 dz10l = sub2(SO_LO(q101), SO_LO(q100)), dz10h = sub2(SO_HI(q101), SO_HI(q100));
-        const float2 dz11l = sub2(SO_LO(q111), SO_LO(q110)), dz11h = sub2(SO_HI(q111), SO_HI(q110));
-        const float2 t00l = lerp2(fz2, dz00l, SO_LO(q000)), t00h = lerp2(fz2, dz00h, SO_HI(q000));
-        const float2 t01l = lerp2(fz2, dz01l, SO_LO(q010)), t01h = lerp2(fz2, dz01h, SO_HI(q010));
-        const float2 t10l = lerp2(fz2, dz10l, SO_LO(q100)), t10h = lerp2(fz2, dz10h, SO_HI(q100));
-        const float2 t11l = lerp2(fz2, dz11l, SO_LO(q110)), t11h = lerp2(fz2, dz11h, SO_HI(q110));
-#undef SO_LO
-#undef SO_HI
-        const float2 dw0l = sub2(t01l, t00l), dw0h = sub2(t01h, t00h), dw1l = sub2(t11l, t10l), dw1h = sub2(t11h, t10h);
-        const float2 u0l = lerp2(fw2, dw0l, t00l), u0h = lerp2(fw2, dw0h, t00h);
-        const float2 u1l = lerp2(fw2, dw1l, t10l), u1h = lerp2(fw2, dw1h, t10h);
-        const float2 dhl = sub2(u1l, u0l), dhh = sub2(u1h, u0h);
-        const float2 vl = lerp2(fh2, dhl, u0l), vh = lerp2(fh2, dhh, u0h);
-        rg = vl; bl = vh.x; sdf = vh.y;
-        dgh = dhh.y;
-        dgw = fmaf(fhw.x, dw1h.y - dw0h.y, dw0h.y);
-        const float dzw0 = fmaf(fhw.y, dz01h.y - dz00h.y, dz00h.y), dzw1 = fmaf(fhw.y, dz11h.y - dz10h.y, dz10h.y);
-        dgd = fmaf(fhw.x, dzw1 - dzw0, dzw0);
+        // sdf: lerp along z, w, h; the gradient from the lerp differences
+        const float c00 = fmaf(fz, dz[0], k[0].w), c01 = fmaf(fz, dz[1], k[2].w);
+        const float c10 = fmaf(fz, dz[2], k[4].w), c11 = fmaf(fz, dz[3], k[6].w);
+        const float dw0 = c01 - c00, dw1 = c11 - c10;
+        const float u0 = fmaf(fw, dw0, c00), u1 = fmaf(fw, dw1, c10);
+        dgh = u1 - u0;
+        sdf = fmaf(fh, dgh, u0);
+        dgw = fmaf(fh, dw1 - dw0, dw0);
+        const float dzw0 = fmaf(fw, ddz0, dz[0]), dzw1 = fmaf(fw, ddz1, dz[2]);
+        dgd = fmaf(fh, dzw1 - dzw0, dzw0);
       }
       const float tc = fmaf(G.gdh, dgh, fmaf(G.gdw, dgw, G.gdd * dgd));     // direction . d sdf / d metre
-      const float alpha = neus_alpha_rcp1(sdf * G.k_log2, fminf(tc, 0.f) * G.h_const);
+      const float alpha = neus_alpha_rcp1<true>(sdf * G.k_log2, fminf(tc, 0.f) * G.h_const);
       float w;
       composite(a, alpha, mid, dgw * G.kw, dgh * G.kh, dgd * G.kd, s, w);
       if (RGB) {
-        // SH degree 0, relu activation (sh_render.py:84-94); the launcher routes sh_act != 0 to the general kernel
-        const float2 c2 = fma2(rg, bc2(kC0), bc2(0.5f));
-        const float r0 = fmaxf(c2.x, 0.f), r1 = fmaxf(c2.y, 0.f), r2 = fmaxf(fmaf(bl, kC0, 0.5f), 0.f);
-        a.c_r = fmaf(w, r0, a.c_r); a.c_g = fmaf(w, r1, a.c_g); a.c_b = fmaf(w, r2, a.c_b);
+        // colour: one set of 8 trilinear weights for r, g, b (value only).  SH degree 0 with relu (sh_render.py:84-94):
+        // the pack holds C0 f + 0.5 and the weights sum to one, so only the relu is left; the launcher routes
+        // sh_act != 0 to the general kernel
+        const float oh = 1.0f - fh, ow = 1.0f - fw, oz = 1.0f - fz;
+        const float m00 = oh * ow, m01 = oh * fw, m10 = fh * ow, m11 = fh * fw;
+        const float wt[8] = {m00 * oz, m00 * fz, m01 * oz, m01 * fz, m10 * oz, m10 * fz, m11 * oz, m11 * fz};
+        float r0 = wt[0] * k[0].x, r1 = wt[0] * k[0].y, r2 = wt[0] * k[0].z;
+#pragma unroll
+        for (int j = 1; j < 8; ++j) { r0 = fmaf(wt[j], k[j].x, r0); r1 = fmaf(wt[j], k[j].y, r1); r2 = fmaf(wt[j], k[j].z, r2); }
+        a.c_r = fmaf(w, fmaxf(r0, 0.f), a.c_r); a.c_g = fmaf(w, fmaxf(r1, 0.f), a.c_g); a.c_b = fmaf(w, fmaxf(r2, 0.f), a.c_b);
       }
       if (!DBG && (s & (SO_RF_EXIT_EVERY - 1)) == SO_RF_EXIT_EVERY - 1 && __all_sync(kFull, a.T < SO_RF_EXIT_T)) break;
     }
@@ -298,7 +326,9 @@ __global__ void __launch_bounds__(256) pack_rgbs_kernel(const float* __restrict_
   long long col = i / Z;
   int z = (int)(i - col * Z);
   const float* f = feat + i * fp;
-  out[i] = make_float4(f[0], f[1], f[2], sdf[col * zp + z]);
+  // the SH-0 colour map C0 f + 0.5 is affine and trilinear weights sum to one, so it is applied here once per voxel
+  // instead of once per sample; render_packed_kernel only applies the relu
+  out[i] = make_float4(fmaf(f[0], kC0, 0.5f), fmaf(f[1], kC0, 0.5f), fmaf(f[2], kC0, 0.5f), sdf[col * zp + z]);
 }
 
 }  // namespace so
@@ -365,7 +395,8 @@ extern "C" int so_render_infer_packed(const float* vol_sdf, const float* vol_fea
   ProfScope prof(0, st);
   long long* midx = reinterpret_cast<long long*>(max_idx);
   const bool rgbs = vol_host->n_feat == 3;
-  const bool nus = V.W == 257 && (rgbs ? V.Z == 31 : V.zpitch == 32);     // the nuScenes depth volume: constant pitches
+  // the nuScenes depth volume: constant pitches; its element index fits the exact fp32 index path (<= 2^23 elements)
+  const bool nus = V.W == 257 && (rgbs ? V.Z == 31 : V.zpitch == 32) && (long long)V.H * V.W * (rgbs ? V.Z : V.zpitch) <= (1 << 23);
 #define SO_RP(RGB, DBG, ZP, WZ) render_packed_kernel<RGB, DBG, ZP, WZ><<<grid, SO_RF_BLOCK, 0, st>>>( \
     V, pack, R, P, workspace, bkgd_rand, depth, max_depth, midx, acc, normal_vis, rgb, dbg_grid)
   if (dbg_grid) { if (rgbs) SO_RP(true, true, 0, 0); else SO_RP(false, true, 0, 0); }

@@ -93,7 +93,7 @@ def make_render_params(aabb, num_samples, inv_s, near_plane=0.0, training=False,
 
 def render_pack(vol_sdf, vol_feat, desc):
     """Once-per-frame repack of the decoded volume for the packed render kernels (so_render_pack): float2 z-pairs when no
-    colour is decoded, float4 (r, g, b, sdf) for color_dims == 3.  Returns None when this channel count has no packed form."""
+    colour is decoded, float4 (C0 r + 0.5, C0 g + 0.5, C0 b + 0.5, sdf) for color_dims == 3 (the SH-0 colour before its relu).  Returns None when this channel count has no packed form."""
     lib = _lib.load()
     _chk(vol_sdf, name='vol_sdf'); _chk(vol_feat, name='vol_feat')
     n = lib.so_render_pack_floats(C.byref(desc))
