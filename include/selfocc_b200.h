@@ -28,8 +28,9 @@ extern "C" {
 #define SO_ERR_CUDA (-3)          /* a CUDA runtime call or launch failed; see so_last_cuda_error */
 #define SO_ERR_NO_DEVICE (-4)
 
-#define SO_ABI_VERSION 5   /* 2: so_render_train_forward gained pair_workspace; 3: packed render volume entry points;
-                              4: backward of the fused attention cores; 5: the colour pack holds the SH-0 colour */
+#define SO_ABI_VERSION 6   /* 2: so_render_train_forward gained pair_workspace; 3: packed render volume entry points;
+                              4: backward of the fused attention cores; 5: the colour pack holds the SH-0 colour;
+                              6: reprojection-loss statistics */
 
 /* ABI version of the loaded library (compare with SO_ABI_VERSION). */
 int so_abi_version(void);
@@ -393,6 +394,42 @@ int so_tpv_self_attn_backward(const float* value, const int64_t* spatial_shapes,
                               const float* offsets, const float* logits, const float* ref, const float* grad_out,
                               float* grad_value, float* grad_offsets, float* grad_logits, int32_t Nv, int32_t Hd, int32_t Dh,
                               int32_t Q, int32_t L, int32_t P, void* stream);
+
+/* ---------------------------------------------------------------------------------------
+ * 8f-2  photometric reprojection loss: per-ray statistics of the rendering weights.  Replaces the per-sample part of
+ * ReprojLossMonoMultiNewCombine (mode SO_REPROJ_COMBINE, loss/reproj_loss_mono_multi_new_combine.py:108-198, grid_sample
+ * padding 'border') and ReprojLossMonoMultiNew (mode SO_REPROJ_MULTI_NEW, loss/reproj_loss_mono_multi_new.py:117-192,
+ * padding 'zeros').  Both use the weights only through masked sums over each ray's samples, normalised by the masked
+ * weight sum:
+ *   per set: W = sum w m,  l1 = (sum w m diff) / max(W, eps),  rgb[3] = (sum w m rgb) / max(W, eps),  any = OR m
+ * where, for the sample point (u t, v t, t, 1) of ray pixel (u, v) at depth t projected through img2prevImg / img2nextImg,
+ * divided by max(z, 1e-5) and valid when z > 0, 0 < x < size_w and 0 < y < size_h:
+ *   COMBINE (one set):  m = prev valid | next valid, cnt = max(#valid, 1),
+ *                       diff = (sum over valid d of mean_c |cur - rgb_d|) / cnt, rgb = (sum over valid d of rgb_d) / cnt
+ *   MULTI_NEW (two sets, prev then next): m, diff = mean_c |cur - rgb_d|, rgb = rgb_d of that direction.
+ * cur / rgb_d are bilinear samples (align_corners=True) of the current / prev / next image at pixel (x / size_w * (W - 1),
+ * y / size_h * (H - 1)); w = weights, or with `deltas` w / max(delta, eps) and 0 where delta < eps; eps = 2^-23 (fp32).
+ *   weights, ts, deltas (NULL = none) [n_cam, rays_per_cam, S] ray-major; pix [rays_per_cam, 2] (x, y) pixel of each ray;
+ *   img2prev, img2next [n_cam, 4, 4]; curr/prev/next images [n_cam, 3, img_h, img_w] fp32;
+ *   size_h, size_w: the loss's img_size (may differ from img_h, img_w)
+ *   -> stats [n_cam, rays_per_cam, 6 * sets] = per set (W, l1, rgb0, rgb1, rgb2, any as 0/1),
+ *      colours [n_cam, rays_per_cam, 9] = current, prev, next image at the ray pixel (NULL ok; no gradient).
+ * One warp per ray, fixed reduction order: deterministic, no atomics.
+ * so_reproj_stats_backward: the forward's `stats` and grad_stats [n_cam, rays_per_cam, 6 * sets] (the `any` slots are
+ *   ignored) -> grad_weights [n_cam, rays_per_cam, S], overwritten: the exact adjoint of the stats above (the clamp of W
+ *   passes no gradient below eps).  The per-sample terms are recomputed with the forward's arithmetic. */
+#define SO_REPROJ_COMBINE 0
+#define SO_REPROJ_MULTI_NEW 1
+int so_reproj_stats_forward(const float* weights, const float* ts, const float* deltas, const float* pix,
+                            const float* img2prev, const float* img2next, const float* curr_imgs, const float* prev_imgs,
+                            const float* next_imgs, int32_t n_cam, int32_t rays_per_cam, int32_t S, int32_t img_h,
+                            int32_t img_w, float size_h, float size_w, int32_t mode, float* stats, float* colours,
+                            void* stream);
+int so_reproj_stats_backward(const float* ts, const float* deltas, const float* pix, const float* img2prev,
+                             const float* img2next, const float* curr_imgs, const float* prev_imgs, const float* next_imgs,
+                             int32_t n_cam, int32_t rays_per_cam, int32_t S, int32_t img_h, int32_t img_w, float size_h,
+                             float size_w, int32_t mode, const float* stats, const float* grad_stats, float* grad_weights,
+                             void* stream);
 
 #ifdef __cplusplus
 }

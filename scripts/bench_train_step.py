@@ -7,7 +7,9 @@ lifter -> encoder (autograd path: the fused self- and image cross-attention core
 forward and input gradient on the wgmma GEMM, weight gradients on cuBLAS) -> NeuSHead.forward (fused decode forward,
 training-form render kernels) -> toy loss on depth / weights / eik_grad / rgb -> backward to every parameter.  Prints one
 JSON line (ms per step, device timed; peak device memory of the timed steps).  nuScenes_occ geometry: TPV 257x257x25,
-6 cams x 48x100 rays."""
+6 cams x 48x100 rays.
+    --loss reproj: the toy loss's weights term is replaced by ReprojLossMonoMultiNewCombine (the nuScenes configs' objective,
+    SSIM + automask) on seeded textured 768x1600 previous / current / next images under a small ego motion (synth)."""
 import json, os, sys, time
 import numpy as np
 import torch
@@ -40,6 +42,13 @@ metas = [dict(lidar2img=list(l2i), img2lidar=list(i2l), img_shape=(768, 1600))]
 g = torch.Generator().manual_seed(1)
 feats = [torch.randn(1, 6, 96, h, w, generator=g).to(dev) for h, w in synth.fpn_level_shapes(768, 1600)]
 opt = torch.optim.AdamW(model.parameters(), lr=1e-4)
+reproj = None
+if '--loss' in sys.argv and sys.argv[sys.argv.index('--loss') + 1] == 'reproj':
+    from selfocc_b200.loss import ReprojLossMonoMultiNewCombine
+    reproj = ReprojLossMonoMultiNewCombine(img_size=[768, 1600], ray_resize=[48, 100])
+    prev, nxt = synth.temporal_rig()
+    metas[0].update(img2prevImg=torch.tensor(prev, dtype=torch.float32, device=dev), img2nextImg=torch.tensor(nxt, dtype=torch.float32, device=dev))
+    imgs = synth.textured_images(18, 768, 1600, seed=2).reshape(3, 1, 6, 3, 768, 1600).to(dev)
 net = model
 if world > 1:
     model.head.ray_shard = (rank, world)
@@ -60,7 +69,11 @@ model.forward = lambda feats, metas: _Step.forward(None, feats, metas)
 def step():
     opt.zero_grad(set_to_none=True)
     out = net(feats, metas)
-    loss = out['ms_depths'][0].mean() * 1e-2 + torch.cat(out['weights']).pow(2).mean() \
+    if reproj is None:
+        w_term = torch.cat(out['weights']).pow(2).mean()
+    else:
+        w_term = reproj(dict(out, curr_imgs=imgs[0], prev_imgs=imgs[1], next_imgs=imgs[2], metas=metas))
+    loss = out['ms_depths'][0].mean() * 1e-2 + w_term \
         + (out['eik_grad'].norm(dim=-1) - 1).pow(2).mean() * 0.1 + out['ms_colors'][0].mean() * 0.1
     loss.backward()
     opt.step()
@@ -92,7 +105,7 @@ if '--profile' in sys.argv and world == 1:
         torch.cuda.synchronize()
     print(prof.key_averages().table(sort_by='cuda_time_total', row_limit=25))
 if rank == 0:
-  print(json.dumps({'workload': 'nuscenes_occ-like training step, %d GPU(s)%s, fp32, 6x48x100 rays x 256, TPV 257x257x25, colour' % (world, ' ray-sharded + DDP' if world > 1 else ''), 'ms_per_step': ms,
+  print(json.dumps({'workload': 'nuscenes_occ-like training step, %d GPU(s)%s, fp32, 6x48x100 rays x 256, TPV 257x257x25, colour%s' % (world, ' ray-sharded + DDP' if world > 1 else '', ', reprojection loss' if reproj is not None else ''), 'ms_per_step': ms,
                   'rays_per_s': 28800 / (ms * 1e-3), 'library_launches_per_step': (_lib.launch_count() - l0) / K, 'peak_mem_gb': peak_gb,
                   'loss': float(last), 'finite': bool(torch.isfinite(last))}))
 if world > 1:

@@ -8,7 +8,7 @@ import os
 
 _PKG = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.environ.get('SELFOCC_B200_LIB') or os.path.join(_PKG, 'lib', 'libselfocc_b200.so')   # env: experimental variant
-ABI_VERSION = 5
+ABI_VERSION = 6
 
 
 class AxisMap(C.Structure):
@@ -90,6 +90,8 @@ SIGNATURES = {
     'so_tpv_self_attn_forward': (C.c_int, [_P, _P, _P, _P, _P, _P, _P, _I, _I, _I, _I, _I, _I, _P]),
     'so_tpv_cross_attn_backward': (C.c_int, [_P] * 12 + [_I] * 7 + [_P]),
     'so_tpv_self_attn_backward': (C.c_int, [_P] * 10 + [_I] * 6 + [_P]),
+    'so_reproj_stats_forward': (C.c_int, [_P] * 9 + [_I] * 5 + [_F, _F, _I, _P, _P, _P]),
+    'so_reproj_stats_backward': (C.c_int, [_P] * 8 + [_I] * 5 + [_F, _F, _I, _P, _P, _P, _P]),
 }
 
 _lib = None

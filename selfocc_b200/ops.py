@@ -697,3 +697,71 @@ def tpv_self_attn_forward_rows(value_rows, Hd, Dh, spatial_shapes, level_start_i
                                                     v.shape[0], Hd, Dh, Q, L, P, vld, old, lld, _stream()),
                'so_tpv_self_attn_forward_strided')
     return out
+
+
+# --------------------------------------------------------------------------------------- 8f-2 reprojection loss
+REPROJ_MODES = {'combine': 0, 'multi_new': 1}     # SO_REPROJ_COMBINE / SO_REPROJ_MULTI_NEW
+REPROJ_SETS = {'combine': 1, 'multi_new': 2}
+
+
+def _one_buffer(ts, name):
+    """[N, numel] view of the per-camera list: the base pointer when the entries are adjacent views of one buffer (what
+    NeuSHead.forward emits), else a stacked copy."""
+    t0 = ts[0]
+    n = t0.numel()
+    adjacent = all(isinstance(t, torch.Tensor) and t.is_contiguous() and t.numel() == n and t.dtype == t0.dtype and
+                   t.device == t0.device and t.data_ptr() == t0.data_ptr() + i * n * t0.element_size() for i, t in enumerate(ts))
+    if adjacent:
+        buf = t0.new_empty(0).set_(t0.untyped_storage(), t0.storage_offset(), (len(ts), n))
+    else:
+        buf = torch.stack([t.reshape(-1) for t in ts])
+    return _chk(buf, name=name)
+
+
+def _reproj_call(fn, cfg, lead, outs):
+    """so_reproj_stats_forward(weights, <shared operands>, stats, colours) / so_reproj_stats_backward(<shared operands>,
+    stats, grad_stats, grad_weights): lead / outs are the pointers before / after the operands both entry points share."""
+    lib = _lib.load()
+    N, R, S = cfg['shape']
+    curr, prev, nxt = cfg['images']
+    H, W = curr.shape[-2:]
+    _lib.check(getattr(lib, fn)(*lead, _p(cfg['ts']), _p(cfg['deltas']), _p(cfg['pix']), _p(cfg['img2prev']), _p(cfg['img2next']),
+                                _p(curr), _p(prev), _p(nxt), N, R, S, H, W, float(cfg['img_size'][0]), float(cfg['img_size'][1]),
+                                REPROJ_MODES[cfg['mode']], *outs, _stream()), fn)
+
+
+class ReprojStatsFunction(torch.autograd.Function):
+    """Per-ray statistics of the reprojection loss (so_reproj_stats_forward), differentiable w.r.t. the weights.
+    apply(cfg, *weights): weights = the per-camera list [R*S] (ray-major, S samples per ray) of NeuSHead.forward;
+    cfg = dict(mode='combine' | 'multi_new', ts=[N, R*S] buffer, deltas=[N, R*S] buffer or None, pix=[R, 2] ray pixels,
+    img2prev / img2next=[N, 4, 4], images=(curr, prev, next) each [N, 3, H, W], img_size=(h, w) of the loss, shape=(N, R, S))
+    -> (stats [N, R, 6 * sets] = per set (W, l1, rgb0, rgb1, rgb2, any) with l1 / rgb the masked-weight-normalised mean
+    photometric error / colour, colours [N, R, 9] = current / prev / next image at the ray pixel).  ts, deltas and colours carry no gradient (ts and deltas are geometry only, RenderTrainFunction marks them so).
+    The weight gradients are returned as views of one [N, R*S] buffer."""
+
+    @staticmethod
+    def forward(ctx, cfg, *weights):
+        N, R, S = cfg['shape']
+        w = _one_buffer(weights, 'weights')
+        for k in ('ts', 'deltas', 'pix', 'img2prev', 'img2next'):
+            _chk(cfg[k], name=k)
+        for t in cfg['images']:
+            _chk(t, name='images')
+        stats = torch.empty(N, R, 6 * REPROJ_SETS[cfg['mode']], device=w.device)
+        colours = torch.empty(N, R, 9, device=w.device)
+        _reproj_call('so_reproj_stats_forward', cfg, (_p(w),), (_p(stats), _p(colours)))
+        ctx.cfg = cfg
+        ctx.shapes = [t.shape for t in weights]
+        ctx.save_for_backward(stats)
+        ctx.mark_non_differentiable(colours)
+        return stats, colours
+
+    @staticmethod
+    @torch.autograd.function.once_differentiable
+    def backward(ctx, g_stats, g_colours):
+        cfg = ctx.cfg
+        N, R, S = cfg['shape']
+        gw = torch.empty(N, R * S, device=g_stats.device)
+        stats, = ctx.saved_tensors
+        _reproj_call('so_reproj_stats_backward', cfg, (), (_p(stats), _p(_chk(g_stats.contiguous(), name='grad_stats')), _p(gw)))
+        return (None,) + tuple(gw[i].view(shp) for i, shp in enumerate(ctx.shapes))

@@ -60,6 +60,12 @@ except Exception:
     HAVE_MMENGINE = False
 
 
+# The reference's loss registry is private to its `loss` package (loss/__init__.py: OPENOCC_LOSS = Registry('openocc_loss')),
+# so this package cannot register into it at import time; its losses live here and INTEGRATION.md shows the two
+# `OPENOCC_LOSS.register_module(module=..., force=True)` lines that hand them to the reference's MultiLoss.
+LOSSES = Registry('selfocc_b200.losses')
+
+
 def build_head(cfg):
     """mmseg.models.builder.build_head: the reference builds lifter, encoder AND head with it
     (model/segmentor/base_segmentor.py:27-32)."""

@@ -88,3 +88,34 @@ def random_mlp(C, n_out, seed=0):
 
 def fpn_level_shapes(img_h, img_w, strides=(8, 16, 32, 64)):
     return [(math.ceil(img_h / s), math.ceil(img_w / s)) for s in strides]
+
+
+def temporal_rig(yaws_deg=NUSC_YAWS, f=1266.0, cx=800.0, cy=450.0, height=1.5, radius=0.5, forward=0.5, yaw_deg=1.0):
+    """img2prevImg / img2nextImg of camera_rig() under a small ego motion: the previous frame's ego pose is `forward`
+    metres behind along the lidar y axis and yawed by -yaw_deg, the next one as far ahead and yawed by +yaw_deg.
+    A pixel (u, v) at camera depth t maps to lidar2img @ inv(ego pose) @ img2lidar @ (u t, v t, t, 1).
+    Returns (img2prevImg [N,4,4], img2nextImg [N,4,4]) float64 numpy."""
+    l2i, i2l = camera_rig(yaws_deg, f, cx, cy, height, radius)
+    out = []
+    for sign in (-1.0, 1.0):
+        a = np.deg2rad(sign * yaw_deg)
+        pose = np.eye(4)
+        pose[:2, :2] = [[np.cos(a), -np.sin(a)], [np.sin(a), np.cos(a)]]
+        pose[1, 3] = sign * forward
+        out.append(np.stack([l2i[c] @ np.linalg.inv(pose) @ i2l[c] for c in range(len(yaws_deg))]))
+    return out[0], out[1]
+
+
+def textured_images(n_img, H, W, seed=0, waves=6):
+    """Smooth seeded RGB images [n_img, 3, H, W] fp32 in about [0.05, 0.95]: a sum of random plane waves with periods of
+    tens to hundreds of pixels per channel, so bilinear colours and their differences vary smoothly and are not degenerate."""
+    g = torch.Generator().manual_seed(seed)
+    y = torch.arange(H, dtype=torch.float64)[:, None] / max(H, W)
+    x = torch.arange(W, dtype=torch.float64)[None, :] / max(H, W)
+    img = torch.full((n_img, 3, H, W), 0.5, dtype=torch.float64)
+    for _ in range(waves):
+        k = (torch.rand(n_img, 3, 2, generator=g, dtype=torch.float64) * 2 - 1) * 40.0      # radians across the image
+        ph = torch.rand(n_img, 3, generator=g, dtype=torch.float64) * 6.283185307179586
+        amp = 0.45 / waves * (0.5 + torch.rand(n_img, 3, generator=g, dtype=torch.float64))
+        img += amp[..., None, None] * torch.sin(k[..., 0, None, None] * x + k[..., 1, None, None] * y + ph[..., None, None])
+    return img.float().contiguous()
