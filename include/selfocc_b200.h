@@ -28,9 +28,9 @@ extern "C" {
 #define SO_ERR_CUDA (-3)          /* a CUDA runtime call or launch failed; see so_last_cuda_error */
 #define SO_ERR_NO_DEVICE (-4)
 
-#define SO_ABI_VERSION 6   /* 2: so_render_train_forward gained pair_workspace; 3: packed render volume entry points;
+#define SO_ABI_VERSION 7   /* 2: so_render_train_forward gained pair_workspace; 3: packed render volume entry points;
                               4: backward of the fused attention cores; 5: the colour pack holds the SH-0 colour;
-                              6: reprojection-loss statistics */
+                              6: reprojection-loss statistics; 7: training-render sample probe */
 
 /* ABI version of the loaded library (compare with SO_ABI_VERSION). */
 int so_abi_version(void);
@@ -218,6 +218,15 @@ int so_render_train_backward(const float* vol_sdf, const float* vol_feat, const 
                              const float* g_depth, const float* g_acc, const float* g_rgb, const float* g_sem,
                              const float* g_weights, const float* g_eik, const float* g_sdf,
                              float* g_vol_sdf, float* g_vol_feat, float* g_inv_s, float* workspace, void* stream);
+
+/* Test probe of the training render's sample geometry (the training analogue of so_render_infer_packed's dbg_grid):
+ * same ray / param / jitter / volume operands as so_render_train_forward.  grid [n, S, 3] receives the fp32 (h, w, d) grid
+ * coordinates of every sample, computed with the device function that so_render_train_forward's one-ray-per-warp kernel
+ * and so_render_train_backward use for this configuration (the backward recomputes the samples with the arithmetic of
+ * the forward it is paired with).  The batched forward kernel builds the same values with its own edge arithmetic; its
+ * `ts` / `deltas` outputs are bit-identical to the one-ray-per-warp kernel's. */
+int so_render_train_probe(const so_volume_desc* vol_host, const float* cam_mats, const float* pix, const so_ray_desc* rays_host,
+                          const so_render_params* params_host, const float* jitter, float* grid, void* stream);
 
 /* Backward of so_field_query: g_sdf [n], g_grad [n,3], g_feat [n,n_feat] (NULL = zero) accumulated into
  * g_vol_sdf / g_vol_feat (caller zero-fills). */

@@ -132,9 +132,10 @@ def uniform_bins(nears, fars, S, jitter=None):
 
 def neus_render_chunk(vol, mapping, o, d, dnorm, aabb, inv_s, S=256, near_plane=0.0, training=False,
                       jitter=None, cos_anneal=1.0, color_dims=0, sh_act='relu', bkgd='white',
-                      bkgd_rand=None, anchor='mid', differentiable=False, grid_override=None):
+                      bkgd_rand=None, anchor='mid', differentiable=False, grid_override=None, depth_clip=None):
     """One ``self.model(ray_bundle)`` call of the reference (neus_head.py:353/394/531) for a chunk
-    of rays o,d [R,3] (d unit), dnorm [R,1].  Returns the dict the head consumes."""
+    of rays o,d [R,3] (d unit), dnorm [R,1].  Returns the dict the head consumes.  ``depth_clip`` = (lo, hi): the
+    expected-depth clip bounds of the whole batch when this call renders only a part of it (default: this chunk's)."""
     R = o.shape[0]
     nears, fars = aabb_near_far(o, d, aabb, near_plane, training)
     starts, ends = uniform_bins(nears, fars, S, jitter)
@@ -165,7 +166,7 @@ def neus_render_chunk(vol, mapping, o, d, dnorm, aabb, inv_s, S=256, near_plane=
     acc = weights.sum(-1)
     # expected-depth renderer incl. its chunk-wide clip, then ray-length -> camera-z units
     depth = (weights * mids).sum(-1) / (acc + 1e-10)
-    depth = depth.clip(mids.min(), mids.max())
+    depth = depth.clip(*(depth_clip if depth_clip is not None else (mids.min(), mids.max())))
     depth = depth / dnorm[:, 0]
     normals = F.normalize(grad, p=2, dim=-1)
     normal = (weights[..., None] * normals).sum(-2)

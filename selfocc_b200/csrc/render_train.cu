@@ -60,25 +60,63 @@ __device__ __forceinline__ void make_ctx(const VolumeDev& V, const RayDev& R, co
   c.u = P.jitter ? P.jitter + gid * (long long)(P.S + 1) : nullptr;
 }
 
-// one sample of one ray (lane = sample): geometry + field + alpha.  `s` must be < S.  Edges are shared between
-// neighbouring lanes with one shuffle (lane 31 computes its own right edge).
-__device__ __forceinline__ void eval_sample(const VolumeDev& V, const RenderDev& P, const RayCtx& c, int s, int lane, Sample& q) {
+// FAST = affine metre->grid map, S a power of two (multiple of 32), cos-anneal finished, mid-point anchor (see
+// train_fast).  Every training kernel of a FAST launch -- both forwards, the backward and the probe -- takes its sample
+// positions from these two helpers, so the backward differentiates exactly the cells the forward rendered.
+// Edge i is re-drawn inside [max(i - 1/2, 0), min(i + 1/2, S)] / S (exact arithmetic for power-of-two S).
+__device__ __forceinline__ float fast_edge(int i, float u, bool jit, int S, float step, float span, float tn) {
+  float fi = (float)i;
+  float lo_b = fmaxf(fi - 0.5f, 0.f) * step, up_b = fminf(fi + 0.5f, (float)S) * step;
+  float b = jit ? fmaf(up_b - lo_b, u, lo_b) : fi * step;
+  return fmaf(b, span, tn);
+}
+// mid-point, width and affine grid coordinates of the bin [e0, e1]
+__device__ __forceinline__ void fast_mid_grid(float e0, float e1, float gh0, float gdh, float gw0, float gdw, float gd0, float gdd,
+                                              float& mid, float& delta, float& gh, float& gw, float& gd) {
+  mid = 0.5f * (e0 + e1);
+  delta = e1 - e0;
+  gh = fmaf(gdh, mid, gh0); gw = fmaf(gdw, mid, gw0); gd = fmaf(gdd, mid, gd0);
+}
+
+// geometry of one sample of one ray (lane = sample): bin mid-point, width, grid coordinates and metre->grid slopes.
+// `s` must be < S.  Edges are shared between neighbouring lanes with one shuffle (lane 31 computes its own right edge).
+// FAST: the shipped forwards' arithmetic; otherwise the reference form b * tf + (1 - b) * tn of the edges.
+template <bool FAST>
+__device__ __forceinline__ void sample_geom(const VolumeDev& V, const RenderDev& P, const RayCtx& c, int s, int lane, float& mid,
+                                            float& delta, float& gh, float& gw, float& gd, float& kh, float& kw, float& kd) {
   const int S = P.S;
   const float step = 1.0f / (float)S;
+  if (FAST) {
+    const float span = c.tf - c.tn;
+    float e0 = fast_edge(s, c.u ? __ldg(c.u + s) : 0.f, c.u != nullptr, S, step, span, c.tn);
+    float e1 = __shfl_down_sync(0xffffffffu, e0, 1);
+    const int s1 = min(s + 1, S);
+    if (lane == 31 || s + 1 >= S) e1 = fast_edge(s1, c.u ? __ldg(c.u + s1) : 0.f, c.u != nullptr, S, step, span, c.tn);
+    fast_mid_grid(e0, e1, c.gh0, c.gdh, c.gw0, c.gdw, c.gd0, c.gdd, mid, delta, gh, gw, gd);
+    kh = V.ax[0].k0; kw = V.ax[1].k0; kd = V.ax[2].k0;
+    return;
+  }
   float e0 = edge_t(bin_edge01_jit(s, S, step, c.u), c.tn, c.tf);
   float e1 = __shfl_down_sync(0xffffffffu, e0, 1);
   if (lane == 31 || s + 1 >= S) e1 = edge_t(bin_edge01_jit(min(s + 1, S), S, step, c.u), c.tn, c.tf);
-  q.mid = __fmul_rn(__fadd_rn(e0, e1), 0.5f);
-  q.delta = __fsub_rn(e1, e0);
-  float tq = P.anchor_mid ? q.mid : e0;
-  float gh, gw, gd;
+  mid = __fmul_rn(__fadd_rn(e0, e1), 0.5f);
+  delta = __fsub_rn(e1, e0);
+  float tq = P.anchor_mid ? mid : e0;
   if (c.affine) {
     gh = fmaf(c.gdh, tq, c.gh0); gw = fmaf(c.gdw, tq, c.gw0); gd = fmaf(c.gdd, tq, c.gd0);
-    q.kh = V.ax[0].k0; q.kw = V.ax[1].k0; q.kd = V.ax[2].k0;
+    kh = V.ax[0].k0; kw = V.ax[1].k0; kd = V.ax[2].k0;
   } else {
     float x = fmaf(c.d[0], tq, c.o[0]), y = fmaf(c.d[1], tq, c.o[1]), z = fmaf(c.d[2], tq, c.o[2]);
-    gh = axis_m2g(V.ax[0], y, q.kh); gw = axis_m2g(V.ax[1], x, q.kw); gd = axis_m2g(V.ax[2], z, q.kd);
+    gh = axis_m2g(V.ax[0], y, kh); gw = axis_m2g(V.ax[1], x, kw); gd = axis_m2g(V.ax[2], z, kd);
   }
+}
+
+// one sample of one ray (lane = sample): geometry + field + alpha.  `s` must be < S.  FAST: the alpha value is the
+// shipped forwards' neus_alpha_log2 as well (pa / pb, which the backward differentiates, are the same logistics).
+template <bool FAST>
+__device__ __forceinline__ void eval_sample(const VolumeDev& V, const RenderDev& P, const RayCtx& c, int s, int lane, Sample& q) {
+  float gh, gw, gd;
+  sample_geom<FAST>(V, P, c, s, lane, q.mid, q.delta, gh, gw, gd, q.kh, q.kw, q.kd);
   q.t = make_taps(V, gh, gw, gd);
   float dgh, dgw, dgd;
   const bool interior = (unsigned)q.t.h0 < (unsigned)(V.H - 1) && (unsigned)q.t.w0 < (unsigned)(V.W - 1) &&
@@ -92,8 +130,13 @@ __device__ __forceinline__ void eval_sample(const VolumeDev& V, const RenderDev&
   float a = (q.sdf - q.half) * P.inv_s, b = (q.sdf + q.half) * P.inv_s;
   q.pa = sigmoid_fast(a);
   q.pb = sigmoid_fast(b);
-  float diff = q.pa * sigmoid_fast(-b) * one_minus_exp_neg(-2.0f * q.half * P.inv_s);
-  q.alpha = __saturatef(__fdividef(diff + 1e-5f, q.pa + 1e-5f));
+  if (FAST) {
+    const float k_log2 = P.inv_s * 1.4426950408889634f;
+    q.alpha = neus_alpha_log2(q.sdf * k_log2, fminf(q.tc, 0.f) * (q.delta * (0.5f * k_log2)));
+  } else {
+    float diff = q.pa * sigmoid_fast(-b) * one_minus_exp_neg(-2.0f * q.half * P.inv_s);
+    q.alpha = __saturatef(__fdividef(diff + 1e-5f, q.pa + 1e-5f));
+  }
 }
 
 __device__ __forceinline__ float warp_incl_prod(float v, int lane) {
@@ -214,21 +257,14 @@ __global__ void __launch_bounds__(128, SEM == 24 ? SO_TRAIN_FWD24_MIN_CTAS : SO_
       if (FAST) {
         const int s_nxt = s + 32;
         const float u_nxt = (c.u && s_nxt <= S) ? __ldg(c.u + s_nxt) : 0.f;
-        // edge i is re-drawn inside [max(i - 1/2, 0), min(i + 1/2, S)] / S (exact arithmetic for power-of-two S)
-        auto edge = [&](int i, float u) {
-          float fi = (float)i;
-          float lo_b = fmaxf(fi - 0.5f, 0.f) * step, up_b = fminf(fi + 0.5f, (float)S) * step;
-          float b = c.u ? fmaf(up_b - lo_b, u, lo_b) : fi * step;
-          return fmaf(b, span, c.tn);
-        };
+        auto edge = [&](int i, float u) { return fast_edge(i, u, c.u != nullptr, S, step, span, c.tn); };
         float e0 = edge(s, u_cur);
         float e_next = edge(k * 32 + 32, __shfl_sync(0xffffffffu, u_nxt, 0));   // right edge of lane 31 = first edge of the next chunk
         float e1 = __shfl_down_sync(0xffffffffu, e0, 1);
         if (lane == 31) e1 = e_next;
         u_cur = u_nxt;
-        q.mid = 0.5f * (e0 + e1);
-        q.delta = e1 - e0;
-        float gh = fmaf(c.gdh, q.mid, c.gh0), gw = fmaf(c.gdw, q.mid, c.gw0), gd = fmaf(c.gdd, q.mid, c.gd0);
+        float gh, gw, gd;
+        fast_mid_grid(e0, e1, c.gh0, c.gdh, c.gw0, c.gdw, c.gd0, c.gdd, q.mid, q.delta, gh, gw, gd);
         q.kh = V.ax[0].k0; q.kw = V.ax[1].k0; q.kd = V.ax[2].k0;
         float flh = floorf(gh), flw = floorf(gw), flz = floorf(gd);
         int h0 = (int)flh, w0 = (int)flw, z0 = (int)flz;
@@ -245,7 +281,7 @@ __global__ void __launch_bounds__(128, SEM == 24 ? SO_TRAIN_FWD24_MIN_CTAS : SO_
         float tc = c.d[0] * q.gx + c.d[1] * q.gy + c.d[2] * q.gz;
         q.alpha = neus_alpha_log2(q.sdf * k_log2, fminf(tc, 0.f) * (q.delta * (0.5f * k_log2)));
       } else {
-        eval_sample(V, P, c, live ? s : S - 1, lane, q);
+        eval_sample<false>(V, P, c, live ? s : S - 1, lane, q);
       }
       float alpha = live ? q.alpha : 0.f;
       float f = live ? (1.0f - alpha + 1e-7f) : 1.0f;
@@ -488,9 +524,7 @@ render_train_fwd5_kernel(VolumeDev V, RayDev R, RenderDev P, const float* __rest
           // right edge = left edge of the next sample: lane l + 1, or lane 0 of the next chunk for lane 31
           const float src = lane == 0 ? (j + 1 < U ? e0[j + 1 < U ? j + 1 : j] : e_next) : e0[j];
           const float e1 = __shfl_sync(kFull, src, (lane + 1) & 31);
-          mid[j] = 0.5f * (e0[j] + e1);
-          delta[j] = e1 - e0[j];
-          gh[j] = fmaf(gdh, mid[j], gh0); gw[j] = fmaf(gdw, mid[j], gw0); gd[j] = fmaf(gdd, mid[j], gd0);
+          fast_mid_grid(e0[j], e1, gh0, gdh, gw0, gdw, gd0, gdd, mid[j], delta[j], gh[j], gw[j], gd[j]);
           float flh = floorf(gh[j]), flw = floorf(gw[j]), flz = floorf(gd[j]);
           h0[j] = (int)flh; w0[j] = (int)flw; z0[j] = (int)flz;
           fh[j] = gh[j] - flh; fw[j] = gw[j] - flw; fz[j] = gd[j] - flz;
@@ -645,7 +679,8 @@ __device__ __forceinline__ void scatter_feat(const VolumeDev& V, float* __restri
   }
 }
 
-template <bool HAS_RGB, int SEM>
+// FAST: recompute the samples with the arithmetic of the FAST forwards (sample_geom<true>, neus_alpha_log2)
+template <bool HAS_RGB, int SEM, bool FAST>
 __global__ void __launch_bounds__(128, SEM == 24 ? SO_TRAIN_BWD24_MIN_CTAS : 1) render_train_bwd_kernel(VolumeDev V, RayDev R, RenderDev P, const float* __restrict__ ws,
                                                                const float* __restrict__ bkgd_rand, TrainGrad G) {
   constexpr bool HAS_SEM = SEM != 0;
@@ -670,7 +705,7 @@ __global__ void __launch_bounds__(128, SEM == 24 ? SO_TRAIN_BWD24_MIN_CTAS : 1) 
       int s = k * 32 + lane;
       bool live = s < S;
       Sample q;
-      eval_sample(V, P, c, live ? s : S - 1, lane, q);
+      eval_sample<FAST>(V, P, c, live ? s : S - 1, lane, q);
       float alpha = live ? q.alpha : 0.f;
       float f = live ? (1.0f - alpha + 1e-7f) : 1.0f;
       float incl = warp_incl_prod(f, lane);
@@ -703,7 +738,7 @@ __global__ void __launch_bounds__(128, SEM == 24 ? SO_TRAIN_BWD24_MIN_CTAS : 1) 
       int s = kk * 32 + lane;
       bool live = s < S;
       Sample q;
-      eval_sample(V, P, c, live ? s : S - 1, lane, q);
+      eval_sample<FAST>(V, P, c, live ? s : S - 1, lane, q);
       float T = Tk[kk], alpha = Ak[kk];
       float w = alpha * T;
       long long oidx = ray * S + (live ? s : S - 1);
@@ -817,6 +852,35 @@ __global__ void __launch_bounds__(256) field_query_bwd_kernel(VolumeDev V, const
     for (int c = 0; c < V.n_feat; ++c) { float g1[1] = {g_feat[i * V.n_feat + c]}; scatter_feat<1>(V, gvf, t, c, g1); }
 }
 
+// test probe: the fp32 grid coordinates of every sample as the forwards and the backward of this launch compute them
+template <bool FAST>
+__global__ void __launch_bounds__(128) render_train_probe_kernel(VolumeDev V, RayDev R, RenderDev P, float* __restrict__ grid) {
+  const int lane = threadIdx.x & 31;
+  const long long warps = (long long)gridDim.x * (blockDim.x >> 5);
+  const int S = P.S;
+  const int K = (S + 31) >> 5;
+  for (long long ray = blockIdx.x * (long long)(blockDim.x >> 5) + (threadIdx.x >> 5); ray < R.ray_count; ray += warps) {
+    RayCtx c;
+    make_ctx(V, R, P, R.ray_begin + ray, c);
+    for (int k = 0; k < K; ++k) {
+      const int s = k * 32 + lane;
+      const bool live = s < S;
+      float mid, delta, gh, gw, gd, kh, kw, kd;
+      sample_geom<FAST>(V, P, c, live ? s : S - 1, lane, mid, delta, gh, gw, gd, kh, kw, kd);
+      if (live) {
+        float* o = grid + 3 * (ray * S + s);
+        o[0] = gh; o[1] = gw; o[2] = gd;
+      }
+    }
+  }
+}
+
+// the lean per-sample path of the forwards applies (see fast_edge)
+static bool train_fast(const VolumeDev& V, const RenderDev& P) {
+  return V.ax[0].k1 == 0.f && V.ax[1].k1 == 0.f && V.ax[2].k1 == 0.f && (P.S & (P.S - 1)) == 0 && P.S >= 32 &&
+         P.cos_anneal == 1.0f && P.anchor_mid;
+}
+
 static int train_common_checks(const float* vol_sdf, const float* vol_feat, const so_volume_desc* d, const float* cam_mats,
                                const so_ray_desc* rd, const so_render_params* pr, const float* workspace, bool want_rgb,
                                bool want_sem, const float* bkgd_rand) {
@@ -872,8 +936,7 @@ extern "C" int so_render_train_forward(const float* vol_sdf, const float* vol_fe
   const long long cap = (long long)num_sms() * 16;
   unsigned grid = (unsigned)(ctas < cap ? ctas : cap);
   ProfScope prof(6, st);
-  const bool fast = V.ax[0].k1 == 0.f && V.ax[1].k1 == 0.f && V.ax[2].k1 == 0.f && (P.S & (P.S - 1)) == 0 && P.S >= 32 &&
-                    P.cos_anneal == 1.0f && P.anchor_mid;
+  const bool fast = train_fast(V, P);
   // batched-ray kernel (U chunks in flight, optional z-pair volume); the one-ray-per-warp kernel covers semantics,
   // non-affine mappings, S not a multiple of 32 U and the cos-anneal phase
   const bool sem24 = want_sem && V.n_feat == 24 && V.feat_pitch == 24 && (reinterpret_cast<uintptr_t>(vol_feat) & 15) == 0 && !g_force_sem_generic;
@@ -931,10 +994,37 @@ extern "C" int so_render_train_backward(const float* vol_sdf, const float* vol_f
   ProfScope prof(7, st);
   const bool sem24 = V.n_feat == 24 && V.feat_pitch == 24 && (want_rgb || want_sem) && !g_force_sem_generic &&
                      ((reinterpret_cast<uintptr_t>(vol_feat) | reinterpret_cast<uintptr_t>(g_vol_feat)) & 15) == 0;
-  if (sem24) render_train_bwd_kernel<true, 24><<<grid, 128, 0, st>>>(V, R, P, workspace, bkgd_rand, G);
-  else if (want_sem) render_train_bwd_kernel<true, 1><<<grid, 128, 0, st>>>(V, R, P, workspace, bkgd_rand, G);
-  else if (want_rgb) render_train_bwd_kernel<true, 0><<<grid, 128, 0, st>>>(V, R, P, workspace, bkgd_rand, G);
-  else render_train_bwd_kernel<false, 0><<<grid, 128, 0, st>>>(V, R, P, workspace, bkgd_rand, G);
+  const bool fast = train_fast(V, P);      // recompute the samples with the arithmetic of the paired forward
+#define SO_TRAIN_BWD(RGB, SEM) do { \
+    if (fast) render_train_bwd_kernel<RGB, SEM, true><<<grid, 128, 0, st>>>(V, R, P, workspace, bkgd_rand, G); \
+    else render_train_bwd_kernel<RGB, SEM, false><<<grid, 128, 0, st>>>(V, R, P, workspace, bkgd_rand, G); } while (0)
+  if (sem24) SO_TRAIN_BWD(true, 24);
+  else if (want_sem) SO_TRAIN_BWD(true, 1);
+  else if (want_rgb) SO_TRAIN_BWD(true, 0);
+  else SO_TRAIN_BWD(false, 0);
+#undef SO_TRAIN_BWD
+  note_launch(1);
+  return check_launch();
+}
+
+extern "C" int so_render_train_probe(const so_volume_desc* vol_host, const float* cam_mats, const float* pix, const so_ray_desc* rd,
+                                     const so_render_params* pr, const float* jitter, float* grid, void* stream) {
+  if (!vol_host || !cam_mats || !rd || !pr || !grid) return SO_ERR_INVALID_ARG;
+  int rc = validate_volume(vol_host);
+  if (rc) return rc;
+  if (pr->num_samples < 1) return SO_ERR_INVALID_ARG;
+  if (pr->num_samples > 32 * kTrainMaxChunks) return SO_ERR_UNSUPPORTED;
+  RayDev R;
+  if ((rc = make_ray_dev(rd, cam_mats, pix, &R))) return rc;
+  if (R.ray_count == 0) return SO_OK;
+  VolumeDev V = make_volume(*vol_host, nullptr, nullptr);
+  RenderDev P = make_render_dev(*pr, jitter);
+  long long ctas = ceil_div64(R.ray_count, 4);
+  const long long cap = (long long)num_sms() * 16;
+  unsigned g = (unsigned)(ctas < cap ? ctas : cap);
+  cudaStream_t st = (cudaStream_t)stream;
+  if (train_fast(V, P)) render_train_probe_kernel<true><<<g, 128, 0, st>>>(V, R, P, grid);
+  else render_train_probe_kernel<false><<<g, 128, 0, st>>>(V, R, P, grid);
   note_launch(1);
   return check_launch();
 }

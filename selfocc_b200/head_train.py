@@ -11,7 +11,8 @@ def chunk_cams(tensor, num_cams):
     return [t.squeeze() for t in torch.chunk(tensor.reshape(num_cams, -1), num_cams, dim=0)]
 
 
-def forward_train(head, representation, metas=None, jitter=None, bkgd_rand=None, **kwargs):
+def forward_train(head, representation, metas=None, jitter=None, bkgd_rand=None, uniform_shift=None, **kwargs):
+    """uniform_shift: the [H*W*D, 3] lattice jitter in [0, 1) of get_uniform_sdf (default: drawn here)."""
     f = head.model.field
     hw, zh, wz = representation
     assert hw.shape[0] == 1, 'only support bs = 1 currently'
@@ -74,7 +75,7 @@ def forward_train(head, representation, metas=None, jitter=None, bkgd_rand=None,
 
     uniform_sdf = None
     if head.return_uniform_sdf:
-        uniform_sdf = _uniform_sdf_train(head, dev)
+        uniform_sdf = _uniform_sdf_train(head, dev, uniform_shift)
     weights_for_cams = chunk_cams(weights, num_cams)
     ts_for_cams = chunk_cams(ts, num_cams)
     deltas_for_cams = chunk_cams(deltas, num_cams)
@@ -116,16 +117,26 @@ def forward_train(head, representation, metas=None, jitter=None, bkgd_rand=None,
     return outputs
 
 
-def _uniform_sdf_train(head, dev):
-    """get_uniform_sdf(aabb, resolution, shift=True) with gradients to the volume (neus_head.py:533-538)."""
-    f = head.model.field
+def uniform_lattice_train(head, dev):
+    """The [H, W, D, 3] metre lattice of get_uniform_sdf (neus_head.py:266-277) on ``dev``."""
     a, r = head.aabb, head.resolution
     xs = torch.linspace(a[0], a[3], int((a[3] - a[0]) / r), device=dev)
     ys = torch.linspace(a[1], a[4], int((a[4] - a[1]) / r), device=dev)
     zs = torch.linspace(a[2], a[5], int((a[5] - a[2]) / r), device=dev)
     W, H, D = len(xs), len(ys), len(zs)
-    xyz = torch.stack([xs[None, :, None].expand(H, W, D), ys[:, None, None].expand(H, W, D),
-                       zs[None, None, :].expand(H, W, D)], dim=-1).flatten(0, 2)
-    xyz = (xyz + torch.rand_like(xyz) * r).contiguous()
+    return torch.stack([xs[None, :, None].expand(H, W, D), ys[:, None, None].expand(H, W, D),
+                        zs[None, None, :].expand(H, W, D)], dim=-1)
+
+
+def _uniform_sdf_train(head, dev, shift=None):
+    """get_uniform_sdf(aabb, resolution, shift=True) with gradients to the volume (neus_head.py:533-538)."""
+    f = head.model.field
+    lat = uniform_lattice_train(head, dev)
+    H, W, D = lat.shape[:3]
+    xyz = lat.flatten(0, 2)
+    if shift is None:
+        shift = torch.rand_like(xyz)
+    assert shift.shape == xyz.shape, 'uniform_shift must be [H*W*D, 3]'
+    xyz = (xyz + shift * head.resolution).contiguous()
     s, _, _ = ops.FieldQueryFunction.apply(f.vol_sdf_live, f.vol_feat_live, f.desc, xyz, False, False)
     return s.reshape(H, W, D)

@@ -405,6 +405,20 @@ class RenderTrainFunction(torch.autograd.Function):
         return gvs, gvf, ginv, None
 
 
+def render_train_probe(desc, cam_mats, rays, params, pix=None, jitter=None):
+    """Test probe (so_render_train_probe): [n, S, 3], the fp32 (h, w, d) grid coordinates of every sample as the training
+    forward and its backward compute them for these operands."""
+    lib = _lib.load()
+    _chk(cam_mats, name='cam_mats'); _chk(pix, name='pix'); _chk(jitter, name='jitter')
+    n, S = rays.ray_count, params.num_samples
+    if jitter is not None:
+        assert jitter.shape == (rays.n_cam * rays.rays_per_cam, S + 1)
+    grid = torch.empty(n, S, 3, device=cam_mats.device)
+    _lib.check(lib.so_render_train_probe(C.byref(desc), _p(cam_mats), _p(pix), C.byref(rays), C.byref(params), _p(jitter),
+                                         _p(grid), _stream()), 'so_render_train_probe')
+    return grid
+
+
 class FieldQueryFunction(torch.autograd.Function):
     """Differentiable (w.r.t. the volume) point query: (vol_sdf, vol_feat, desc, points[n,3]) -> (sdf[n], grad[n,3], feat[n,nf])."""
 

@@ -121,6 +121,25 @@ def test_entry_points_reject_bad_arguments_without_a_gpu():
     # strided attention entry points: odd offset pitch / mis-aligned offsets are refused (float2 loads)
     assert lib.so_tpv_self_attn_forward_strided(one, one, one, one, one, one, one, 10, 6, 16, 4, 3, 4, 96, 6 * 3 * 4 * 2 + 1, 6 * 3 * 4, N) == -1
     assert lib.so_tpv_self_attn_forward_strided(one, one, one, C.c_void_p(20), one, one, one, 10, 6, 16, 4, 3, 4, 96, 6 * 3 * 4 * 2, 6 * 3 * 4, N) == -1
+    # training-render sample probe: operands checked before any launch
+    rd, pr = _lib.RayDesc(), _lib.RenderParams()
+    rd.n_cam, rd.rays_per_cam, rd.ray_count = 1, 4, 4
+    pr.num_samples = 64
+    assert lib.so_render_train_probe(N, one, one, C.byref(rd), C.byref(pr), N, one, N) == -1          # no volume
+    assert lib.so_render_train_probe(C.byref(ok), N, one, C.byref(rd), C.byref(pr), N, one, N) == -1  # no cameras
+    assert lib.so_render_train_probe(C.byref(ok), one, one, C.byref(rd), C.byref(pr), N, N, N) == -1  # no output
+    assert lib.so_render_train_probe(C.byref(d), one, one, C.byref(rd), C.byref(pr), N, one, N) == -1   # zpitch < Z
+    assert lib.so_render_train_probe(C.byref(big), one, one, C.byref(rd), C.byref(pr), N, one, N) == -2
+    assert lib.so_render_train_probe(C.byref(ok), one, N, C.byref(rd), C.byref(pr), N, one, N) == -1    # no pixels, no grid
+    rd.nx, rd.ny = 2, 2
+    rd.ray_begin = 3                                                                                   # 3 + 4 rays > 4
+    assert lib.so_render_train_probe(C.byref(ok), one, N, C.byref(rd), C.byref(pr), N, one, N) == -1
+    rd.ray_begin, rd.ray_count = 0, 0
+    assert lib.so_render_train_probe(C.byref(ok), one, N, C.byref(rd), C.byref(pr), N, one, N) == 0    # no rays: nothing to do
+    pr.num_samples = 0
+    assert lib.so_render_train_probe(C.byref(ok), one, N, C.byref(rd), C.byref(pr), N, one, N) == -1
+    pr.num_samples = 257                                                                               # S <= 256
+    assert lib.so_render_train_probe(C.byref(ok), one, N, C.byref(rd), C.byref(pr), N, one, N) == -2
     for hook in (lib.so_attn_force_v1, lib.so_linear_force_ss, lib.so_render_train_force_sem_generic):
         assert hook(1) == 0 and hook(0) == 0
 

@@ -1,5 +1,6 @@
 """CPU: analytic self-checks of the (unpinned) parts of the oracle (SURVEY.md 8c iii)."""
 import math
+import pytest
 import torch
 from oracle.mapping import GridMeterMappingRef
 from oracle import render as orender, lifting as ol, rays as orays
@@ -70,3 +71,49 @@ def test_max_depth_first_maximum():
     d = torch.full((1, 4), 0.5)
     md, idx = orender.max_depth_ref(w, ts, d)
     assert idx.item() == 1 and md.item() == 2.0
+
+
+def test_train_parity_reproduces_itself_and_masks_exactly_the_flip_rays():
+    """oracle/train_parity.py on the oracle's own fp64 results: with its own coordinates as the kernel's probe the same-cells
+    run reproduces the independent one exactly (outputs and gradients) and every tolerance keeps its unscaled value;
+    flip_rays flags exactly the rays with a sample moved into another cell (a move inside the cell is not a flip), and a
+    cotangent left on a flagged ray is refused."""
+    from oracle import train_parity as tp
+    m, aabb = _map(10, 6)
+    g = torch.Generator().manual_seed(2)
+    sdf = synth.analytic_sdf_volume(m, ground_z=-1.0, spheres=((3., 5., 0., 1.5),), boxes=(), noise=0.05, seed=1)
+    vol = torch.cat([sdf[None], torch.randn(4, *sdf.shape, generator=g)], 0).double()
+    _, i2l = synth.camera_rig(synth.NUSC_YAWS[:2], f=126.6, cx=80., cy=45., height=0.5, radius=0.2)
+    origin, direction = orays.img2lidar_rays(torch.tensor(i2l, dtype=torch.float32)[None], orays.fixed_ray_grid([3, 4], [90, 160]))
+    o, d, nrm = orays.flatten_rays(origin.double(), direction.double())
+    n, S = o.shape[0], 32
+    jitter = torch.rand(n, S + 1, generator=g, dtype=torch.float64)
+    bk = torch.rand(n, 3, generator=g, dtype=torch.float64)
+    g64, clip = tp.sample_geometry(m, o, d, aabb, S, jitter)
+    moved = g64.clone()
+    moved[1, 7, 0] = moved[1, 7, 0].floor() + 1.5          # next cell along h
+    moved[4, 20, 2] = moved[4, 20, 2].floor() - 0.5        # previous cell along d
+    moved[6, 3, 1] = moved[6, 3, 1].floor() + 0.25         # same cell
+    flip = tp.flip_rays(g64, moved)
+    assert flip.nonzero()[:, 0].tolist() == [1, 4]
+    shapes = dict(depth=(n,), acc=(n,), weights=(n, S), eik_grad=(n, S, 3), sample_sdf=(n, S), rgb=(n, 3), sem=(n, 1))
+    cot = {k: torch.randn(s, generator=g, dtype=torch.float64) for k, s in shapes.items()}
+    for t in cot.values():
+        t[flip] = 0
+    got, gvol, ginv, _ = tp.oracle_train(vol, m, o, d, nrm, aabb, 12.0, S, cot, jitter=jitter, color_dims=3, bkgd_rand=bk,
+                                         depth_clip=clip, chunk=5)
+    whole, gvol1, ginv1, _ = tp.oracle_train(vol, m, o, d, nrm, aabb, 12.0, S, cot, jitter=jitter, color_dims=3, bkgd_rand=bk, chunk=n)
+    assert torch.equal(got['depth'], whole['depth']) and torch.allclose(gvol, gvol1, atol=1e-12)   # chunking keeps the batch clip
+    assert torch.allclose(ginv, ginv1, rtol=1e-12)
+    rep = tp.train_parity(got, {'vol': gvol, 'inv_s': ginv}, cot, vol, m, o, d, nrm, aabb, 12.0, S, g64, jitter=jitter,
+                          color_dims=3, bkgd_rand=bk, chunk=5)
+    print(tp.format_report('selfcheck', rep))
+    assert rep['ok'] and rep['geometry']['max_abs_grid_units'] == 0 and rep['independent']['rays_with_cell_flip'] == 0
+    assert rep['kappa']['same_cells'] == 1.0 and rep['kappa']['independent'] == 1.0
+    for part in ('same_cells', 'independent'):
+        assert all(v[1] == 0 for v in rep[part].values() if isinstance(v, tuple)), rep[part]
+    # the kernel's probe (here: the moved coordinates) flags the same rays, whose cotangents must be zero
+    cot['weights'][1, 0] = 1.0
+    with pytest.raises(AssertionError, match='not zero on a flip ray'):
+        tp.train_parity(got, {'vol': gvol, 'inv_s': ginv}, cot, vol, m, o, d, nrm, aabb, 12.0, S, moved, jitter=jitter,
+                        color_dims=3, bkgd_rand=bk, chunk=5)
