@@ -28,9 +28,10 @@ extern "C" {
 #define SO_ERR_CUDA (-3)          /* a CUDA runtime call or launch failed; see so_last_cuda_error */
 #define SO_ERR_NO_DEVICE (-4)
 
-#define SO_ABI_VERSION 7   /* 2: so_render_train_forward gained pair_workspace; 3: packed render volume entry points;
+#define SO_ABI_VERSION 8   /* 2: so_render_train_forward gained pair_workspace; 3: packed render volume entry points;
                               4: backward of the fused attention cores; 5: the colour pack holds the SH-0 colour;
-                              6: reprojection-loss statistics; 7: training-render sample probe */
+                              6: reprojection-loss statistics; 7: training-render sample probe;
+                              8: occupancy labels and confusion matrix */
 
 /* ABI version of the loaded library (compare with SO_ABI_VERSION). */
 int so_abi_version(void);
@@ -259,6 +260,33 @@ int so_depth_metric_sums(const float* sampled, const float* depth_gt, const uint
  * sdf [n], grad [n,3] (NULL ok), feat [n, n_feat] raw decoded channels 1.. (NULL ok). */
 int so_field_query(const float* vol_sdf, const float* vol_feat, const so_volume_desc* vol_host,
                    const float* points, int64_t n, float* sdf, float* grad, float* feat, void* stream);
+
+/* ---------------------------------------------------------------------------------------
+ * Occupancy evaluation (eval_iou.py:196-270, eval_iou_kitti.py:160-190) from the decoded volume.
+ * The uniform lattice of NeuSHead.get_uniform_sdf (neus_head.py:265-293) is given by its axes xs [nx], ys [ny], zs [nz]
+ * (metres; lattice point (iy, ix, iz) = (xs[ix], ys[iy], zs[iz]), layout [ny, nx, nz]).  A lattice value is the field
+ * query of so_field_query at that point, evaluated on the fly: nothing but the byte labels is written.
+ * Semantics: the argmax (first maximum, like torch.argmax) over the n_sem vol_feat channels [sem_begin, sem_begin + n_sem)
+ * (the head's logits h[..., 4:] are vol_feat channels 3..), mapped through lut (uint8 [n_sem], NULL = the raw argmax).
+ *   so_occ_lattice_labels: occ [ny, nx, nz] = sdf <= thresh;  sem [ny, nx, nz] = occ ? lut[argmax] : 0 (sem NULL: not
+ *     computed).  Equals thresholding / arg-maxing forward_occ's sdf / logits.
+ *   so_occ_sample_labels: points [m, 3] normalised to the lattice's unit cube (u = (p - aabb_min) / expansion); each label
+ *     uses the values of F.grid_sample(lattice[None, None], u[..., [2, 0, 1]] * 2 - 1, bilinear, padding_mode='zeros',
+ *     align_corners=True) for the sdf and every logit channel: occ [m] = sdf' <= thresh, sem [m] = occ ? lut[argmax'] : 0.
+ * Logits are only gathered where occ is set.  Refused: null pointers, sizes < 1, a channel range outside n_feat when sem
+ * is requested. */
+int so_occ_lattice_labels(const float* vol_sdf, const float* vol_feat, const so_volume_desc* vol_host, const float* xs,
+                          int32_t nx, const float* ys, int32_t ny, const float* zs, int32_t nz, float thresh, int32_t sem_begin,
+                          int32_t n_sem, const uint8_t* lut, uint8_t* occ, uint8_t* sem, void* stream);
+int so_occ_sample_labels(const float* vol_sdf, const float* vol_feat, const so_volume_desc* vol_host, const float* xs,
+                         int32_t nx, const float* ys, int32_t ny, const float* zs, int32_t nz, const float* points, int64_t m,
+                         float thresh, int32_t sem_begin, int32_t n_sem, const uint8_t* lut, uint8_t* occ, uint8_t* sem,
+                         void* stream);
+/* Confusion matrix of two label arrays pred, gt (uint8 [n]) over the elements with mask != 0 (mask NULL = all) and
+ * gt != ignore (-1 = none): counts[(n_cls + 1) * g + p] += 1, labels >= n_cls counted in bin n_cls.  counts int64
+ * [(n_cls + 1)^2] is ACCUMULATED (the caller zero-fills it).  1 <= n_cls <= 255.  Integer atomics: deterministic. */
+int so_occ_confusion(const uint8_t* pred, const uint8_t* gt, const uint8_t* mask, int64_t n, int32_t n_cls, int32_t ignore,
+                     int64_t* counts, void* stream);
 
 /* ---------------------------------------------------------------------------------------
  * A7/A8  multi-scale deformable attention forward.  Drop-in for

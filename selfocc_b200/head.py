@@ -11,7 +11,7 @@ import numpy as np
 import torch
 import torch.nn as nn
 
-from . import ops
+from . import occupancy, ops
 from .encoder import _metas_matrix
 from .mapping import GridMeterMapping
 from .registry import HEADS
@@ -395,9 +395,7 @@ class NeuSHead(nn.Module):
 
     def get_uniform_sdf(self, aabb, resolution, device, shift=False):
         """neus_head.py:265-293."""
-        xs = torch.linspace(aabb[0], aabb[3], int((aabb[3] - aabb[0]) / resolution), device=device)
-        ys = torch.linspace(aabb[1], aabb[4], int((aabb[4] - aabb[1]) / resolution), device=device)
-        zs = torch.linspace(aabb[2], aabb[5], int((aabb[5] - aabb[2]) / resolution), device=device)
+        xs, ys, zs = occupancy.lattice_axes(aabb, resolution, device)
         W, H, D = len(xs), len(ys), len(zs)
         xyzs = torch.stack([xs[None, :, None].expand(H, W, D), ys[:, None, None].expand(H, W, D),
                             zs[None, None, :].expand(H, W, D)], dim=-1).flatten(0, 2)
@@ -422,6 +420,34 @@ class NeuSHead(nn.Module):
             return {'sdf': sdf, 'rep': representation, 'sem': sem, 'logits': sem_logits, 'xyz': xyz}
         sdf, xyz = self.get_uniform_sdf(aabb, reso, device=device)
         return {'sdf': sdf, 'rep': representation, 'xyz': xyz}
+
+    @torch.no_grad()
+    def occupancy(self, aabb, resolution, thresh=0.0, lut=None, points=None, expansion=None, representation=None):
+        """Occupancy labels of the prepared frame without materialising forward_occ's lattice (eval_iou.py:196-270,
+        eval_iou_kitti.py:160-190).  ``representation``: decode it first, as forward_occ does; otherwise the volume of the
+        last prepare() / forward() is used.
+
+        points None: labels on the lattice of get_uniform_sdf(aabb, resolution), uint8 [H, W, D]:
+            occ = sdf <= thresh,  sem = occ * lut[argmax(logits)]  (lut None: the raw argmax).
+        points [..., 3] lidar-frame metres: the lattice resampled there as the Occ3D branch does with F.grid_sample
+            (bilinear, zero padding, align_corners=True) over the sdf and every logit channel after normalising the points
+            with (p - aabb[:3]) / expansion (default: the aabb's extent) -> uint8 [...].
+        Returns {'occ': ..., 'sem': ...}, 'sem' only for return_sem heads.  Crops stay with the caller."""
+        f = self.model.field
+        if representation is not None:
+            f.pre_compute_density_color(representation)
+        if f.vol_sdf is None:
+            raise RuntimeError('occupancy() called before prepare()/forward(): no decoded volume')
+        axes = occupancy.lattice_axes(aabb, resolution, f.vol_sdf.device)
+        u = None
+        if points is not None:
+            if expansion is None:
+                expansion = [aabb[3] - aabb[0], aabb[4] - aabb[1], aabb[5] - aabb[2]]
+            u = occupancy.normalise_points(points, aabb, expansion)
+        n_sem = f.color_dims - 3 if self.return_sem else 0
+        occ, sem = occupancy.occupancy_labels(f.vol_sdf, f.vol_feat, f.desc, axes, thresh, sem_begin=3, n_sem=n_sem,
+                                              lut=lut if n_sem else None, points_u=u)
+        return {'occ': occ, 'sem': sem} if n_sem else {'occ': occ}
 
     def forward(self, representation, metas=None, **kwargs):
         """neus_head.py:473-713 (training form: per-sample weights / ts / deltas / eik_grad)."""
