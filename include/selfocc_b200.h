@@ -28,10 +28,10 @@ extern "C" {
 #define SO_ERR_CUDA (-3)          /* a CUDA runtime call or launch failed; see so_last_cuda_error */
 #define SO_ERR_NO_DEVICE (-4)
 
-#define SO_ABI_VERSION 8   /* 2: so_render_train_forward gained pair_workspace; 3: packed render volume entry points;
+#define SO_ABI_VERSION 9   /* 2: so_render_train_forward gained pair_workspace; 3: packed render volume entry points;
                               4: backward of the fused attention cores; 5: the colour pack holds the SH-0 colour;
                               6: reprojection-loss statistics; 7: training-render sample probe;
-                              8: occupancy labels and confusion matrix */
+                              8: occupancy labels and confusion matrix; 9: per-sample loss-term means */
 
 /* ABI version of the loaded library (compare with SO_ABI_VERSION). */
 int so_abi_version(void);
@@ -467,6 +467,27 @@ int so_reproj_stats_backward(const float* ts, const float* deltas, const float* 
                              int32_t n_cam, int32_t rays_per_cam, int32_t S, int32_t img_h, int32_t img_w, float size_h,
                              float size_w, int32_t mode, const float* stats, const float* grad_stats, float* grad_weights,
                              void* stream);
+
+/* ---------------------------------------------------------------------------------------
+ * 8f-2  per-sample regularisers of the training objective: mean of an elementwise function over a fp32 tensor, and the
+ * gradient of that mean.
+ *   SO_SAMPLE_MEAN_EIKONAL  EikonalLoss (loss/eikonal_loss.py:19-21): x is rows of 3, f = (|g|_2 - 1)^2 per row,
+ *                           df/dg = 2 (|g| - 1) g / |g| and 0 where |g| = 0 (torch's vector_norm backward); n % 3 == 0
+ *   SO_SAMPLE_MEAN_ABS      SecondGradLoss (loss/second_grad_loss.py:19-20): f = |x|, df/dx = sign(x), 0 at 0
+ *   SO_SAMPLE_MEAN_NEG_RELU SoftSparsityLoss (loss/sparsity_loss.py:80-81): f = relu(-x), df/dx = -1 where x < 0, else 0
+ * count = n / 3 rows (EIKONAL) or n elements.  x [n] fp32 (4-byte aligned; 128-bit words are used from the first aligned
+ * one on, the unaligned head and the tail element by element).
+ * so_sample_mean_forward -> out[0] = sum f / count (fp32, device scalar).  Each CTA of a fixed grid (a function of n only)
+ *   accumulates in fp64 into workspace, SO_SAMPLE_MEAN_WORKSPACE_BYTES of 8-byte aligned device memory (contents on entry
+ *   ignored), and a second one-CTA launch sums those partials in index order: deterministic, no atomics.
+ * so_sample_mean_backward: grad_out [1] on the device -> grad_x [n] = grad_out[0] / count * df/dx, overwritten.  One
+ *   read of x, one write of grad_x; the scale never reaches the host. */
+#define SO_SAMPLE_MEAN_EIKONAL 0
+#define SO_SAMPLE_MEAN_ABS 1
+#define SO_SAMPLE_MEAN_NEG_RELU 2
+#define SO_SAMPLE_MEAN_WORKSPACE_BYTES 8192
+int so_sample_mean_forward(const float* x, int64_t n, int32_t op, void* workspace, float* out, void* stream);
+int so_sample_mean_backward(const float* x, int64_t n, int32_t op, const float* grad_out, float* grad_x, void* stream);
 
 #ifdef __cplusplus
 }

@@ -9,7 +9,11 @@ training-form render kernels) -> toy loss on depth / weights / eik_grad / rgb ->
 JSON line (ms per step, device timed; peak device memory of the timed steps).  nuScenes_occ geometry: TPV 257x257x25,
 6 cams x 48x100 rays.
     --loss reproj: the toy loss's weights term is replaced by ReprojLossMonoMultiNewCombine (the nuScenes configs' objective,
-    SSIM + automask) on seeded textured 768x1600 previous / current / next images under a small ego motion (synth)."""
+    SSIM + automask) on seeded textured 768x1600 previous / current / next images under a small ego motion (synth).
+    --loss shipped: the toy loss is replaced by nuscenes_occ's whole MultiLoss (reprojection, RGBLossMS with SSIM,
+    EikonalLoss, SecondGradLoss, SemCELossMS), with the head as that config sets it: color_dims = 24, return_sem, and
+    return_second_grad under the declared opt-in assumption (second_grad_assumption=True); seeded synthetic previous /
+    current / next / colour images and semantic labels."""
 import json, os, sys, time
 import numpy as np
 import torch
@@ -27,8 +31,12 @@ if world > 1:
     dist.init_process_group('nccl', device_id=dev)
 margs = dict(synth.NUSC_MAPPING, h_size=[128, 0], h_range=[40.0, 0], w_size=[128, 0], w_range=[40.0, 0], d_size=[24, 0], d_range=[-1.0, 5.4, 5.4])
 rng = [-40.0, -40.0, -1.0, 40.0, 40.0, 5.4]
-cfg = configs.hot_path_config(mapping_args=margs, pc_range=rng, ray_number=(48, 100), ray_img_size=(768, 1600), color_dims=3,
-                              ray_sample_mode='cellular', render_bkgd='random', return_max_depth=False, dropout=0.1)
+loss_mode = sys.argv[sys.argv.index('--loss') + 1] if '--loss' in sys.argv else None
+shipped = loss_mode == 'shipped'
+cfg = configs.hot_path_config(mapping_args=margs, pc_range=rng, ray_number=(48, 100), ray_img_size=(768, 1600), color_dims=24 if shipped else 3,
+                              ray_sample_mode='cellular', render_bkgd='random', return_max_depth=False, dropout=0.1, return_sem=shipped)
+if shipped:
+    cfg['head'].update(return_second_grad=True, second_grad_assumption=True)
 torch.manual_seed(0)
 model = build_head(cfg)
 model.encoder.init_weights()
@@ -42,8 +50,17 @@ metas = [dict(lidar2img=list(l2i), img2lidar=list(i2l), img_shape=(768, 1600))]
 g = torch.Generator().manual_seed(1)
 feats = [torch.randn(1, 6, 96, h, w, generator=g).to(dev) for h, w in synth.fpn_level_shapes(768, 1600)]
 opt = torch.optim.AdamW(model.parameters(), lr=1e-4)
-reproj = None
-if '--loss' in sys.argv and sys.argv[sys.argv.index('--loss') + 1] == 'reproj':
+reproj = objective = None
+if shipped:
+    from bench_train_objective import CFG
+    from selfocc_b200.registry import LOSSES
+    objective = LOSSES.build(dict(type='MultiLoss', loss_cfgs=CFG))
+    prev, nxt = synth.temporal_rig()
+    lab = torch.randint(0, 17, (6, 768, 1600), generator=torch.Generator().manual_seed(3)).to(torch.uint8).numpy()
+    metas[0].update(img2prevImg=torch.tensor(prev, dtype=torch.float32, device=dev), img2nextImg=torch.tensor(nxt, dtype=torch.float32, device=dev),
+                    sem=lab)
+    imgs = synth.textured_images(24, 768, 1600, seed=2).reshape(4, 1, 6, 3, 768, 1600).to(dev)
+if loss_mode == 'reproj':
     from selfocc_b200.loss import ReprojLossMonoMultiNewCombine
     reproj = ReprojLossMonoMultiNewCombine(img_size=[768, 1600], ray_resize=[48, 100])
     prev, nxt = synth.temporal_rig()
@@ -69,6 +86,11 @@ model.forward = lambda feats, metas: _Step.forward(None, feats, metas)
 def step():
     opt.zero_grad(set_to_none=True)
     out = net(feats, metas)
+    if objective is not None:
+        loss, _ = objective(dict(out, curr_imgs=imgs[0], prev_imgs=imgs[1], next_imgs=imgs[2], color_imgs=imgs[3], metas=metas))
+        loss.backward()
+        opt.step()
+        return loss.detach()
     if reproj is None:
         w_term = torch.cat(out['weights']).pow(2).mean()
     else:
@@ -105,7 +127,7 @@ if '--profile' in sys.argv and world == 1:
         torch.cuda.synchronize()
     print(prof.key_averages().table(sort_by='cuda_time_total', row_limit=25))
 if rank == 0:
-  print(json.dumps({'workload': 'nuscenes_occ-like training step, %d GPU(s)%s, fp32, 6x48x100 rays x 256, TPV 257x257x25, colour%s' % (world, ' ray-sharded + DDP' if world > 1 else '', ', reprojection loss' if reproj is not None else ''), 'ms_per_step': ms,
+  print(json.dumps({'workload': 'nuscenes_occ-like training step, %d GPU(s)%s, fp32, 6x48x100 rays x 256, TPV 257x257x25, colour%s' % (world, ' ray-sharded + DDP' if world > 1 else '', ', reprojection loss' if reproj is not None else ', nuscenes_occ MultiLoss (24 colour dims, semantics, second grad)' if shipped else ''), 'ms_per_step': ms,
                   'rays_per_s': 28800 / (ms * 1e-3), 'library_launches_per_step': (_lib.launch_count() - l0) / K, 'peak_mem_gb': peak_gb,
                   'loss': float(last), 'finite': bool(torch.isfinite(last))}))
 if world > 1:

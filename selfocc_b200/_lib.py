@@ -8,7 +8,7 @@ import os
 
 _PKG = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.environ.get('SELFOCC_B200_LIB') or os.path.join(_PKG, 'lib', 'libselfocc_b200.so')   # env: experimental variant
-ABI_VERSION = 8
+ABI_VERSION = 9
 
 
 class AxisMap(C.Structure):
@@ -96,6 +96,8 @@ SIGNATURES = {
     'so_occ_lattice_labels': (C.c_int, [_P, _P, C.POINTER(VolumeDesc), _P, _I, _P, _I, _P, _I, _F, _I, _I, _P, _P, _P, _P]),
     'so_occ_sample_labels': (C.c_int, [_P, _P, C.POINTER(VolumeDesc), _P, _I, _P, _I, _P, _I, _P, _L, _F, _I, _I, _P, _P, _P, _P]),
     'so_occ_confusion': (C.c_int, [_P, _P, _P, _L, _I, _I, _P, _P]),
+    'so_sample_mean_forward': (C.c_int, [_P, _L, _I, _P, _P, _P]),
+    'so_sample_mean_backward': (C.c_int, [_P, _L, _I, _P, _P, _P]),
 }
 
 _lib = None

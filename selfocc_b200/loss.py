@@ -1,6 +1,8 @@
-"""Photometric reprojection losses of SelfOcc on the per-ray statistics kernel (SURVEY.md 8f-2):
-drop-in ``ReprojLossMonoMultiNewCombine`` (reference loss/reproj_loss_mono_multi_new_combine.py) and
-``ReprojLossMonoMultiNew`` (loss/reproj_loss_mono_multi_new.py).
+"""The training objectives of SelfOcc's shipped configs (SURVEY.md 8f-2): drop-in ``MultiLoss`` and every term it builds.
+
+Photometric reprojection losses on the per-ray statistics kernel: ``ReprojLossMonoMultiNewCombine`` (reference
+loss/reproj_loss_mono_multi_new_combine.py) and ``ReprojLossMonoMultiNew`` (loss/reproj_loss_mono_multi_new.py).  The other
+terms (eikonal, second-grad, sparsity, RGB, semantic, edge) and ``MultiLoss`` follow in the second half of this file.
 
 The per-sample work (reprojection of every sample into the previous / next frame, bilinear colour gathers, masks, the
 weighted sums over each ray) runs in ``so_reproj_stats_forward`` / ``_backward`` (csrc/reproj.cu) through
@@ -173,3 +175,240 @@ class ReprojLossMonoMultiNew(_ReprojLoss):
         self._log(idx, 1)
         self.iter_counter += 1
         return (loss.mean(1).sum() / num_cams).float()
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# The remaining terms of the shipped configs' objectives and MultiLoss.
+#
+# EikonalLoss, SecondGradLoss and SoftSparsityLoss read the largest per-sample tensors of the objective (eik_grad,
+# second_grad: [rays, S, 3]; uniform_sdf: the lattice) and run on so_sample_mean_forward / _backward (csrc/loss_terms.cu):
+# one read forward, one read and one write backward, no per-sample temporaries.  RGBLossMS, SemLossMS, SemCELossMS and
+# EdgeLoss3DMS work per ray ([cameras, rays] grids) and stay in torch, batched over cameras.
+
+class _Term(nn.Module):
+    """BaseLoss (reference loss/base_loss.py): weight * loss over the inputs named by input_dict."""
+    DEFAULT_KEYS = ()
+
+    def __init__(self, weight=1.0, input_dict=None):
+        super().__init__()
+        self.weight = weight
+        self.input_dict = dict(input_dict) if input_dict is not None else {k: k for k in self.DEFAULT_KEYS}
+        self.writer = None
+
+    def forward(self, inputs):
+        return self.weight * self.loss_func(**{k: inputs[v] for k, v in self.input_dict.items()})
+
+
+@LOSSES.register_module()
+class EikonalLoss(_Term):
+    """mean over samples of (|eik_grad|_2 - 1)^2 (loss/eikonal_loss.py)."""
+    DEFAULT_KEYS = ('eik_grad',)
+
+    def __init__(self, weight=1.0, input_dict=None, **kwargs):
+        super().__init__(weight, input_dict)
+
+    def loss_func(self, eik_grad):
+        return ops.SampleMeanFunction.apply(eik_grad, 'eikonal')
+
+
+@LOSSES.register_module()
+class SecondGradLoss(_Term):
+    """mean |second_grad| (loss/second_grad_loss.py)."""
+    DEFAULT_KEYS = ('second_grad',)
+
+    def __init__(self, weight=1.0, input_dict=None, **kwargs):
+        super().__init__(weight, input_dict)
+
+    def loss_func(self, second_grad):
+        return ops.SampleMeanFunction.apply(second_grad, 'abs')
+
+
+@LOSSES.register_module()
+class SoftSparsityLoss(_Term):
+    """mean relu(-density) (loss/sparsity_loss.py SoftSparsityLoss); the shipped configs feed it uniform_sdf."""
+    DEFAULT_KEYS = ('density',)
+
+    def __init__(self, weight=1.0, input_dict=None, **kwargs):
+        super().__init__(weight, input_dict)
+
+    def loss_func(self, density):
+        return ops.SampleMeanFunction.apply(density, 'neg_relu')
+
+
+def sample_at_rays(imgs, rays, img_size, padding):
+    """Bilinear samples of imgs [M, C, H, W] at the ray pixels rays [R, 2] (x, y in img_size pixels) -> [M, C, R]: the
+    reference's F.grid_sample(align_corners=True) at (x / img_size[1], y / img_size[0]) * 2 - 1, normalised by the loss's
+    img_size, not by the image's shape.  padding: 'zeros' (RGBLossMS) or 'border' (EdgeLoss3DMS)."""
+    rays = rays.to(imgs.dtype)
+    pix = torch.stack([rays[:, 0] / img_size[1], rays[:, 1] / img_size[0]], -1)     # scalar divisions: no host copy
+    grid = (pix * 2 - 1).reshape(1, 1, -1, 2).expand(imgs.shape[0], 1, -1, 2)
+    return F.grid_sample(imgs, grid, mode='bilinear', padding_mode=padding, align_corners=True)[:, :, 0]
+
+
+def _single_rays(ms_rays, what):
+    if isinstance(ms_rays, (list, tuple)):
+        raise NotImplementedError('%s: list-valued ms_rays is not supported (the reference raises too)' % what)
+    return ms_rays
+
+
+def _check_grid(ray_resize, R, what):
+    if R != ray_resize[0] * ray_resize[1]:
+        raise ValueError('%s needs the rays to fill ray_resize %s, got %d rays (ray sharding or a partial ray set)'
+                         % (what, list(ray_resize), R))
+
+
+@LOSSES.register_module()
+class RGBLossMS(_Term):
+    """Per scale mean |colour - gt| at the ray pixels, 0.15 l1 + 0.85 SSIM over the ray grid when SSIM is on
+    (loss/rgb_loss_ms.py RGBLossMS)."""
+    DEFAULT_KEYS = ('ms_colors', 'ms_rays', 'gt_imgs')
+
+    def __init__(self, weight=1.0, img_size=None, no_ssim=True, ray_resize=None, input_dict=None, **kwargs):
+        super().__init__(weight, input_dict)
+        assert img_size is not None
+        self.img_size = list(img_size)
+        self.no_ssim = no_ssim or ray_resize is None
+        self.ray_resize = list(ray_resize) if ray_resize is not None else None
+
+    def loss_func(self, ms_colors, ms_rays, gt_imgs):
+        rays = _single_rays(ms_rays, 'RGBLossMS')
+        bs, num_cams = gt_imgs.shape[:2]
+        R = rays.shape[0]
+        if not self.no_ssim:
+            _check_grid(self.ray_resize, R, 'RGBLossMS with SSIM')
+        gt = sample_at_rays(gt_imgs.flatten(0, 1), rays, self.img_size, 'zeros')          # [B*N, 3, R]
+        gt_grid = None if self.no_ssim else gt.reshape(bs * num_cams, 3, *self.ray_resize)
+        gt = gt.reshape(bs, num_cams, 3, R).transpose(-1, -2)
+        tot = 0.
+        for color in ms_colors:
+            loss = (color - gt).abs().mean()
+            if not self.no_ssim:
+                c = color.reshape(bs * num_cams, *self.ray_resize, 3).permute(0, 3, 1, 2)
+                loss = 0.15 * loss + 0.85 * ssim(c, gt_grid).mean()
+            tot = tot + loss
+        return tot / len(ms_colors)
+
+
+def _sem_labels(metas, rays, dev):
+    """metas[b]['sem'] [N, H, W] integer labels -> labels at the ray pixels, int64 [B, N, R] on dev.  numpy labels travel
+    once, pinned and non-blocking, in their own dtype; the gather and the widening run on the device."""
+    lab = [m['sem'] for m in metas]
+    if isinstance(lab[0], np.ndarray):
+        t = torch.from_numpy(np.ascontiguousarray(np.stack(lab)))
+        if dev.type == 'cuda':
+            t = t.pin_memory()
+        t = t.to(dev, non_blocking=True)
+    elif isinstance(lab[0], torch.Tensor):
+        t = torch.stack(lab).to(dev, non_blocking=True)
+    else:
+        raise NotImplementedError('metas[i]["sem"] must be a numpy array or a tensor')
+    r = rays.to(dev).long()
+    return t[:, :, r[:, 1], r[:, 0]].long()
+
+
+class _SemTerm(_Term):
+    DEFAULT_KEYS = ('sem', 'metas', 'ms_rays')
+
+    def __init__(self, weight=1.0, img_size=None, ray_resize=None, input_dict=None, **kwargs):
+        super().__init__(weight, input_dict)
+        assert img_size is not None
+        self.img_size = img_size
+        self.ray_resize = ray_resize
+
+    def loss_func(self, sem, metas, ms_rays):
+        rays = _single_rays(ms_rays, type(self).__name__)
+        gt = _sem_labels(metas, rays, sem[0].device)
+        return sum(self.term(s, gt) for s in sem) / len(sem)
+
+
+@LOSSES.register_module()
+class SemLossMS(_SemTerm):
+    """Binary cross-entropy of the clamped semantic probabilities against one-hot labels at the ray pixels
+    (loss/rgb_loss_ms.py SemLossMS; F.binary_cross_entropy clamps the log at -100)."""
+
+    @staticmethod
+    def term(s, gt):
+        return F.binary_cross_entropy(torch.clamp(s, 0, 1), F.one_hot(gt, num_classes=s.shape[-1]).to(s.dtype))
+
+
+@LOSSES.register_module()
+class SemCELossMS(_SemTerm):
+    """Cross-entropy -log(clamp(s, 1e-6, 1)) of the label class, mean over rays (loss/rgb_loss_ms.py SemCELossMS).  The
+    reference's sum over one-hot classes has exactly one non-zero term; this gathers it."""
+
+    @staticmethod
+    def term(s, gt):
+        return -torch.log(torch.clamp(s.gather(-1, gt.unsqueeze(-1)), 1e-6, 1)).mean()
+
+
+def _smooth(disp, img):
+    """Edge-aware smoothness of disp [M, 1, h, w] weighted by exp(-|d img|) (edge_loss_3d_ms.py get_smooth_loss)."""
+    gx = (disp[:, :, :, :-1] - disp[:, :, :, 1:]).abs() * torch.exp(-(img[:, :, :, :-1] - img[:, :, :, 1:]).abs().mean(1, True))
+    gy = (disp[:, :, :-1, :] - disp[:, :, 1:, :]).abs() * torch.exp(-(img[:, :, :-1, :] - img[:, :, 1:, :]).abs().mean(1, True))
+    return gx.mean() + gy.mean()
+
+
+@LOSSES.register_module()
+class EdgeLoss3DMS(_Term):
+    """Edge-aware smoothness of the mean-normalised depth over the ray grid, weighted by the current image at the ray
+    pixels (padding 'border'); with use_inf_mask the depth is blended towards max_depths by 1 - ms_accs
+    (loss/edge_loss_3d_ms.py)."""
+    DEFAULT_KEYS = ('curr_imgs', 'ms_depths', 'ms_rays')
+
+    def __init__(self, weight=1.0, input_dict=None, **kwargs):
+        super().__init__(weight, input_dict)
+        self.img_size = list(kwargs.get('img_size', [768, 1600]))
+        self.ray_resize = kwargs.get('ray_resize', None)
+        self.use_inf_mask = kwargs.get('use_inf_mask', False)
+        assert self.ray_resize is not None
+        self.ray_resize = list(self.ray_resize)
+
+    def loss_func(self, curr_imgs, ms_depths, ms_rays, ms_accs=None, max_depths=None):
+        if self.use_inf_mask:
+            assert ms_accs is not None and max_depths is not None
+        if not isinstance(ms_rays, (list, tuple)):
+            ms_rays = [ms_rays] * len(ms_depths)
+        bs, num_cams, num_rays = ms_depths[0].shape
+        _check_grid(self.ray_resize, num_rays, 'EdgeLoss3DMS')
+        imgs = curr_imgs.flatten(0, 1)
+        tot = 0.
+        for scale, (depth, rays) in enumerate(zip(ms_depths, ms_rays)):
+            rgb = sample_at_rays(imgs, rays, self.img_size, 'border').reshape(bs * num_cams, -1, *self.ray_resize)
+            if self.use_inf_mask:
+                depth = depth * ms_accs[scale] + max_depths[scale] * (1 - ms_accs[scale])
+            depth = depth.reshape(bs * num_cams, 1, *self.ray_resize)
+            norm = depth / (depth.mean(2, True).mean(3, True) + 1e-6)
+            tot = tot + _smooth(norm, rgb)
+        return tot / len(ms_depths)
+
+
+@LOSSES.register_module()
+class MultiLoss(nn.Module):
+    """Sum of the terms built from loss_cfgs through LOSSES (loss/multi_loss.py) -> (tot_loss, loss_dict).
+    loss_dict maps each term's class name to its detached 0-d device tensor, not a Python float: nothing here reads the
+    host, and f'{v:.5f}' formats the tensor as it would the float.  An attached ``writer`` (add_scalar(tag, value, step))
+    logs every term and the total on every 10th call, as the reference does; that logging reads the host."""
+
+    def __init__(self, loss_cfgs):
+        super().__init__()
+        assert isinstance(loss_cfgs, list)
+        self.num_losses = len(loss_cfgs)
+        self.losses = nn.ModuleList([LOSSES.build(c) for c in loss_cfgs])
+        self.iter_counter = 0
+        self.writer = None
+
+    def forward(self, inputs):
+        loss_dict = {}
+        tot_loss = 0.
+        log = self.writer is not None and self.iter_counter % 10 == 0
+        for loss_func in self.losses:
+            loss = loss_func(inputs)
+            tot_loss = tot_loss + loss
+            name = loss_func.__class__.__name__
+            loss_dict[name] = loss.detach()
+            if log:
+                self.writer.add_scalar(f'loss/{name}', loss.detach().item(), self.iter_counter)
+        if log:
+            self.writer.add_scalar('loss/total', tot_loss.detach().item(), self.iter_counter)
+        self.iter_counter += 1
+        return tot_loss, loss_dict

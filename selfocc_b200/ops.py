@@ -779,3 +779,45 @@ class ReprojStatsFunction(torch.autograd.Function):
         stats, = ctx.saved_tensors
         _reproj_call('so_reproj_stats_backward', cfg, (), (_p(stats), _p(_chk(g_stats.contiguous(), name='grad_stats')), _p(gw)))
         return (None,) + tuple(gw[i].view(shp) for i, shp in enumerate(ctx.shapes))
+
+
+# --------------------------------------------------------------------------------------- 8f-2 per-sample loss terms
+SAMPLE_MEAN_OPS = {'eikonal': 0, 'abs': 1, 'neg_relu': 2}     # SO_SAMPLE_MEAN_EIKONAL / _ABS / _NEG_RELU
+SAMPLE_MEAN_WORKSPACE_BYTES = 8192                             # SO_SAMPLE_MEAN_WORKSPACE_BYTES
+
+
+class SampleMeanFunction(torch.autograd.Function):
+    """Mean of an elementwise function over a fp32 CUDA tensor (so_sample_mean_forward / _backward).
+    apply(x, op): op 'eikonal' -> mean over rows of (|x[..., :3]|_2 - 1)^2 (x.shape[-1] == 3); 'abs' -> mean |x|;
+    'neg_relu' -> mean relu(-x).  Returns a 0-d fp32 tensor; the gradient is torch's subgradient of the same expression
+    (0 at a zero norm, at x = 0, and for relu(-x) at x >= 0).  Non-contiguous input is copied contiguous."""
+
+    @staticmethod
+    def forward(ctx, x, op):
+        if op not in SAMPLE_MEAN_OPS:
+            raise ValueError('op must be one of %s, got %r' % (sorted(SAMPLE_MEAN_OPS), op))
+        if isinstance(x, torch.Tensor) and x.is_cuda and x.dtype == torch.float32:
+            x = x.contiguous()
+        _chk(x, name='x')
+        if op == 'eikonal' and (x.dim() == 0 or x.shape[-1] != 3):
+            raise ValueError('eikonal: rows of 3 expected, got shape %s' % (tuple(x.shape),))
+        if x.numel() == 0:
+            raise ValueError('%s: the mean of an empty tensor is undefined' % op)
+        lib = _lib.load()
+        ws = torch.empty(SAMPLE_MEAN_WORKSPACE_BYTES // 8, dtype=torch.float64, device=x.device)
+        out = torch.empty((), device=x.device)
+        _lib.check(lib.so_sample_mean_forward(_p(x), x.numel(), SAMPLE_MEAN_OPS[op], _p(ws), _p(out), _stream()),
+                   'so_sample_mean_forward')
+        ctx.op = op
+        ctx.save_for_backward(x)
+        return out
+
+    @staticmethod
+    @torch.autograd.function.once_differentiable
+    def backward(ctx, g):
+        x, = ctx.saved_tensors
+        g = _chk(g.reshape(1).contiguous(), name='grad_out')
+        gx = torch.empty_like(x)
+        _lib.check(_lib.load().so_sample_mean_backward(_p(x), x.numel(), SAMPLE_MEAN_OPS[ctx.op], _p(g), _p(gx), _stream()),
+                   'so_sample_mean_backward')
+        return gx, None
