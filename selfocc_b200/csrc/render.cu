@@ -127,9 +127,8 @@ __global__ void __launch_bounds__(SO_RENDER_BLOCK, SO_RENDER_MIN_CTAS) render_in
   // g(t) = g0 + gd * t along the ray, one FMA per axis per sample
   const bool affine = FAST || (V.ax[0].k1 == 0.f && V.ax[1].k1 == 0.f && V.ax[2].k1 == 0.f);
   const float kh0 = V.ax[0].k0, kw0 = V.ax[1].k0, kd0 = V.ax[2].k0;
-  const float gh0 = fmaf(o[1] - V.ax[0].start, kh0, V.ax[0].offset), gdh = d[1] * kh0;
-  const float gw0 = fmaf(o[0] - V.ax[1].start, kw0, V.ax[1].offset), gdw = d[0] * kw0;
-  const float gd0 = fmaf(o[2] - V.ax[2].start, kd0, V.ax[2].offset), gdd = d[2] * kd0;
+  float gh0, gdh, gw0, gdw, gd0, gdd;
+  affine_grid_ray(V, o, d, gh0, gdh, gw0, gdw, gd0, gdd);
   const int Hm1 = V.H - 1, Wm1 = V.W - 1, Zm1 = V.Z - 1;
   const bool anneal_done = FAST || P.cos_anneal == 1.0f;   // -(relu(-tc)) == min(tc, 0)
   const float k_log2 = P.inv_s * 1.4426950408889634f;       // inv_s * log2(e)
@@ -203,12 +202,10 @@ __global__ void __launch_bounds__(SO_RENDER_BLOCK, SO_RENDER_MIN_CTAS) render_in
     float cand = FAST ? w : (delta < eps_len ? 0.f : __fdividef(w, delta));   // FAST: delta is a positive per-ray constant
     if (cand > best) { best = cand; best_i = s; best_mid = mid; }
     if (HAS_RGB) {
-      float f[3];
+      float f[3], col[3], raw[3];
       gather_feat<3>(V, t, 0, f);
-      float r0 = f[0] * kC0, r1 = f[1] * kC0, r2 = f[2] * kC0;
-      if (P.sh_act == 0) { r0 = fmaxf(r0 + 0.5f, 0.f); r1 = fmaxf(r1 + 0.5f, 0.f); r2 = fmaxf(r2 + 0.5f, 0.f); }
-      else { r0 = sigmoidf_acc(r0); r1 = sigmoidf_acc(r1); r2 = sigmoidf_acc(r2); }
-      c_r = fmaf(w, r0, c_r); c_g = fmaf(w, r1, c_g); c_b = fmaf(w, r2, c_b);
+      colour_act(P.sh_act, f, col, raw);
+      c_r = fmaf(w, col[0], c_r); c_g = fmaf(w, col[1], c_g); c_b = fmaf(w, col[2], c_b);
     }
     if (HAS_SEM) {
       // rendered semantics = sum_s w * softmax(logits) (bev_nerf.py:147-148 + SemanticRenderer)
@@ -224,13 +221,9 @@ __global__ void __launch_bounds__(SO_RENDER_BLOCK, SO_RENDER_MIN_CTAS) render_in
   if (!valid) return;
   if (FAST && delta_c < eps_len) { best_i = 0; best_mid = fmaf(0.5f * step, span, tn); }   // all candidates are 0: first index
 
-  long long chunk = R.chunk_len > 0 ? gid / R.chunk_len : 0;
-  float lo = __ldg(ws + 2 * chunk), hi = __ldg(ws + 2 * chunk + 1);
-  if (depth) {
-    float dd = dsum / (acc + 1e-10f);
-    dd = fminf(fmaxf(dd, lo), hi);
-    depth[lid] = dd / nrm;
-  }
+  float lo, hi;
+  depth_clip_range(ws, R, gid, lo, hi);
+  if (depth) depth[lid] = clipped_depth(dsum, acc, lo, hi, nrm);
   if (max_depth) max_depth[lid] = best_mid / nrm;
   if (max_idx) max_idx[lid] = best_i;
   if (acc_out) acc_out[lid] = acc;
@@ -239,15 +232,7 @@ __global__ void __launch_bounds__(SO_RENDER_BLOCK, SO_RENDER_MIN_CTAS) render_in
     normal_vis[3 * lid + 1] = (n1 + 1.0f) * 0.5f;
     normal_vis[3 * lid + 2] = (n2 + 1.0f) * 0.5f;
   }
-  if (HAS_RGB && rgb_out) {
-    float b0, b1, b2;
-    if (P.bkgd_mode == 2) { b0 = bkgd_rand[3 * lid]; b1 = bkgd_rand[3 * lid + 1]; b2 = bkgd_rand[3 * lid + 2]; }
-    else { b0 = b1 = b2 = (P.bkgd_mode == 1) ? 1.f : 0.f; }
-    float rem = 1.0f - acc;
-    float r = fmaf(b0, rem, c_r), g = fmaf(b1, rem, c_g), b = fmaf(b2, rem, c_b);
-    if (P.eval_clamp) { r = fminf(fmaxf(r, 0.f), 1.f); g = fminf(fmaxf(g, 0.f), 1.f); b = fminf(fmaxf(b, 0.f), 1.f); }
-    rgb_out[3 * lid] = r; rgb_out[3 * lid + 1] = g; rgb_out[3 * lid + 2] = b;
-  }
+  if (HAS_RGB && rgb_out) store_rgb(P, bkgd_rand, lid, acc, c_r, c_g, c_b, rgb_out);
   if (HAS_SEM && sem_out)
     for (int c = 0; c < n_sem; ++c) sem_out[lid * n_sem + c] = sem[c];
 }
@@ -280,25 +265,18 @@ extern "C" int so_render_infer(const float* vol_sdf, const float* vol_feat, cons
                                const so_render_params* pr, const float* bkgd_rand, float* depth, float* max_depth,
                                int64_t* max_idx, float* acc, float* normal_vis, float* rgb, float* sem,
                                float* workspace, void* stream) {
-  if (!vol_sdf || !cam_mats || !rd || !pr || !workspace) return SO_ERR_INVALID_ARG;
-  int rc = validate_volume(vol_host);
+  int rc = check_render_operands(vol_sdf, workspace, cam_mats, rd, pr, vol_host);
   if (rc) return rc;
-  if (rd->n_cam < 1 || rd->rays_per_cam < 1 || pr->num_samples < 1) return SO_ERR_INVALID_ARG;
-  if (!pix && (rd->nx < 1 || rd->ny < 1 || (int64_t)rd->nx * rd->ny != rd->rays_per_cam)) return SO_ERR_INVALID_ARG;
-  int64_t total = (int64_t)rd->n_cam * rd->rays_per_cam;
-  if (rd->ray_begin < 0 || rd->ray_count < 0 || rd->ray_begin + rd->ray_count > total) return SO_ERR_INVALID_ARG;
-  bool want_rgb = rgb != nullptr, want_sem = sem != nullptr;
-  if (want_rgb && (vol_host->n_feat < 3 || !vol_feat)) return SO_ERR_INVALID_ARG;
-  if (want_sem && (vol_host->n_feat <= 3 || !vol_feat || !want_rgb)) return SO_ERR_INVALID_ARG;
-  if (want_sem && vol_host->n_feat - 3 > kMaxSem) return SO_ERR_UNSUPPORTED;
-  if (pr->bkgd_mode == 2 && want_rgb && !bkgd_rand) return SO_ERR_INVALID_ARG;
-  if (pr->bkgd_mode < 0 || pr->bkgd_mode > 2 || pr->sh_act < 0 || pr->sh_act > 1) return SO_ERR_INVALID_ARG;
+  if (pr->num_samples < 1) return SO_ERR_INVALID_ARG;
+  RayDev R;
+  if ((rc = make_ray_dev(rd, cam_mats, pix, &R))) return rc;
+  const bool want_rgb = rgb != nullptr, want_sem = sem != nullptr;
+  if (want_sem && !want_rgb) return SO_ERR_INVALID_ARG;
+  if ((rc = check_shading(vol_host, vol_feat, pr, want_rgb, want_sem, bkgd_rand))) return rc;
   if (rd->ray_count == 0) return SO_OK;
   cudaStream_t st = (cudaStream_t)stream;
 
   VolumeDev V = make_volume(*vol_host, vol_sdf, vol_feat);
-  RayDev R;
-  if ((rc = make_ray_dev(rd, cam_mats, pix, &R))) return rc;
   RenderDev P = make_render_dev(*pr, nullptr);
 
   if ((rc = launch_depth_bounds(R, P, workspace, st))) return rc;
@@ -306,8 +284,7 @@ extern "C" int so_render_infer(const float* vol_sdf, const float* vol_feat, cons
   unsigned grid = (unsigned)ceil_div64(rd->ray_count, SO_RENDER_BLOCK);
   ProfScope prof(0, st);
   long long* midx = reinterpret_cast<long long*>(max_idx);
-  const bool fast = V.ax[0].k1 == 0.f && V.ax[1].k1 == 0.f && V.ax[2].k1 == 0.f && (P.S & (P.S - 1)) == 0 &&
-                    P.cos_anneal == 1.0f && P.anchor_mid;
+  const bool fast = uniform_affine_march(V, P);
 #define SO_RENDER(RGB, SEM, F) render_infer_kernel<RGB, SEM, F><<<grid, SO_RENDER_BLOCK, 0, st>>>(V, R, P, workspace, bkgd_rand, depth, max_depth, midx, acc, normal_vis, rgb, sem)
   if (want_sem) { if (fast) SO_RENDER(true, true, true); else SO_RENDER(true, true, false); }
   else if (want_rgb) { if (fast) SO_RENDER(true, false, true); else SO_RENDER(true, false, false); }

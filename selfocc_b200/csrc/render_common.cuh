@@ -1,4 +1,5 @@
-// Device functions shared by the inference and training render kernels (render.cu, render_train.cu).
+// Device functions and host-side checks shared by the inference and training render kernels (render.cu,
+// render_fast.cu, render_train.cu).
 #pragma once
 #include "common.cuh"
 #include <math.h>
@@ -21,6 +22,8 @@ struct RenderDev {
   int anchor_mid, sh_act, bkgd_mode, eval_clamp;
   const float* jitter;  // [total rays][S + 1] stratified-sampling uniforms (training) or nullptr
 };
+
+constexpr int kMaxSem = 32;  // rendered semantic classes (n_feat - 3) supported per ray
 
 inline RenderDev make_render_dev(const so_render_params& pr, const float* jitter) {
   RenderDev P;
@@ -46,6 +49,44 @@ inline int make_ray_dev(const so_ray_desc* rd, const float* cam_mats, const floa
   return SO_OK;
 }
 
+// ---- argument checks of the render entry points.  Each entry point applies them in a fixed order with make_ray_dev,
+// and that order decides which code it returns when several checks fail (SO_ERR_INVALID_ARG or SO_ERR_UNSUPPORTED).
+
+// the operands every render entry point needs: the volume (`vol`), one buffer it writes (`out`), cameras, rays,
+// parameters and a valid volume descriptor
+inline int check_render_operands(const void* vol, const void* out, const float* cam_mats, const so_ray_desc* rd,
+                                 const so_render_params* pr, const so_volume_desc* d) {
+  if (!vol || !out || !cam_mats || !rd || !pr) return SO_ERR_INVALID_ARG;
+  return validate_volume(d);
+}
+
+inline int check_background(const so_render_params* pr, bool want_rgb, const float* bkgd_rand) {
+  if (pr->bkgd_mode == 2 && want_rgb && !bkgd_rand) return SO_ERR_INVALID_ARG;
+  if (pr->bkgd_mode < 0 || pr->bkgd_mode > 2 || pr->sh_act < 0 || pr->sh_act > 1) return SO_ERR_INVALID_ARG;
+  return SO_OK;
+}
+
+// the feature channels that colour (0..2) and rendered semantics (3..n_feat-1) read, then the background
+inline int check_shading(const so_volume_desc* d, const float* vol_feat, const so_render_params* pr, bool want_rgb,
+                         bool want_sem, const float* bkgd_rand) {
+  if (want_rgb && (d->n_feat < 3 || !vol_feat)) return SO_ERR_INVALID_ARG;
+  if (want_sem && (d->n_feat <= 3 || !vol_feat)) return SO_ERR_INVALID_ARG;
+  if (want_sem && d->n_feat - 3 > kMaxSem) return SO_ERR_UNSUPPORTED;
+  return check_background(pr, want_rgb, bkgd_rand);
+}
+
+// The uniform affine march: affine metre->grid map (no outer ring), power-of-two S, cos-anneal finished, mid-point
+// anchor (every shipped config).  Its bins are uniform in t and its grid coordinates are one FMA per axis, which the FAST
+// kernel paths assume; each caller adds its own bound on S.
+inline bool uniform_affine_march(const VolumeDev& V, const RenderDev& P) {
+  return V.ax[0].k1 == 0.f && V.ax[1].k1 == 0.f && V.ax[2].k1 == 0.f && (P.S & (P.S - 1)) == 0 && P.cos_anneal == 1.0f &&
+         P.anchor_mid;
+}
+
+// z-pair copy of the sdf volume, float2 {v[z], v[z + 1]} per voxel (zpair_pack_kernel): its size in floats, its launch
+inline int64_t zpair_floats(const so_volume_desc& d) { return 2 * (int64_t)d.H * d.W * d.zpitch; }
+void launch_zpair_pack(const float* vol_sdf, const so_volume_desc& d, float* pack, cudaStream_t st);
+
 __device__ __forceinline__ void make_ray(const RayDev& R, long long gid, float o[3], float d[3], float& nrm) {
   int cam = (int)(gid / R.rays_per_cam);
   int r = (int)(gid - (long long)cam * R.rays_per_cam);
@@ -65,6 +106,14 @@ __device__ __forceinline__ void make_ray(const RayDev& R, long long gid, float o
   o[0] = __ldg(M + 3); o[1] = __ldg(M + 7); o[2] = __ldg(M + 11);
   nrm = sqrtf(dx * dx + dy * dy + dz * dz);
   d[0] = dx / nrm; d[1] = dy / nrm; d[2] = dz / nrm;
+}
+
+// affine grid-space ray (mapping without outer ring): g(t) = g0 + gd * t per grid axis; h, w, d follow metre y, x, z
+__device__ __forceinline__ void affine_grid_ray(const VolumeDev& V, const float o[3], const float d[3], float& gh0, float& gdh,
+                                                float& gw0, float& gdw, float& gd0, float& gdd) {
+  gh0 = fmaf(o[1] - V.ax[0].start, V.ax[0].k0, V.ax[0].offset); gdh = d[1] * V.ax[0].k0;
+  gw0 = fmaf(o[0] - V.ax[1].start, V.ax[1].k0, V.ax[1].offset); gdw = d[0] * V.ax[1].k0;
+  gd0 = fmaf(o[2] - V.ax[2].start, V.ax[2].k0, V.ax[2].offset); gdd = d[2] * V.ax[2].k0;
 }
 
 // upstream AABBBoxCollider: slab test with 1/(d + 1e-6)
@@ -211,7 +260,44 @@ __device__ __forceinline__ float neus_alpha_log2(float s2, float h2) {
 
 constexpr float kC0 = 0.28209479177387814f;  // sh_render.py:4
 
-constexpr int kMaxSem = 32;  // rendered semantic classes (n_feat - 3) supported per ray
+// SH degree 0 colour of the interpolated features f (sh_render.py:84-94): raw = C0 f, col = relu(raw + 1/2) (sh_act 0)
+// or sigmoid(raw)
+__device__ __forceinline__ void colour_act(int sh_act, const float f[3], float col[3], float raw[3]) {
+#pragma unroll
+  for (int c = 0; c < 3; ++c) raw[c] = f[c] * kC0;
+  if (sh_act == 0) {
+#pragma unroll
+    for (int c = 0; c < 3; ++c) col[c] = fmaxf(raw[c] + 0.5f, 0.f);
+  } else {
+#pragma unroll
+    for (int c = 0; c < 3; ++c) col[c] = sigmoidf_acc(raw[c]);
+  }
+}
+
+// ---- per-ray tails
+// [lo, hi] clip of ray gid's expected depth: the mid-point range of its reference chunk (launch_depth_bounds)
+__device__ __forceinline__ void depth_clip_range(const float* ws, const RayDev& R, long long gid, float& lo, float& hi) {
+  const long long chunk = R.chunk_len > 0 ? gid / R.chunk_len : 0;
+  lo = __ldg(ws + 2 * chunk);
+  hi = __ldg(ws + 2 * chunk + 1);
+}
+// expected depth: clip(dsum / acc, lo, hi) / |dir|
+__device__ __forceinline__ float clipped_depth(float dsum, float acc, float lo, float hi, float nrm) {
+  return fminf(fmaxf(dsum / (acc + 1e-10f), lo), hi) / nrm;
+}
+
+// rgb[i] = colour + (1 - acc) * background (black, white or bkgd_rand[i] for bkgd_mode 0 / 1 / 2), clamped to [0, 1] in
+// eval mode
+__device__ __forceinline__ void store_rgb(const RenderDev& P, const float* bkgd_rand, long long i, float acc, float cr, float cg,
+                                          float cb, float* rgb) {
+  float b[3];
+  if (P.bkgd_mode == 2) { b[0] = bkgd_rand[3 * i]; b[1] = bkgd_rand[3 * i + 1]; b[2] = bkgd_rand[3 * i + 2]; }
+  else b[0] = b[1] = b[2] = (P.bkgd_mode == 1) ? 1.f : 0.f;
+  const float rem = 1.0f - acc;
+  float r = fmaf(b[0], rem, cr), g = fmaf(b[1], rem, cg), bl = fmaf(b[2], rem, cb);
+  if (P.eval_clamp) { r = __saturatef(r); g = __saturatef(g); bl = __saturatef(bl); }
+  rgb[3 * i] = r; rgb[3 * i + 1] = g; rgb[3 * i + 2] = bl;
+}
 
 int launch_depth_bounds(const RayDev& R, const RenderDev& P, float* ws, cudaStream_t st);
 

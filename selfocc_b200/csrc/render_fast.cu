@@ -120,12 +120,10 @@ __device__ __noinline__ void march_padded(const VolumeDev& V, const RayGeo& G, i
     float w;
     composite(a, alpha, mid, dgw * G.kw, dgh * G.kh, dgd * G.kd, s, w);
     if (RGB) {
-      float f[3];
+      float f[3], col[3], raw[3];
       gather_feat<3>(V, t, 0, f);
-      float r0 = f[0] * kC0, r1 = f[1] * kC0, r2 = f[2] * kC0;
-      if (sh_act == 0) { r0 = fmaxf(r0 + 0.5f, 0.f); r1 = fmaxf(r1 + 0.5f, 0.f); r2 = fmaxf(r2 + 0.5f, 0.f); }
-      else { r0 = sigmoidf_acc(r0); r1 = sigmoidf_acc(r1); r2 = sigmoidf_acc(r2); }
-      a.c_r = fmaf(w, r0, a.c_r); a.c_g = fmaf(w, r1, a.c_g); a.c_b = fmaf(w, r2, a.c_b);
+      colour_act(sh_act, f, col, raw);
+      a.c_r = fmaf(w, col[0], a.c_r); a.c_g = fmaf(w, col[1], a.c_g); a.c_b = fmaf(w, col[2], a.c_b);
     }
   }
 }
@@ -154,9 +152,7 @@ render_packed_kernel(VolumeDev V, const void* __restrict__ pack, RayDev R, Rende
   RayGeo G;
   G.tn = tn; G.span = tf - tn; G.step = 1.0f / (float)S;
   G.kh = V.ax[0].k0; G.kw = V.ax[1].k0; G.kd = V.ax[2].k0;
-  G.gh0 = fmaf(o[1] - V.ax[0].start, G.kh, V.ax[0].offset); G.gdh = d[1] * G.kh;
-  G.gw0 = fmaf(o[0] - V.ax[1].start, G.kw, V.ax[1].offset); G.gdw = d[0] * G.kw;
-  G.gd0 = fmaf(o[2] - V.ax[2].start, G.kd, V.ax[2].offset); G.gdd = d[2] * G.kd;
+  affine_grid_ray(V, o, d, G.gh0, G.gdh, G.gw0, G.gdw, G.gd0, G.gdd);
   G.dx = d[0]; G.dy = d[1]; G.dz = d[2];
   G.k_log2 = P.inv_s * 1.4426950408889634f;
   const float delta_c = G.span * G.step;
@@ -285,13 +281,9 @@ render_packed_kernel(VolumeDev V, const void* __restrict__ pack, RayDev R, Rende
   if (delta_c < eps_len) a.best_i = 0;                   // every candidate is 0: first index
   a.best_mid = fmaf(((float)a.best_i + 0.5f) * G.step, G.span, tn);   // (i + 1/2) / S is exact: the loop's mid_i bit for bit
 
-  const long long chunk = R.chunk_len > 0 ? gid / R.chunk_len : 0;
-  const float lo = __ldg(ws + 2 * chunk), hi = __ldg(ws + 2 * chunk + 1);
-  if (depth) {
-    float dd = a.dsum / (a.acc + 1e-10f);
-    dd = fminf(fmaxf(dd, lo), hi);
-    depth[lid] = dd / nrm;
-  }
+  float lo, hi;
+  depth_clip_range(ws, R, gid, lo, hi);
+  if (depth) depth[lid] = clipped_depth(a.dsum, a.acc, lo, hi, nrm);
   if (max_depth) max_depth[lid] = a.best_mid / nrm;
   if (max_idx) max_idx[lid] = a.best_i;
   if (acc_out) acc_out[lid] = a.acc;
@@ -300,23 +292,20 @@ render_packed_kernel(VolumeDev V, const void* __restrict__ pack, RayDev R, Rende
     normal_vis[3 * lid + 1] = (a.n1 + 1.0f) * 0.5f;
     normal_vis[3 * lid + 2] = (a.n2 + 1.0f) * 0.5f;
   }
-  if (RGB && rgb_out) {
-    float b0, b1, b2;
-    if (P.bkgd_mode == 2) { b0 = bkgd_rand[3 * lid]; b1 = bkgd_rand[3 * lid + 1]; b2 = bkgd_rand[3 * lid + 2]; }
-    else { b0 = b1 = b2 = (P.bkgd_mode == 1) ? 1.f : 0.f; }
-    const float rem = 1.0f - a.acc;
-    float r = fmaf(b0, rem, a.c_r), g = fmaf(b1, rem, a.c_g), b = fmaf(b2, rem, a.c_b);
-    if (P.eval_clamp) { r = fminf(fmaxf(r, 0.f), 1.f); g = fminf(fmaxf(g, 0.f), 1.f); b = fminf(fmaxf(b, 0.f), 1.f); }
-    rgb_out[3 * lid] = r; rgb_out[3 * lid + 1] = g; rgb_out[3 * lid + 2] = b;
-  }
+  if (RGB && rgb_out) store_rgb(P, bkgd_rand, lid, a.acc, a.c_r, a.c_g, a.c_b, rgb_out);
 }
 
-// ---- once-per-frame repack of the decoded volume -------------------------------------------------------
-__global__ void __launch_bounds__(256) pack_pair_kernel(const float* __restrict__ v, float2* __restrict__ out, long long n, int zp) {
+// ---- repack of the decoded volume: once per frame for inference (so_render_pack), per launch for the training forward
+__global__ void __launch_bounds__(256) zpair_pack_kernel(const float* __restrict__ v, float2* __restrict__ out, long long n, int zp) {
   long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x;
   if (i >= n) return;
   int z = (int)(i % zp);
   out[i] = make_float2(v[i], z + 1 < zp ? v[i + 1] : 0.f);       // the volume's z pad is already zero (so_tpv_decode)
+}
+
+void launch_zpair_pack(const float* vol_sdf, const so_volume_desc& d, float* pack, cudaStream_t st) {
+  const long long n = (long long)d.H * d.W * d.zpitch;
+  zpair_pack_kernel<<<(unsigned)ceil_div64(n, 256), 256, 0, st>>>(vol_sdf, reinterpret_cast<float2*>(pack), n, d.zpitch);
 }
 
 __global__ void __launch_bounds__(256) pack_rgbs_kernel(const float* __restrict__ sdf, const float* __restrict__ feat,
@@ -337,7 +326,7 @@ using namespace so;
 
 extern "C" int64_t so_render_pack_floats(const so_volume_desc* d) {
   if (!d || validate_volume(d)) return 0;
-  if (d->n_feat == 0) return 2 * (int64_t)d->H * d->W * d->zpitch;
+  if (d->n_feat == 0) return zpair_floats(*d);
   if (d->n_feat == 3) return 4 * (int64_t)d->H * d->W * d->Z;
   return 0;
 }
@@ -348,8 +337,7 @@ extern "C" int so_render_pack(const float* vol_sdf, const float* vol_feat, const
   if (rc) return rc;
   cudaStream_t st = (cudaStream_t)stream;
   if (d->n_feat == 0) {
-    long long n = (long long)d->H * d->W * d->zpitch;
-    pack_pair_kernel<<<(unsigned)ceil_div64(n, 256), 256, 0, st>>>(vol_sdf, reinterpret_cast<float2*>(pack), n, d->zpitch);
+    launch_zpair_pack(vol_sdf, *d, pack, st);
   } else if (d->n_feat == 3) {
     if (!vol_feat) return SO_ERR_INVALID_ARG;
     long long n = (long long)d->H * d->W * d->Z;
@@ -368,27 +356,22 @@ extern "C" int so_render_infer_packed(const float* vol_sdf, const float* vol_fea
                                       const so_render_params* pr, const float* bkgd_rand, float* depth, float* max_depth,
                                       int64_t* max_idx, float* acc, float* normal_vis, float* rgb, float* sem,
                                       float* workspace, float* dbg_grid, void* stream) {
-  if (!vol_sdf || !cam_mats || !rd || !pr || !workspace) return SO_ERR_INVALID_ARG;
-  int rc = validate_volume(vol_host);
+  int rc = check_render_operands(vol_sdf, workspace, cam_mats, rd, pr, vol_host);
   if (rc) return rc;
   VolumeDev V = make_volume(*vol_host, vol_sdf, vol_feat);
-  const bool fast = V.ax[0].k1 == 0.f && V.ax[1].k1 == 0.f && V.ax[2].k1 == 0.f && pr->num_samples >= 2 &&
-                    (pr->num_samples & (pr->num_samples - 1)) == 0 && pr->cos_anneal == 1.0f && pr->anchor_mid;
+  RenderDev P = make_render_dev(*pr, nullptr);
   const bool want_rgb = rgb != nullptr;
   const bool shape_ok = (vol_host->n_feat == 0 && !want_rgb) || (vol_host->n_feat == 3 && (!want_rgb || pr->sh_act == 0));
-  if (!pack || !fast || !shape_ok || sem) {
+  if (!pack || !uniform_affine_march(V, P) || P.S < 2 || !shape_ok || sem) {
     if (dbg_grid) return SO_ERR_UNSUPPORTED;         // the sample-coordinate probe exists on the packed kernels only
     return so_render_infer(vol_sdf, vol_feat, vol_host, cam_mats, pix, rd, pr, bkgd_rand, depth, max_depth, max_idx, acc,
                            normal_vis, rgb, sem, workspace, stream);
   }
-  if (rd->n_cam < 1 || rd->rays_per_cam < 1) return SO_ERR_INVALID_ARG;
-  if (pr->bkgd_mode == 2 && want_rgb && !bkgd_rand) return SO_ERR_INVALID_ARG;
-  if (pr->bkgd_mode < 0 || pr->bkgd_mode > 2 || pr->sh_act < 0 || pr->sh_act > 1) return SO_ERR_INVALID_ARG;
+  if ((rc = check_background(pr, want_rgb, bkgd_rand))) return rc;
   RayDev R;
   if ((rc = make_ray_dev(rd, cam_mats, pix, &R))) return rc;
   if (rd->ray_count == 0) return SO_OK;
   cudaStream_t st = (cudaStream_t)stream;
-  RenderDev P = make_render_dev(*pr, nullptr);
   if ((rc = launch_depth_bounds(R, P, workspace, st))) return rc;
 
   const unsigned grid = (unsigned)ceil_div64(rd->ray_count, SO_RF_BLOCK);

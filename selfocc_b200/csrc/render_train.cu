@@ -54,9 +54,7 @@ __device__ __forceinline__ void make_ctx(const VolumeDev& V, const RayDev& R, co
   slab(P, c.o, c.d, c.tn, c.tf);
   c.inv_nrm = 1.0f / c.nrm;
   c.affine = V.ax[0].k1 == 0.f && V.ax[1].k1 == 0.f && V.ax[2].k1 == 0.f;
-  c.gh0 = fmaf(c.o[1] - V.ax[0].start, V.ax[0].k0, V.ax[0].offset); c.gdh = c.d[1] * V.ax[0].k0;
-  c.gw0 = fmaf(c.o[0] - V.ax[1].start, V.ax[1].k0, V.ax[1].offset); c.gdw = c.d[0] * V.ax[1].k0;
-  c.gd0 = fmaf(c.o[2] - V.ax[2].start, V.ax[2].k0, V.ax[2].offset); c.gdd = c.d[2] * V.ax[2].k0;
+  affine_grid_ray(V, c.o, c.d, c.gh0, c.gdh, c.gw0, c.gdw, c.gd0, c.gdd);
   c.u = P.jitter ? P.jitter + gid * (long long)(P.S + 1) : nullptr;
 }
 
@@ -152,6 +150,15 @@ __device__ __forceinline__ float warp_sum(float v) {
   for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
   return v;
 }
+// transmittance of this lane's sample from the factors f = 1 - alpha + 1e-7 of one 32-sample chunk: the exclusive product
+// along the lanes times `carry`, the product over the earlier chunks, which then takes on this chunk's product
+__device__ __forceinline__ float warp_transmittance(float f, int lane, float& carry) {
+  float incl = warp_incl_prod(f, lane);
+  float excl = __shfl_up_sync(0xffffffffu, incl, 1);
+  float T = carry * (lane == 0 ? 1.0f : excl);
+  carry *= __shfl_sync(0xffffffffu, incl, 31);
+  return T;
+}
 // reverse inclusive sum: out[lane] = sum_{i >= lane} v[i]
 __device__ __forceinline__ float warp_rev_incl_sum(float v, int lane) {
 #pragma unroll
@@ -212,6 +219,8 @@ __device__ __forceinline__ void scatter_feat24(const VolumeDev& V, float* __rest
   }
 }
 
+// the training kernels' form of colour_act(sh_act, ...) (render_common.cuh): the same values; the two forms are kept because
+// each compiles to the machine code its kernels were tuned with
 __device__ __forceinline__ void colour_act(const RenderDev& P, const float f[3], float col[3], float raw[3]) {
 #pragma unroll
   for (int c = 0; c < 3; ++c) {
@@ -285,10 +294,7 @@ __global__ void __launch_bounds__(128, SEM == 24 ? SO_TRAIN_FWD24_MIN_CTAS : SO_
       }
       float alpha = live ? q.alpha : 0.f;
       float f = live ? (1.0f - alpha + 1e-7f) : 1.0f;
-      float incl = warp_incl_prod(f, lane);
-      float excl = __shfl_up_sync(0xffffffffu, incl, 1);
-      float T = carry * (lane == 0 ? 1.0f : excl);
-      carry *= __shfl_sync(0xffffffffu, incl, 31);
+      float T = warp_transmittance(f, lane, carry);
       float w = alpha * T;
       if (live) {
         long long oidx = ray * S + s;
@@ -418,13 +424,6 @@ __device__ __forceinline__ void prefetch_global(const void* p) {
 #else
   asm volatile("prefetch.global.L2 [%0];" ::"l"(__cvta_generic_to_global(p)));
 #endif
-}
-
-__global__ void __launch_bounds__(256) zpair_pack_kernel(const float* __restrict__ v, float2* __restrict__ out, long long n, int zp) {
-  long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x;
-  if (i >= n) return;
-  int z = (int)(i % zp);
-  out[i] = make_float2(v[i], z + 1 < zp ? v[i + 1] : 0.f);
 }
 
 // ZP / WZP: compile-time zpitch and W * zpitch (0 = take them from the descriptor)
@@ -585,6 +584,7 @@ render_train_fwd5_kernel(VolumeDev V, RayDev R, RenderDev P, const float* __rest
         for (int j = 0; j < U; ++j) {
           const int s = ((k + j) << 5) + lane;
           float f = 1.0f - alpha[j] + 1e-7f;
+          // warp_transmittance written out: calling it changes this kernel's machine code
           float incl = warp_incl_prod(f, lane);
           float excl = __shfl_up_sync(kFull, incl, 1);
           float T = carry * (lane == 0 ? 1.0f : excl);
@@ -708,10 +708,7 @@ __global__ void __launch_bounds__(128, SEM == 24 ? SO_TRAIN_BWD24_MIN_CTAS : 1) 
       eval_sample<FAST>(V, P, c, live ? s : S - 1, lane, q);
       float alpha = live ? q.alpha : 0.f;
       float f = live ? (1.0f - alpha + 1e-7f) : 1.0f;
-      float incl = warp_incl_prod(f, lane);
-      float excl = __shfl_up_sync(0xffffffffu, incl, 1);
-      float T = carry * (lane == 0 ? 1.0f : excl);
-      carry *= __shfl_sync(0xffffffffu, incl, 31);
+      float T = warp_transmittance(f, lane, carry);
       Tk[k] = T; Ak[k] = alpha;
       acc += alpha * T;
       dsum = fmaf(alpha * T, q.mid, dsum);
@@ -876,25 +873,27 @@ __global__ void __launch_bounds__(128) render_train_probe_kernel(VolumeDev V, Ra
 }
 
 // the lean per-sample path of the forwards applies (see fast_edge)
-static bool train_fast(const VolumeDev& V, const RenderDev& P) {
-  return V.ax[0].k1 == 0.f && V.ax[1].k1 == 0.f && V.ax[2].k1 == 0.f && (P.S & (P.S - 1)) == 0 && P.S >= 32 &&
-         P.cos_anneal == 1.0f && P.anchor_mid;
+static bool train_fast(const VolumeDev& V, const RenderDev& P) { return uniform_affine_march(V, P) && P.S >= 32; }
+
+static int train_num_samples_check(const so_render_params* pr) {
+  if (pr->num_samples < 1) return SO_ERR_INVALID_ARG;
+  if (pr->num_samples > 32 * kTrainMaxChunks) return SO_ERR_UNSUPPORTED;
+  return SO_OK;
 }
 
 static int train_common_checks(const float* vol_sdf, const float* vol_feat, const so_volume_desc* d, const float* cam_mats,
                                const so_ray_desc* rd, const so_render_params* pr, const float* workspace, bool want_rgb,
                                bool want_sem, const float* bkgd_rand) {
-  if (!vol_sdf || !cam_mats || !rd || !pr || !workspace) return SO_ERR_INVALID_ARG;
-  int rc = validate_volume(d);
-  if (rc) return rc;
-  if (pr->num_samples < 1) return SO_ERR_INVALID_ARG;
-  if (pr->num_samples > 32 * kTrainMaxChunks) return SO_ERR_UNSUPPORTED;
-  if (want_rgb && (d->n_feat < 3 || !vol_feat)) return SO_ERR_INVALID_ARG;
-  if (want_sem && (d->n_feat <= 3 || !vol_feat)) return SO_ERR_INVALID_ARG;
-  if (want_sem && d->n_feat - 3 > kMaxSem) return SO_ERR_UNSUPPORTED;
-  if (pr->bkgd_mode == 2 && want_rgb && !bkgd_rand) return SO_ERR_INVALID_ARG;
-  if (pr->bkgd_mode < 0 || pr->bkgd_mode > 2 || pr->sh_act < 0 || pr->sh_act > 1) return SO_ERR_INVALID_ARG;
-  return SO_OK;
+  int rc = check_render_operands(vol_sdf, workspace, cam_mats, rd, pr, d);
+  if (rc || (rc = train_num_samples_check(pr))) return rc;
+  return check_shading(d, vol_feat, pr, want_rgb, want_sem, bkgd_rand);
+}
+
+// persistent-style grid of the one-ray-per-warp kernels: warps stride over rays; 4 warps per CTA, enough CTAs to fill
+// every SM several times over
+static unsigned train_grid(long long ray_count) {
+  const long long ctas = ceil_div64(ray_count, 4), cap = (long long)num_sms() * 16;
+  return (unsigned)(ctas < cap ? ctas : cap);
 }
 
 }  // namespace so
@@ -910,7 +909,7 @@ extern "C" int so_render_train_force_fwd32(int on) { g_force_fwd32 = on != 0; re
 
 extern "C" int64_t so_render_train_pair_floats(const so_volume_desc* vol_host) {
   if (!vol_host || validate_volume(vol_host)) return 0;
-  return 2 * (int64_t)vol_host->H * vol_host->W * vol_host->zpitch;
+  return zpair_floats(*vol_host);
 }
 
 extern "C" int so_render_train_forward(const float* vol_sdf, const float* vol_feat, const so_volume_desc* vol_host,
@@ -931,10 +930,7 @@ extern "C" int so_render_train_forward(const float* vol_sdf, const float* vol_fe
   RenderDev P = make_render_dev(*pr, jitter);
   if ((rc = launch_depth_bounds(R, P, workspace, st))) return rc;
   TrainOut O{depth, acc, fars, rgb, sem, max_depth, weights, ts, deltas, eik_grad, sample_sdf};
-  // persistent-style grid: warps stride over rays; 4 warps per CTA, enough CTAs to fill 132 SMs several times over
-  long long ctas = ceil_div64(R.ray_count, 4);
-  const long long cap = (long long)num_sms() * 16;
-  unsigned grid = (unsigned)(ctas < cap ? ctas : cap);
+  const unsigned grid = train_grid(R.ray_count);
   ProfScope prof(6, st);
   const bool fast = train_fast(V, P);
   // batched-ray kernel (U chunks in flight, optional z-pair volume); the one-ray-per-warp kernel covers semantics,
@@ -945,8 +941,7 @@ extern "C" int so_render_train_forward(const float* vol_sdf, const float* vol_fe
   if (v5) {
     const float2* vp = nullptr;
     if (pair_workspace) {
-      const long long nv = (long long)V.H * V.W * V.zpitch;
-      zpair_pack_kernel<<<(unsigned)ceil_div64(nv, 256), 256, 0, st>>>(vol_sdf, reinterpret_cast<float2*>(pair_workspace), nv, V.zpitch);
+      launch_zpair_pack(vol_sdf, *vol_host, pair_workspace, st);
       note_launch(1);
       vp = reinterpret_cast<const float2*>(pair_workspace);
     }
@@ -988,9 +983,7 @@ extern "C" int so_render_train_backward(const float* vol_sdf, const float* vol_f
   RenderDev P = make_render_dev(*pr, jitter);
   if ((rc = launch_depth_bounds(R, P, workspace, st))) return rc;
   TrainGrad G{g_depth, g_acc, g_rgb, g_sem, g_weights, g_eik, g_sdf, g_vol_sdf, g_vol_feat, g_inv_s};
-  long long ctas = ceil_div64(R.ray_count, 4);
-  const long long cap = (long long)num_sms() * 16;
-  unsigned grid = (unsigned)(ctas < cap ? ctas : cap);
+  const unsigned grid = train_grid(R.ray_count);
   ProfScope prof(7, st);
   const bool sem24 = V.n_feat == 24 && V.feat_pitch == 24 && (want_rgb || want_sem) && !g_force_sem_generic &&
                      ((reinterpret_cast<uintptr_t>(vol_feat) | reinterpret_cast<uintptr_t>(g_vol_feat)) & 15) == 0;
@@ -1009,19 +1002,14 @@ extern "C" int so_render_train_backward(const float* vol_sdf, const float* vol_f
 
 extern "C" int so_render_train_probe(const so_volume_desc* vol_host, const float* cam_mats, const float* pix, const so_ray_desc* rd,
                                      const so_render_params* pr, const float* jitter, float* grid, void* stream) {
-  if (!vol_host || !cam_mats || !rd || !pr || !grid) return SO_ERR_INVALID_ARG;
-  int rc = validate_volume(vol_host);
-  if (rc) return rc;
-  if (pr->num_samples < 1) return SO_ERR_INVALID_ARG;
-  if (pr->num_samples > 32 * kTrainMaxChunks) return SO_ERR_UNSUPPORTED;
+  int rc = check_render_operands(vol_host, grid, cam_mats, rd, pr, vol_host);
+  if (rc || (rc = train_num_samples_check(pr))) return rc;
   RayDev R;
   if ((rc = make_ray_dev(rd, cam_mats, pix, &R))) return rc;
   if (R.ray_count == 0) return SO_OK;
   VolumeDev V = make_volume(*vol_host, nullptr, nullptr);
   RenderDev P = make_render_dev(*pr, jitter);
-  long long ctas = ceil_div64(R.ray_count, 4);
-  const long long cap = (long long)num_sms() * 16;
-  unsigned g = (unsigned)(ctas < cap ? ctas : cap);
+  const unsigned g = train_grid(R.ray_count);
   cudaStream_t st = (cudaStream_t)stream;
   if (train_fast(V, P)) render_train_probe_kernel<true><<<g, 128, 0, st>>>(V, R, P, grid);
   else render_train_probe_kernel<false><<<g, 128, 0, st>>>(V, R, P, grid);

@@ -91,6 +91,13 @@ def make_render_params(aabb, num_samples, inv_s, near_plane=0.0, training=False,
     return p
 
 
+def _render_ws(lib, rays, dev):
+    """Depth-clip workspace of a render launch: [min first-mid, max last-mid] per reference chunk of the whole batch."""
+    total = rays.n_cam * rays.rays_per_cam
+    n_chunks = (total + rays.chunk_len - 1) // rays.chunk_len if rays.chunk_len > 0 else 1
+    return torch.empty(lib.so_render_workspace_floats(n_chunks), device=dev, dtype=torch.float32)
+
+
 def render_pack(vol_sdf, vol_feat, desc):
     """Once-per-frame repack of the decoded volume for the packed render kernels (so_render_pack): float2 z-pairs when no
     colour is decoded, float4 (C0 r + 0.5, C0 g + 0.5, C0 b + 0.5, sdf) for color_dims == 3 (the SH-0 colour before its relu).  Returns None when this channel count has no packed form."""
@@ -117,9 +124,7 @@ def render_infer(vol_sdf, vol_feat, desc, cam_mats, rays, params, pix=None, bkgd
     assert cam_mats.shape == (rays.n_cam, 4, 4)
     n = rays.ray_count
     dev = vol_sdf.device
-    total = rays.n_cam * rays.rays_per_cam
-    n_chunks = (total + rays.chunk_len - 1) // rays.chunk_len if rays.chunk_len > 0 else 1
-    ws = torch.empty(lib.so_render_workspace_floats(n_chunks), device=dev, dtype=torch.float32)
+    ws = _render_ws(lib, rays, dev)
     shapes = dict(depth=((n,), torch.float32), max_depth=((n,), torch.float32), max_idx=((n,), torch.int64),
                   acc=((n,), torch.float32), normal_vis=((n, 3), torch.float32), rgb=((n, 3), torch.float32),
                   sem=((n, max(desc.n_feat - 3, 0)), torch.float32))
@@ -130,11 +135,7 @@ def render_infer(vol_sdf, vol_feat, desc, cam_mats, rays, params, pix=None, bkgd
         else:
             res[k] = torch.empty(shapes[k][0], device=dev, dtype=shapes[k][1])
     g = lambda k: _p(res.get(k))
-    if pack is None and not probe_grid:
-        _lib.check(lib.so_render_infer(_p(vol_sdf), _p(vol_feat), C.byref(desc), _p(cam_mats), _p(pix), C.byref(rays),
-                                       C.byref(params), _p(bkgd_rand), g('depth'), g('max_depth'), g('max_idx'), g('acc'),
-                                       g('normal_vis'), g('rgb'), g('sem'), _p(ws), _stream()), 'so_render_infer')
-        return res
+    # without a pack the library renders with the general kernels (so_render_infer); it refuses a probe without one
     if probe_grid:
         res['grid'] = torch.empty(n, params.num_samples, 3, device=dev, dtype=torch.float32)
     _lib.check(lib.so_render_infer_packed(_p(vol_sdf), _p(vol_feat), C.byref(desc), _p(pack), _p(cam_mats), _p(pix), C.byref(rays),
@@ -337,12 +338,6 @@ class TPVSelfAttnFunction(torch.autograd.Function):
 
 
 # --------------------------------------------------------------------------------------- training form (B6-B10, B13)
-def _render_ws(lib, rays, dev):
-    total = rays.n_cam * rays.rays_per_cam
-    n_chunks = (total + rays.chunk_len - 1) // rays.chunk_len if rays.chunk_len > 0 else 1
-    return torch.empty(lib.so_render_workspace_floats(n_chunks), device=dev, dtype=torch.float32)
-
-
 class RenderTrainFunction(torch.autograd.Function):
     """Differentiable (w.r.t. the decoded volume and inv_s) training-form render.
     forward(vol_sdf, vol_feat_or_None, inv_s[1], cfg) -> (depth, acc, fars, max_depth, rgb, sem, weights, ts, deltas,
