@@ -135,12 +135,12 @@ class ShardedLifter:
     """Inference-only, bs = 1, post-norm layers ('self_attn','norm','cross_attn','norm','ffn','norm' -- every shipped config)."""
 
     def __init__(self, encoder):
-        from . import encoder as E
-        self.E, self.enc = E, encoder
+        from .encoder import POST_NORM_ORDER
+        self.enc = encoder
         H, W, Z = encoder.tpv_size
         self.sizes = [H * W, Z * H, W * Z]
         for layer in encoder.layers:
-            if tuple(layer.operation_order) != ('self_attn', 'norm', 'cross_attn', 'norm', 'ffn', 'norm'):
+            if tuple(layer.operation_order) != POST_NORM_ORDER:
                 raise NotImplementedError('ShardedLifter: operation_order %r' % (layer.operation_order,))
 
     # ---- slices
@@ -163,57 +163,23 @@ class ShardedLifter:
     @torch.no_grad()
     def prepare(self, ms_img_feats, metas):
         enc = self.enc
-        feat, shapes, lsi = enc.flatten_features(ms_img_feats)
-        dev = feat.device
-        uvs, masks, vises = enc.project_reference_points(metas, dev)
-        pv = enc._tpv_pos()
-        pos = enc._pos_cat[0] if getattr(enc, '_pos_val', None) is pv else torch.cat(list(pv), 0)      # [Q_total, C]
-        return dict(feat=feat, shapes=shapes, lsi=lsi, uvs=uvs, vises=vises, pos=pos,
+        tpv_pos, feat, shapes, lsi = enc.frame_inputs(ms_img_feats)     # bs = 1, no autograd: the [1, Q_total, C] tensor
+        uvs, masks, vises = enc.project_reference_points(metas, feat.device)
+        return dict(feat=feat, shapes=shapes, lsi=lsi, uvs=uvs, vises=vises, pos=tpv_pos[0],
                     ref=enc.cross_view_ref_points)                            # [Q_total, 3, P, 2]
 
     # ---- one layer on this rank's queries
     @torch.no_grad()
     def layer_local(self, li, qfull, st, rank, world):
         """qfull [Q_total, C] (all planes, input of layer li) -> this rank's updated rows [sum(count_i), C]."""
-        E, ops_ = self.E, ops
-        layer = self.enc.layers[li]
-        sa, ca = layer.attentions[0], layer.attentions[1]
-        sl = self.slices(rank, world)
+        enc = self.enc
         q = self._local_rows(qfull, rank, world).contiguous()
         if q.shape[0] == 0:
             return q
-        Hd, L, P = sa.num_heads, sa.num_levels, sa.num_points
-        # -- self attention (cross_view_hybrid_attention.py:63-124): value = ALL tokens, queries = local rows (+ pos)
-        v = E.fast_linear(sa.value_proj, qfull)
-        qp = q + self._local_rows(st['pos'], rank, world)
-        _, (offs, logits) = E.fast_linear_cat(sa, '_so_offlog', [sa.sampling_offsets, sa.attention_weights], qp)
-        ref = self._local_rows(st['ref'], rank, world).contiguous()
-        out = ops_.tpv_self_attn_forward_rows(v, Hd, v.shape[1] // Hd, self.enc.tpv_spatial_shapes, self.enc.tpv_level_start,
-                                              offs, logits, ref, L, P)
-        q = E.fast_linear(sa.output_proj, out, residual=q, ln=layer.norms[0])
-        # -- image cross attention, one plane at a time (tpvformer/attention/image_cross_attention.py:83-93)
-        feat = st['feat']
-        n_cam, nv = feat.shape[0], feat.shape[1]
-        vps = [a.deformable_attention.value_proj for a in ca.attns]
-        _, vrows = E.fast_linear_cat(ca, '_so_value3', vps, feat[:, :, 0].reshape(-1, feat.shape[-1]))
-        outs, o0 = [], 0
-        for i, (b, c) in enumerate(sl):
-            if c == 0:
-                continue
-            att = ca.attns[i]
-            da = att.deformable_attention
-            qi = q[o0:o0 + c]
-            _, (offs, logits) = E.fast_linear_cat(da, '_so_offlog', [da.sampling_offsets, da.attention_weights], qi)
-            uv = st['uvs'][i][:, 0, b:b + c].contiguous()
-            vis = st['vises'][i][:, b:b + c].contiguous()
-            slots = ops_.tpv_cross_attn_forward_rows(vrows[i], n_cam, da.num_heads, qi.shape[1] // da.num_heads, st['shapes'], st['lsi'],
-                                                     offs, logits, uv, vis, da.num_levels, da.num_points)
-            outs.append(E.fast_linear(att.output_proj, slots, residual=qi, ln=layer.norms[1]))
-            o0 += c
-        q = torch.cat(outs, 0)
-        ffn = layer.ffns[0]
-        h = E.fast_linear(ffn.layers[0][0], q, relu=True)
-        return E.fast_linear(ffn.layers[1], h, residual=q if ffn.add_identity else None, ln=layer.norms[2])
+        return enc.layers[li].forward_rows(q, qfull, self._local_rows(st['pos'], rank, world),
+                                           self._local_rows(st['ref'], rank, world), self.slices(rank, world), st['feat'],
+                                           st['shapes'], st['lsi'], (enc.tpv_spatial_shapes, enc.tpv_level_start),
+                                           st['uvs'], st['vises'])
 
     # ---- exchange
     def pad_local(self, local, rank, world):

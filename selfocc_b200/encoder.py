@@ -4,12 +4,13 @@ Class names, constructor kwargs, forward signatures, output dict keys and ``stat
 follow the reference (file:line in each docstring) so that configs and checkpoints carry over.
 The arithmetic of the hot ops runs in ``libselfocc_b200.so``:
 
-* inference (no autograd): one fused kernel per attention -- softmax + sampling-location arithmetic +
-  bilinear gather + head sum (+ camera loop / visible-count average for the image cross-attention),
-  no ``nonzero()`` host sync, no padded per-camera rebatch (``ops.tpv_self_attn_forward*`` /
-  ``ops.tpv_cross_attn_forward*``); every dense projection (value / offset / weight / output Linear, FFN) runs on
+* inference (eval, no autograd, batch 1, post-norm layers -- every shipped config): ``TPVFormerLayer.forward_rows``,
+  one routine per layer shared with the query-sharded lifter (``dist.ShardedLifter``).  One fused kernel per attention --
+  softmax + sampling-location arithmetic + bilinear gather + head sum (+ camera loop / visible-count average for the
+  image cross-attention), no ``nonzero()`` host sync, no padded per-camera rebatch (``ops.tpv_self_attn_forward_rows`` /
+  ``ops.tpv_cross_attn_forward_rows``); every dense projection (value / offset / weight / output Linear, FFN) runs on
   the wgmma split-precision GEMM (``ops.linear_3xtf32``, fp32-level accuracy), projections of the same input are
-  fused into one GEMM; LayerNorm is a warp-per-row kernel (``ops.layer_norm``);
+  fused into one GEMM, and each LayerNorm is folded into the epilogue of the GEMM before it;
 * training (autograd), batch 1: the same fused attention cores with their backward kernels
   (``ops.TPVSelfAttnFunction`` / ``ops.TPVCrossAttnFunction``: no host sync, no padded rebatch, no
   sampling-location tensor); the projections run forward and input gradient on the wgmma GEMM
@@ -148,7 +149,7 @@ def fast_linear(lin, x, relu=False, residual=None, out=None, ln=None):
     (``so_linear_3xtf32_ln``), a separate ``so_layer_norm`` launch otherwise."""
     if ln is not None:
         N, K = lin.weight.shape
-        if x.is_cuda and x.dtype == torch.float32 and ops.linear_ln_supported(N, K) and not _ln_fusion_off():
+        if x.is_cuda and x.dtype == torch.float32 and ops.linear_ln_supported(N, K):
             return _fast_linear_impl(lin, x, relu, residual, out, (ln.weight.detach(), ln.bias.detach(), ln.eps))
         y = _fast_linear_impl(lin, x, relu, residual, None, None)
         if y.is_cuda and y.dtype == torch.float32 and y.shape[-1] <= 256:
@@ -160,11 +161,6 @@ def fast_linear(lin, x, relu=False, residual=None, out=None, ln=None):
             return out
         return y
     return _fast_linear_impl(lin, x, relu, residual, out, None)
-
-
-def _ln_fusion_off():
-    import os
-    return os.environ.get('SELFOCC_B200_NO_LN_FUSION', '0') == '1'          # A/B switch for measurements
 
 
 def _fast_linear_impl(lin, x, relu, residual, out, ln):
@@ -228,6 +224,15 @@ def _fusable(lins, x):
     return x.is_cuda and x.dtype == torch.float32 and all(ops.linear_supported(l.weight.shape[1], l.weight.shape[0]) for l in lins)
 
 
+def _offsets_logits(da, x):
+    """sampling_offsets(x), attention_weights(x) of a deformable attention as [n, *] row views: one GEMM when both shapes
+    allow it, two otherwise."""
+    lins = [da.sampling_offsets, da.attention_weights]
+    if _fusable(lins, x):
+        return fast_linear_cat(da, '_so_offlog', lins, x)[1]
+    return fast_linear(lins[0], x), fast_linear(lins[1], x)
+
+
 def _needs_grad(*tensors):
     return torch.is_grad_enabled() and any(t is not None and t.requires_grad for t in tensors)
 
@@ -256,10 +261,7 @@ class CrossViewHybridAttention(_DeformBase):
         nn.init.constant_(self.output_proj.bias, 0.)
 
     def forward(self, query, key=None, value=None, identity=None, query_pos=None, key_padding_mask=None,
-                reference_points=None, spatial_shapes=None, level_start_index=None, fuse_norm=None, **kwargs):
-        """fuse_norm: the nn.LayerNorm that follows this op in the layer (inference path only): applied inside the
-        output_proj GEMM's epilogue; the caller then skips its norm step (``self.fused_norm_applied``)."""
-        self.fused_norm_applied = False
+                reference_points=None, spatial_shapes=None, level_start_index=None, **kwargs):
         if value is None:
             value = query
         if identity is None:
@@ -273,28 +275,8 @@ class CrossViewHybridAttention(_DeformBase):
         Hd, L, P = self.num_heads, self.num_levels, self.num_points
         if reference_points.shape[-1] != 2:
             raise ValueError('Last dim of reference_points must be 2, but get %d instead.' % reference_points.shape[-1])
-        fused = bs == 1 and key_padding_mask is None and not _needs_grad(value, query, self.value_proj.weight)
-        if fused:   # inference: tensor-core projections + one fused sampling kernel, dropout is the identity
-            v = fast_linear(self.value_proj, value[0])
-            ref = reference_points[0] if reference_points.dim() == 5 else reference_points
-            if _fusable([self.sampling_offsets, self.attention_weights], query):
-                _, (offsets, logits) = fast_linear_cat(self, '_so_offlog', [self.sampling_offsets, self.attention_weights], query[0])
-                out = ops.tpv_self_attn_forward_rows(v, Hd, v.shape[1] // Hd, spatial_shapes, level_start_index, offsets, logits,
-                                                     ref.contiguous(), L, P)
-            else:
-                offsets = fast_linear(self.sampling_offsets, query[0]).view(num_query, Hd, L, P, 2)
-                logits = fast_linear(self.attention_weights, query[0]).view(num_query, Hd, L, P)
-                out = ops.tpv_self_attn_forward(v.view(num_value, Hd, -1), spatial_shapes, level_start_index, offsets, logits,
-                                                ref.contiguous())
-            idt = identity[0] if self.batch_first else identity[:, 0]
-            if self.training:
-                out = self.dropout(fast_linear(self.output_proj, out)) + idt
-            else:
-                out = fast_linear(self.output_proj, out, residual=idt, ln=fuse_norm)
-                self.fused_norm_applied = fuse_norm is not None
-            return out[None] if self.batch_first else out[:, None]
         if bs == 1 and key_padding_mask is None and _cuda_fp32(query, value):
-            # training: the same fused core with its backward kernel; projections on the autograd GEMM
+            # the fused core with its backward kernel; projections on the autograd GEMM
             v = train_linear(self.value_proj, value[0]).view(num_value, Hd, -1)
             offsets = train_linear(self.sampling_offsets, query[0]).view(num_query, Hd, L, P, 2)
             logits = train_linear(self.attention_weights, query[0]).view(num_query, Hd, L, P)
@@ -382,12 +364,9 @@ class BEVCrossAttention(nn.Module):
         nn.init.constant_(self.output_proj.bias, 0.)
 
     def forward(self, query, key, value, residual=None, spatial_shapes=None, reference_points_cams=None,
-                bev_masks=None, level_start_index=None, bev_vis=None, value_rows=None, out_rows=None, fuse_norm=None, **kwargs):
+                bev_masks=None, level_start_index=None, bev_vis=None, **kwargs):
         """query [B,Q,C]; key/value [N, sum(hw), B, C]; reference_points_cams [N,B,Q,D,2];
-        bev_masks [N,B,Q,D] (bool/uint8); bev_vis optional uint8 [N,Q] = any_D(mask) from so_point_sampling;
-        value_rows optional [N*sum(hw), >= C] view holding value_proj(value) already (TPVCrossAttention projects the image
-        features for its three planes in one GEMM); out_rows optional contiguous [Q, C] destination (a row range of the
-        layer's concatenated token buffer, so the three planes need no torch.cat afterwards)."""
+        bev_masks [N,B,Q,D] (bool/uint8); bev_vis optional uint8 [N,Q] = any_D(mask) from so_point_sampling."""
         if key is None:
             key = query
         if value is None:
@@ -398,29 +377,8 @@ class BEVCrossAttention(nn.Module):
         da = self.deformable_attention
         Hd, L, D = da.num_heads, da.num_levels, da.num_points
         assert reference_points_cams.size(3) == D
-        if bs == 1 and not _needs_grad(query, value, da.value_proj.weight):
-            n_cam, nv = value.shape[0], value.shape[1]
-            if bev_vis is None:
-                bev_vis = (bev_masks[:, 0].sum(-1) > 0).to(torch.uint8)
-            uv = reference_points_cams[:, 0].contiguous()
-            v_rows = value_rows if value_rows is not None else fast_linear(da.value_proj, value[:, :, 0]).view(n_cam * nv, -1)
-            if _fusable([da.sampling_offsets, da.attention_weights], query):
-                _, (offsets, logits) = fast_linear_cat(da, '_so_offlog', [da.sampling_offsets, da.attention_weights], query[0])
-                slots = ops.tpv_cross_attn_forward_rows(v_rows, n_cam, Hd, C // Hd, spatial_shapes, level_start_index, offsets, logits,
-                                                        uv, bev_vis.contiguous(), L, D)
-            else:
-                offsets = fast_linear(da.sampling_offsets, query[0]).view(num_query, Hd, L, D, 2)
-                logits = fast_linear(da.attention_weights, query[0]).view(num_query, Hd, L, D)
-                slots = ops.tpv_cross_attn_forward(v_rows.contiguous().view(n_cam, nv, Hd, -1), spatial_shapes, level_start_index,
-                                                   offsets, logits, uv, bev_vis.contiguous())
-            self.fused_norm_applied = False
-            if self.training:
-                return self.dropout(fast_linear(self.output_proj, slots))[None] + residual
-            self.fused_norm_applied = fuse_norm is not None
-            return fast_linear(self.output_proj, slots, residual=residual[0], out=out_rows, ln=fuse_norm)[None]
-        self.fused_norm_applied = False
         if bs == 1 and kwargs.get('key_padding_mask') is None and _cuda_fp32(query, value):
-            # training: the rebatch-free core with its backward kernel (no host sync, no padded per-camera copies)
+            # the rebatch-free core with its backward kernel (no host sync, no padded per-camera copies)
             n_cam, nv = value.shape[0], value.shape[1]
             if bev_vis is None:
                 bev_vis = (bev_masks[:, 0].sum(-1) > 0).to(torch.uint8)
@@ -479,27 +437,12 @@ class TPVCrossAttention(nn.Module):
         self.attns = [self.attn_hw, self.attn_zh, self.attn_wz]
 
     def forward(self, query, key, value, residual=None, spatial_shapes=None, reference_points_cams=None, tpv_masks=None,
-                level_start_index=None, tpv_vis=None, out_cat=None, fuse_norm=None, **kwargs):
-        rows = [None, None, None]
-        vps = [a.deformable_attention.value_proj for a in self.attns]
-        if value.shape[2] == 1 and _fusable(vps, value) and not _needs_grad(value, query[0], vps[0].weight):
-            # the three planes project the SAME image features with their own value_proj: one GEMM, three column slices
-            _, rows = fast_linear_cat(self, '_so_value3', vps, value[:, :, 0].reshape(-1, value.shape[-1]))
-        outs = [None, None, None]
-        if out_cat is not None:                       # [1, Q_hw + Q_zh + Q_wz, C] token buffer of the layer
-            o0 = 0
-            for i in range(3):
-                n = query[i].shape[1]
-                outs[i] = out_cat[0, o0:o0 + n]
-                o0 += n
-        res = [self.attns[i](query[i], key, value, residual[i] if residual is not None else None,
-                             spatial_shapes=spatial_shapes, level_start_index=level_start_index,
-                             reference_points_cams=reference_points_cams[i], bev_masks=tpv_masks[i],
-                             bev_vis=None if tpv_vis is None else tpv_vis[i], value_rows=rows[i], out_rows=outs[i],
-                             fuse_norm=fuse_norm)
-               for i in range(3)]
-        self.fused_norm_applied = fuse_norm is not None and all(getattr(a, 'fused_norm_applied', False) for a in self.attns)
-        return res
+                level_start_index=None, tpv_vis=None, **kwargs):
+        return [self.attns[i](query[i], key, value, residual[i] if residual is not None else None,
+                              spatial_shapes=spatial_shapes, level_start_index=level_start_index,
+                              reference_points_cams=reference_points_cams[i], bev_masks=tpv_masks[i],
+                              bev_vis=None if tpv_vis is None else tpv_vis[i])
+                for i in range(3)]
 
 
 class FFN(nn.Module):
@@ -516,13 +459,7 @@ class FFN(nn.Module):
             nn.Sequential(nn.Linear(embed_dims, feedforward_channels), nn.ReLU(inplace=True), nn.Dropout(ffn_drop)),
             nn.Linear(feedforward_channels, embed_dims), nn.Dropout(ffn_drop))
 
-    def forward(self, x, identity=None, fuse_norm=None):
-        self.fused_norm_applied = False
-        if not self.training and not _needs_grad(x, self.layers[0][0].weight):
-            h = fast_linear(self.layers[0][0], x, relu=True)
-            idt = (x if identity is None else identity) if self.add_identity else None
-            self.fused_norm_applied = fuse_norm is not None
-            return fast_linear(self.layers[1], h, residual=idt, ln=fuse_norm)
+    def forward(self, x, identity=None):
         l0 = self.layers[0]
         out = self.layers[2](train_linear(self.layers[1], l0[2](F.relu(train_linear(l0[0], x)))))
         if not self.add_identity:
@@ -532,6 +469,9 @@ class FFN(nn.Module):
 
 if not HAVE_MMENGINE:  # mmcv registers its own FFN when present
     MODELS.register_module(name='FFN', module=FFN)
+
+
+POST_NORM_ORDER = ('self_attn', 'norm', 'cross_attn', 'norm', 'ffn', 'norm')     # every shipped config's layer
 
 
 def _whole(views, split):
@@ -594,8 +534,6 @@ class TPVFormerLayer(nn.Module):
 
     def forward(self, query, key=None, value=None, tpv_pos=None, ref_2d=None, spatial_shapes=None, level_start_index=None,
                 reference_points_cams=None, tpv_masks=None, tpv_size=None, tpv_vis=None, tpv_levels=None, **kwargs):
-        norm_i = attn_i = ffn_i = 0
-        identity = query
         H, W, Z = tpv_size
         split = [H * W, Z * H, W * Z]
         dev = query[0].device
@@ -606,30 +544,26 @@ class TPVFormerLayer(nn.Module):
         # `qc` is the concatenated [B, Q_hw + Q_zh + Q_wz, C] token buffer; `query` are its per-plane views.  Keeping both
         # avoids the reference's torch.cat before every self-attention / norm / ffn step (5 x 31 MB copies per layer).
         qc = _whole(query, split)
+        if self._takes_rows(query[0], kwargs):
+            if tpv_vis is None:
+                tpv_vis = [(m[:, 0].sum(-1) > 0).to(torch.uint8) for m in tpv_masks]
+            q = (qc if qc is not None else torch.cat(query, dim=1))[0]
+            out = self.forward_rows(q, q, pos_cat[0], ref_2d[0] if ref_2d.dim() == 5 else ref_2d, [(0, n) for n in split], value,
+                                    spatial_shapes, level_start_index, tpv_levels, reference_points_cams, tpv_vis)
+            return torch.split(out[None], split, 1)
+        norm_i = attn_i = ffn_i = 0
+        identity = query
         cat = lambda views, whole: whole if whole is not None else torch.cat(views, dim=1)
-        # inference: a 'norm' that directly follows an attention / ffn step is folded into that step's last GEMM
-        # (so_linear_3xtf32_ln); `skip_norm` marks it as done (the module reports whether it really applied it)
-        infer = query[0].is_cuda and query[0].dtype == torch.float32 and query[0].shape[0] == 1 and not self.training \
-            and not torch.is_grad_enabled()
-        order = list(self.operation_order)
-        skip_norm = False
-        for oi, op in enumerate(order):
-            nxt = self.norms[norm_i] if (infer and oi + 1 < len(order) and order[oi + 1] == 'norm' and not self.pre_norm) else None
+        for op in self.operation_order:
             if op == 'self_attn':
                 q = cat(query, qc)
                 idt = (q if identity is query else torch.cat(identity, dim=1)) if self.pre_norm else None
-                att = self.attentions[attn_i]
-                qc = att(q, q, q, idt, query_pos=pos_cat, reference_points=ref_2d,
-                         spatial_shapes=tpv_levels[0], level_start_index=tpv_levels[1], fuse_norm=nxt, **kwargs)
-                skip_norm = nxt is not None and getattr(att, 'fused_norm_applied', False)
+                qc = self.attentions[attn_i](q, q, q, idt, query_pos=pos_cat, reference_points=ref_2d,
+                                             spatial_shapes=tpv_levels[0], level_start_index=tpv_levels[1], **kwargs)
                 query = torch.split(qc, split, 1)
                 attn_i += 1
                 identity = query
             elif op == 'norm':
-                if skip_norm:                       # already applied inside the previous step's GEMM epilogue
-                    skip_norm = False
-                    norm_i += 1
-                    continue
                 q = cat(query, qc)
                 ln = self.norms[norm_i]
                 if q.is_cuda and q.dtype == torch.float32 and q.shape[-1] <= 256 and not _needs_grad(q, ln.weight):
@@ -639,29 +573,67 @@ class TPVFormerLayer(nn.Module):
                 query = torch.split(qc, split, 1)
                 norm_i += 1
             elif op == 'cross_attn':
-                fused = query[0].is_cuda and not self.training and not _needs_grad(query[0], key)
-                buf = query[0].new_empty(1, sum(split), query[0].shape[-1]) if (fused and query[0].shape[0] == 1) else None
-                att = self.attentions[attn_i]
-                outs = att(query, key, value, identity if self.pre_norm else None,
-                           spatial_shapes=spatial_shapes, level_start_index=level_start_index,
-                           reference_points_cams=reference_points_cams, tpv_masks=tpv_masks,
-                           tpv_vis=tpv_vis, out_cat=buf, fuse_norm=nxt if fused else None, **kwargs)
-                skip_norm = nxt is not None and fused and getattr(att, 'fused_norm_applied', False)
-                if buf is not None and all(o.data_ptr() == v.data_ptr() for o, v in zip(outs, torch.split(buf, split, 1))):
-                    qc, query = buf, torch.split(buf, split, 1)       # the three planes were written in place
-                else:
-                    qc, query = None, outs
+                query = self.attentions[attn_i](query, key, value, identity if self.pre_norm else None,
+                                                spatial_shapes=spatial_shapes, level_start_index=level_start_index,
+                                                reference_points_cams=reference_points_cams, tpv_masks=tpv_masks,
+                                                tpv_vis=tpv_vis, **kwargs)
+                qc = None
                 attn_i += 1
                 identity = query
             elif op == 'ffn':
                 q = cat(query, qc)
                 idt = (q if identity is query else torch.cat(identity, dim=1)) if self.pre_norm else None
-                ffn = self.ffns[ffn_i]
-                qc = ffn(q, idt, fuse_norm=nxt)
-                skip_norm = nxt is not None and getattr(ffn, 'fused_norm_applied', False)
+                qc = self.ffns[ffn_i](q, idt)
                 query = torch.split(qc, split, 1)
                 ffn_i += 1
         return query
+
+    def _takes_rows(self, q, kwargs):
+        """Whether forward runs as forward_rows: inference at batch 1 in CUDA fp32, batch_first, post-norm order, no mask."""
+        return not self.training and not torch.is_grad_enabled() and q.shape[0] == 1 and _cuda_fp32(q) and self.batch_first \
+            and tuple(self.operation_order) == POST_NORM_ORDER and kwargs.get('key_padding_mask') is None
+
+    def forward_rows(self, q, q_full, pos, ref, slices, value, spatial_shapes, level_start_index, tpv_levels, uvs, vises):
+        """The layer's inference (eval, no autograd, bs = 1, POST_NORM_ORDER) on a set of token rows.
+        q [n, C]: the rows, each plane's contiguous slice in hw | zh | wz order, ``slices`` [(begin, count)] per plane;
+        q_full [Q, C]: all tokens, the self-attention's value; pos [n, C] / ref [n, 3, P, 2]: the rows' positional embedding and
+        cross-view reference points; value [N, sum(hw), 1, C]: the frame's flattened image features with their level tables;
+        tpv_levels: the (spatial_shapes, level_start_index) of the three planes; uvs [N, 1, Q_i, D, 2] / vises [N, Q_i]: each
+        whole plane's camera projections.  Returns the updated rows [n, C].  Every LayerNorm is folded into the GEMM before it.
+        Rows are independent, so any split of the tokens over calls gives bit-identical rows (``dist.ShardedLifter``)."""
+        sa, ca, ffn = self.attentions[0], self.attentions[1], self.ffns[0]
+        # self-attention (cross_view_hybrid_attention.py:63-124): value = all tokens, queries = these rows (+ pos)
+        v = fast_linear(sa.value_proj, q_full)
+        qp = q + pos
+        offs, logits = _offsets_logits(sa, qp)
+        out = ops.tpv_self_attn_forward_rows(v, sa.num_heads, v.shape[1] // sa.num_heads, tpv_levels[0], tpv_levels[1],
+                                             offs, logits, ref.contiguous(), sa.num_levels, sa.num_points)
+        q = fast_linear(sa.output_proj, out, residual=q, ln=self.norms[0])
+        # image cross-attention, one plane at a time (tpvformer/attention/image_cross_attention.py:83-93); the three planes
+        # project the same image features with their own value_proj: one GEMM, three column slices
+        feat = value[:, :, 0].reshape(-1, value.shape[-1])
+        vps = [a.deformable_attention.value_proj for a in ca.attns]
+        vrows = fast_linear_cat(ca, '_so_value3', vps, feat)[1] if _fusable(vps, feat) else None
+        x = q.new_empty(q.shape)                      # each plane's output_proj writes its own row range: no torch.cat
+        o0 = 0
+        for i, (b, c) in enumerate(slices):
+            if c == 0:
+                continue
+            att = ca.attns[i]
+            da = att.deformable_attention
+            qi = q[o0:o0 + c]
+            v = vrows[i] if vrows is not None else fast_linear(da.value_proj, feat)
+            offs, logits = _offsets_logits(da, qi)
+            slots = ops.tpv_cross_attn_forward_rows(v, value.shape[0], da.num_heads, qi.shape[1] // da.num_heads, spatial_shapes,
+                                                    level_start_index, offs, logits, uvs[i][:, 0, b:b + c].contiguous(),
+                                                    vises[i][:, b:b + c].contiguous(), da.num_levels, da.num_points)
+            fast_linear(att.output_proj, slots, residual=qi, out=x[o0:o0 + c], ln=self.norms[1])
+            o0 += c
+        # FFN on [1, n, C]: the layer's forward returns torch.split views of this one token buffer, which the next layer
+        # takes whole (`_whole`) instead of concatenating the planes again
+        x = x[None]
+        h = fast_linear(ffn.layers[0][0], x, relu=True)
+        return fast_linear(ffn.layers[1], h, residual=x if ffn.add_identity else None, ln=self.norms[2])[0]
 
 
 @MODELS.register_module()
@@ -788,14 +760,20 @@ class TPVFormerEncoder(nn.Module):
                 self._pos_cat = torch.cat(vals, 0).unsqueeze(0)      # [1, Q_hw + Q_zh + Q_wz, C]: what every layer concatenates
         return self._pos_val
 
-    def forward(self, representation, ms_img_feats=None, metas=None, **kwargs):
+    def frame_inputs(self, ms_img_feats):
+        """The per-frame inputs every layer reads besides the camera projections (``project_reference_points``):
+        (tpv_pos, feat_flatten, spatial_shapes, level_start_index).  tpv_pos is the cached [1, Q_hw + Q_zh + Q_wz, C]
+        concatenation at bs = 1 without autograd (the layers accept a tensor: no 31 MB cat per layer), else the per-plane list."""
         bs = ms_img_feats[0].shape[0]
         pos = self._tpv_pos()
         if bs == 1 and getattr(self, '_pos_val', None) is pos:
-            tpv_pos = self._pos_cat                               # cached concatenation (the layers accept a tensor): no 31 MB cat per layer
+            tpv_pos = self._pos_cat
         else:
             tpv_pos = [p.unsqueeze(0).repeat(bs, 1, 1) if bs > 1 else p.unsqueeze(0) for p in pos]
-        feat_flatten, spatial_shapes, level_start_index = self.flatten_features(ms_img_feats)
+        return (tpv_pos,) + self.flatten_features(ms_img_feats)
+
+    def forward(self, representation, ms_img_feats=None, metas=None, **kwargs):
+        tpv_pos, feat_flatten, spatial_shapes, level_start_index = self.frame_inputs(ms_img_feats)
         tpv_embed = self.forward_layers(representation, feat_flatten, feat_flatten, tpv_pos=tpv_pos,
                                         spatial_shapes=spatial_shapes, level_start_index=level_start_index, img_metas=metas)
         return {'representation': list(tpv_embed)}

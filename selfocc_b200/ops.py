@@ -682,10 +682,10 @@ def _rows(t, name):
     return t, t.stride(0)
 
 
-def tpv_cross_attn_forward_rows(value_rows, n_cam, Hd, Dh, spatial_shapes, level_start_index, offsets_rows, logits_rows, uv, vis, L, D):
-    """Strided form: value_rows [n_cam*Nv, >= Hd*Dh] view, offsets_rows [Q, Hd*L*D*2] view, logits_rows [Q, Hd*L*D] view."""
+def tpv_cross_attn_forward_rows(value, n_cam, Hd, Dh, spatial_shapes, level_start_index, offsets_rows, logits_rows, uv, vis, L, D):
+    """Strided form: value [n_cam*Nv, >= Hd*Dh] view, offsets_rows [Q, Hd*L*D*2] view, logits_rows [Q, Hd*L*D] view."""
     lib = _lib.load()
-    v, vld = _rows(value_rows, 'value'); o, old = _rows(offsets_rows, 'offsets'); lg, lld = _rows(logits_rows, 'logits')
+    v, vld = _rows(value, 'value'); o, old = _rows(offsets_rows, 'offsets'); lg, lld = _rows(logits_rows, 'logits')
     _chk(uv, name='uv'); _chk(vis, torch.uint8, 'vis')
     Q = o.shape[0]
     Nv = v.shape[0] // n_cam
@@ -696,9 +696,9 @@ def tpv_cross_attn_forward_rows(value_rows, n_cam, Hd, Dh, spatial_shapes, level
     return slots
 
 
-def tpv_self_attn_forward_rows(value_rows, Hd, Dh, spatial_shapes, level_start_index, offsets_rows, logits_rows, ref, L, P):
+def tpv_self_attn_forward_rows(value, Hd, Dh, spatial_shapes, level_start_index, offsets_rows, logits_rows, ref, L, P):
     lib = _lib.load()
-    v, vld = _rows(value_rows, 'value'); o, old = _rows(offsets_rows, 'offsets'); lg, lld = _rows(logits_rows, 'logits')
+    v, vld = _rows(value, 'value'); o, old = _rows(offsets_rows, 'offsets'); lg, lld = _rows(logits_rows, 'logits')
     _chk(ref, name='ref')
     Q = o.shape[0]
     out = torch.empty(Q, Hd * Dh, device=v.device)
