@@ -13,7 +13,11 @@ JSON line (ms per step, device timed; peak device memory of the timed steps).  n
     --loss shipped: the toy loss is replaced by nuscenes_occ's whole MultiLoss (reprojection, RGBLossMS with SSIM,
     EikonalLoss, SecondGradLoss, SemCELossMS), with the head as that config sets it: color_dims = 24, return_sem, and
     return_second_grad under the declared opt-in assumption (second_grad_assumption=True); seeded synthetic previous /
-    current / next / colour images and semantic labels."""
+    current / next / colour images and semantic labels.
+Under torchrun both objectives run ray-sharded: MultiLoss gathers the per-ray loss inputs of every rank (one collective per
+step), so its terms have the 1-GPU values, and each rank prints its last step's terms.  With --loss reproj the printed total
+also holds the toy terms (depth, eikonal and colour means), which stay per-rank means of the rank's own rays and differ
+between ranks and from the 1-GPU run; with --loss shipped the total is the MultiLoss total."""
 import json, os, sys, time
 import numpy as np
 import torch
@@ -38,6 +42,7 @@ cfg = configs.hot_path_config(mapping_args=margs, pc_range=rng, ray_number=(48, 
 if shipped:
     cfg['head'].update(return_second_grad=True, second_grad_assumption=True)
 torch.manual_seed(0)
+np.random.seed(0)                  # every rank must draw the same cellular ray grid (RaySampler.draw uses numpy)
 model = build_head(cfg)
 model.encoder.init_weights()
 with torch.no_grad():
@@ -61,8 +66,9 @@ if shipped:
                     sem=lab)
     imgs = synth.textured_images(24, 768, 1600, seed=2).reshape(4, 1, 6, 3, 768, 1600).to(dev)
 if loss_mode == 'reproj':
-    from selfocc_b200.loss import ReprojLossMonoMultiNewCombine
-    reproj = ReprojLossMonoMultiNewCombine(img_size=[768, 1600], ray_resize=[48, 100])
+    from selfocc_b200.loss import MultiLoss
+    # inside a MultiLoss so that a ray-sharded step gathers the per-ray statistics for SSIM over the whole ray grid
+    reproj = MultiLoss([dict(type='ReprojLossMonoMultiNewCombine', img_size=[768, 1600], ray_resize=[48, 100])])
     prev, nxt = synth.temporal_rig()
     metas[0].update(img2prevImg=torch.tensor(prev, dtype=torch.float32, device=dev), img2nextImg=torch.tensor(nxt, dtype=torch.float32, device=dev))
     imgs = synth.textured_images(18, 768, 1600, seed=2).reshape(3, 1, 6, 3, 768, 1600).to(dev)
@@ -83,18 +89,23 @@ class _Step(torch.nn.Module):
 model.forward = lambda feats, metas: _Step.forward(None, feats, metas)
 
 
+terms = {}
+
+
 def step():
     opt.zero_grad(set_to_none=True)
     out = net(feats, metas)
     if objective is not None:
-        loss, _ = objective(dict(out, curr_imgs=imgs[0], prev_imgs=imgs[1], next_imgs=imgs[2], color_imgs=imgs[3], metas=metas))
+        loss, terms_ = objective(dict(out, curr_imgs=imgs[0], prev_imgs=imgs[1], next_imgs=imgs[2], color_imgs=imgs[3], metas=metas))
+        terms.update(terms_)
         loss.backward()
         opt.step()
         return loss.detach()
     if reproj is None:
         w_term = torch.cat(out['weights']).pow(2).mean()
     else:
-        w_term = reproj(dict(out, curr_imgs=imgs[0], prev_imgs=imgs[1], next_imgs=imgs[2], metas=metas))
+        w_term, terms_ = reproj(dict(out, curr_imgs=imgs[0], prev_imgs=imgs[1], next_imgs=imgs[2], metas=metas))
+        terms.update(terms_)
     loss = out['ms_depths'][0].mean() * 1e-2 + w_term \
         + (out['eik_grad'].norm(dim=-1) - 1).pow(2).mean() * 0.1 + out['ms_colors'][0].mean() * 0.1
     loss.backward()
@@ -126,6 +137,9 @@ if '--profile' in sys.argv and world == 1:
         step()
         torch.cuda.synchronize()
     print(prof.key_averages().table(sort_by='cuda_time_total', row_limit=25))
+if world > 1 and terms:            # the last step's loss terms on every rank: ray sharding gives every rank the same values
+    print(json.dumps({'rank': rank, 'terms': {k: float(v) for k, v in terms.items()}}), flush=True)
+    dist.barrier()
 if rank == 0:
   print(json.dumps({'workload': 'nuscenes_occ-like training step, %d GPU(s)%s, fp32, 6x48x100 rays x 256, TPV 257x257x25, colour%s' % (world, ' ray-sharded + DDP' if world > 1 else '', ', reprojection loss' if reproj is not None else ', nuscenes_occ MultiLoss (24 colour dims, semantics, second grad)' if shipped else ''), 'ms_per_step': ms,
                   'rays_per_s': 28800 / (ms * 1e-3), 'library_launches_per_step': (_lib.launch_count() - l0) / K, 'peak_mem_gb': peak_gb,

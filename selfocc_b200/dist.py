@@ -1,7 +1,11 @@
 """Multi-GPU plumbing for the render path (SURVEY.md 8e): rays are independent given the decoded
 volume, so the flat (cam, ray) order of neus_head.py:324-325 is split into contiguous per-rank slices
 (the same split ``torch.chunk`` produces) and the rendered maps are put back together with ONE
-all_gather.  Backend-agnostic (``nccl`` on the GPUs, ``gloo`` in the CPU tests)."""
+all_gather.  Ray-sharded TRAINING slices every camera's rays instead (head.ray_shard) and gathers the loss
+inputs per camera, differentiably (all_gather_ray_payload).  Backend-agnostic (``nccl`` on the GPUs, ``gloo`` in
+the CPU tests)."""
+import math
+
 import torch
 import torch.distributed as dist
 
@@ -37,29 +41,80 @@ def all_gather_rays(local, total, group=None):
     return out[:total]
 
 
+def pack_planar(tensors, totals, world, dtype=None):
+    """This rank's payload -> the 1-D buffer one all_gather_into_tensor exchanges.  tensors[i] is [L, count_i, k] (L rows of
+    slices, e.g. one per camera); its slice is padded to ceil(totals[i] / world) along dim 1.  The buffer is PLANAR (tensor
+    after tensor -- contiguous copies; an interleaved [count, sum k] pack would cost a strided write of every column)."""
+    sizes = [t.shape[0] * -(-n // world) * t.shape[2] for t, n in zip(tensors, totals)]
+    buf = tensors[0].new_zeros(sum(sizes), dtype=dtype)
+    off = 0
+    for t, n, size in zip(tensors, totals, sizes):
+        buf[off:off + size].view(t.shape[0], -1, t.shape[2])[:, :t.shape[1]] = t
+        off += size
+    return buf
+
+
+def unpack_planar(out, tensors, totals, world):
+    """The gathered [world * per-rank buffer] -> for each tensor of pack_planar its full [L, totals[i], k] (views of out)."""
+    out = out.view(world, -1)
+    res, off = [], 0
+    for t, n in zip(tensors, totals):
+        L, per, k = t.shape[0], -(-n // world), t.shape[2]
+        res.append(out[:, off:off + L * per * k].reshape(world, L, per, k).transpose(0, 1).reshape(L, world * per, k)[:, :n])
+        off += L * per * k
+    return res
+
+
 def all_gather_planar(tensors, total, group=None):
     """Several per-ray tensors of this rank ([count] or [count, k], same count) -> their full versions ([total, ...]) with ONE
-    collective: the payload is packed PLANAR (tensor after tensor, each padded to the common per-rank length -- contiguous
-    copies; an interleaved [count, sum k] pack would cost a strided write of every column)."""
+    collective (pack_planar)."""
     if not dist.is_available() or not dist.is_initialized() or dist.get_world_size(group) == 1:
         return list(tensors)
     world = dist.get_world_size(group)
-    per = -(-total // world)
-    widths = [1 if t.dim() == 1 else t.shape[1] for t in tensors]
-    buf = tensors[0].new_zeros(sum(widths) * per)
-    off = 0
-    for t, w in zip(tensors, widths):
-        buf[off:off + t.numel()] = t.reshape(-1)
-        off += w * per
+    views = [t.reshape(1, t.shape[0], math.prod(t.shape[1:])) for t in tensors]     # explicit width: empty slices too
+    buf = pack_planar(views, [total] * len(views), world)
     out = buf.new_empty(world * buf.numel())                     # concatenated form: accepted by nccl AND gloo
     dist.all_gather_into_tensor(out, buf, group=group)
-    out = out.view(world, buf.numel())
-    res, off = [], 0
-    for t, w in zip(tensors, widths):
-        full = out[:, off:off + w * per].reshape(world * per, *([w] if t.dim() > 1 else []))[:total]
-        res.append(full.contiguous())
-        off += w * per
-    return res
+    full = unpack_planar(out, views, [total] * len(views), world)
+    return [f.reshape((total,) + tuple(t.shape[1:])).contiguous() for f, t in zip(full, tensors)]
+
+
+class _RayPayloadGather(torch.autograd.Function):
+    """forward: this rank's [L, count_i, k] slices -> the full [L, totals[i], k] tensors; backward: world x the incoming
+    gradient at this rank's own rows (see all_gather_ray_payload)."""
+
+    @staticmethod
+    def forward(ctx, spec, *tensors):
+        rank, world, totals, collective = spec
+        buf = pack_planar(tensors, totals, world, dtype=torch.float64)
+        out = buf.new_empty(world * buf.numel())
+        collective(out, buf)
+        ctx.world = world
+        ctx.rows = [ray_slice(n, world, rank) for n in totals]
+        ctx.set_materialize_grads(False)
+        return tuple(f.to(t.dtype).contiguous() for f, t in zip(unpack_planar(out, tensors, totals, world), tensors))
+
+    @staticmethod
+    def backward(ctx, *grads):
+        return (None,) + tuple(None if g is None else g[:, b:b + c] * ctx.world for g, (b, c) in zip(grads, ctx.rows))
+
+
+def all_gather_ray_payload(tensors, totals, rank, world, collective=None, group=None):
+    """Per-camera ray payloads of a ray-sharded step -> their full versions on every rank, with ONE collective.
+
+    tensors[i] is this rank's [L, count_i, k] slice of a [L, totals[i], k] tensor: rank r holds rows ray_slice(totals[i],
+    world, r) of every one of the L rows (the head's ray_shard gives each rank the same slice of every camera's rays; a
+    per-rank scalar is a [1, 1, k] slice of totals[i] = world).  The payload travels in fp64 (exact for fp32 inputs) and comes
+    back in each tensor's dtype.  ``collective(out, buf)`` fills ``out`` [world * buf.numel()] with every rank's ``buf`` in
+    rank order; default: dist.all_gather_into_tensor over ``group``.
+
+    Gradient contract: every rank evaluates the SAME loss graph on the gathered tensors, so rank r's share of the full
+    gradient is the incoming gradient at its own rows.  The backward returns world x that (no collective): parameter
+    gradients averaged over the ranks, as DistributedDataParallel does, are then the full gradient."""
+    if collective is None:
+        def collective(out, buf):
+            dist.all_gather_into_tensor(out, buf, group=group)
+    return list(_RayPayloadGather.apply((rank, world, list(totals), collective), *tensors))
 
 
 def _num_cams(head, metas):

@@ -12,7 +12,16 @@ def chunk_cams(tensor, num_cams):
 
 
 def forward_train(head, representation, metas=None, jitter=None, bkgd_rand=None, uniform_shift=None, **kwargs):
-    """uniform_shift: the [H*W*D, 3] lattice jitter in [0, 1) of get_uniform_sdf (default: drawn here)."""
+    """uniform_shift: the [H*W*D, 3] lattice jitter in [0, 1) of get_uniform_sdf (default: drawn here).
+
+    Ray-sharded training: with ``head.ray_shard = (rank, world)``, world > 1, this rank renders the rank-th contiguous slice
+    (dist.ray_slice) of every camera's rays and ``outputs['ray_shard'] = (rank, world, R_full)`` tells MultiLoss to gather
+    its inputs across the ranks.  Every rank must see the same frame and the same random numbers: give every rank the same
+    training frames (a distributed sampler that hands each rank its own frames must be built with one replica) and seed
+    torch AND numpy identically on all ranks (the reference's train.py seeds them; INTEGRATION.md lists what else it needs
+    for a sharded run).  The cellular ray grid comes from numpy (RaySampler.draw); the stratified
+    jitter and the random background are drawn for all rays and sliced; the uniform_sdf lattice shift and the encoder's
+    dropout masks are then drawn identically.  An explicit ``jitter`` / ``bkgd_rand`` is this rank's slice."""
     f = head.model.field
     hw, zh, wz = representation
     assert hw.shape[0] == 1, 'only support bs = 1 currently'
@@ -26,13 +35,15 @@ def forward_train(head, representation, metas=None, jitter=None, bkgd_rand=None,
     sampler = head._sampler()
     grid = sampler.draw()
     rays = sampler.table(grid)
+    r_full = rays.shape[0]
     shard = getattr(head, 'ray_shard', None)
-    if shard is not None and shard[1] > 1:
+    sharded = shard is not None and shard[1] > 1
+    if sharded:
         # ray-sharded training (BASELINE configs[4]): rank r renders the r-th contiguous slice of EVERY camera's pixel rays, so the
-        # per-camera output lists the losses consume keep their structure (fewer rays per camera); with every rank on the same
-        # frame and the loss a mean over rays, averaging the parameter gradients over ranks (DDP) gives the full-batch gradient
+        # per-camera output lists the losses consume keep their structure (fewer rays per camera); MultiLoss gathers the loss
+        # inputs across the ranks (outputs['ray_shard'])
         from .dist import ray_slice
-        b, c = ray_slice(rays.shape[0], shard[1], shard[0])
+        b, c = ray_slice(r_full, shard[1], shard[0])
         rays, grid = rays[b:b + c].contiguous(), None
     M = head.img2lidar.matrices(metas, dev)
     bs, num_cams = M.shape[:2]
@@ -41,11 +52,18 @@ def forward_train(head, representation, metas=None, jitter=None, bkgd_rand=None,
     total = num_cams * num_rays
     S = head.num_samples
     training = head.training
+
+    def draw(k):
+        """torch.rand for every camera's rays; a sharded rank draws the FULL set and keeps its slice, so every rank consumes
+        the torch RNG identically and its rays get the numbers the unsharded step gives them"""
+        if not sharded:
+            return torch.rand(total, k, device=dev)
+        return torch.rand(num_cams, r_full, k, device=dev)[:, b:b + c].reshape(total, k)
     if jitter is None and training:                       # perturb=True: stratified jitter (upstream UniformSampler)
-        jitter = torch.rand(total, S + 1, device=dev)
+        jitter = draw(S + 1)
     has_rgb = f.color_dims >= 3
     if bkgd_rand is None and head.render_bkgd == 'random' and has_rgb:
-        bkgd_rand = torch.rand(total, 3, device=dev)
+        bkgd_rand = draw(3)
     inv_s = f.deviation_network.get_variance()
     params = ops.make_render_params(head.aabb, S, float(inv_s), near_plane=head.near_plane, training=training,
                                     cos_anneal=head.cos_anneal_ratio, anchor_mid=head.sample_anchor == 'mid', sh_act=f.sh_act,
@@ -114,6 +132,8 @@ def forward_train(head, representation, metas=None, jitter=None, bkgd_rand=None,
         outputs['sample_sdf'] = sample_sdf_for_cams
     if head.return_sem:
         outputs['sem'] = [sem]
+    if sharded:
+        outputs['ray_shard'] = (shard[0], shard[1], r_full)
     return outputs
 
 

@@ -16,6 +16,11 @@ call, as the reference does), whose ``add_scalar`` reads a count.
 Input layout: every camera's ``weights`` / ``ts`` (/ ``deltas``) entry holds R * S values ray-major (S samples per ray,
 R = len(ms_rays)), which is what ``NeuSHead.forward`` emits (``ray_indices[cam]`` = arange(R).repeat_interleave(S)); the
 kernel uses that layout and does not read ``ray_indices``, whose lengths are checked.  Batch size 1, fp32, CUDA.
+
+Ray-sharded training (MultiLoss.forward with inputs['ray_shard']): every term splits into ``local_payload`` (the per-ray
+quantities of this rank's rays: the reprojection statistics, colours and image values at the ray pixels, depths, the
+semantic elements; a per-sample term's sum and count) and ``from_gathered`` (the same tail formulas as the unsharded
+term, on the full ray grid).
 """
 import numpy as np
 import torch
@@ -72,7 +77,20 @@ class _ReprojLoss(nn.Module):
         """BaseLoss.forward: weight * loss over the inputs named by input_dict."""
         return self.weight * self.reproj_loss(**{k: inputs[v] for k, v in self.input_dict.items()})
 
-    def _stats(self, curr_imgs, prev_imgs, next_imgs, ray_indices, weights, ts, metas, ms_rays, deltas):
+    def reproj_loss(self, curr_imgs, prev_imgs, next_imgs, ray_indices, weights, ts, metas, ms_rays, deltas=None,
+                    sample_sdfs=None):
+        return self.tail(*self._stats(curr_imgs, prev_imgs, next_imgs, ray_indices, weights, ts, metas, ms_rays, deltas))
+
+    # ray-sharded evaluation (MultiLoss): the per-ray statistics of this rank's rays, the tail on the gathered grid
+    def local_payload(self, inputs, shard):
+        kw = {k: inputs[v] for k, v in self.input_dict.items() if k != 'sample_sdfs'}
+        stats, colours, _ = self._stats(**kw, full_grid=False)
+        return [(stats, shard[2]), (colours, shard[2])]
+
+    def from_gathered(self, full, inputs):
+        return self.weight * self.tail(full[0], full[1], inputs[self.input_dict['curr_imgs']].shape[1])
+
+    def _stats(self, curr_imgs, prev_imgs, next_imgs, ray_indices, weights, ts, metas, ms_rays, deltas=None, full_grid=True):
         bs, num_cams = curr_imgs.shape[:2]
         if bs != 1:
             raise NotImplementedError('batch size %d: the reprojection loss supports batch size 1 (as the reference)' % bs)
@@ -88,7 +106,7 @@ class _ReprojLoss(nn.Module):
                 raise ValueError('%s must have %d entries of %d samples (R = %d rays x S = %d), as weights' % (k, n_cam, n, R, n // R))
         if n_cam > num_cams:
             raise ValueError('%d cameras of weights but %d images' % (n_cam, num_cams))
-        if not self.no_ssim and R != self.ray_resize[0] * self.ray_resize[1]:
+        if full_grid and not self.no_ssim and R != self.ray_resize[0] * self.ray_resize[1]:
             raise ValueError('SSIM needs the rays to fill ray_resize %s, got %d rays (ray sharding or a partial ray set: '
                              'set no_ssim=True)' % (self.ray_resize, R))
         dev = weights[0].device
@@ -134,8 +152,7 @@ class ReprojLossMonoMultiNewCombine(_ReprojLoss):
     per ray 0.15 l1 + 0.85 SSIM of the weighted colour over the ray grid, min with the two automask terms."""
     MODE = 'combine'
 
-    def reproj_loss(self, curr_imgs, prev_imgs, next_imgs, ray_indices, weights, ts, metas, ms_rays, deltas=None):
-        stats, colours, num_cams = self._stats(curr_imgs, prev_imgs, next_imgs, ray_indices, weights, ts, metas, ms_rays, deltas)
+    def tail(self, stats, colours, num_cams):
         cur = colours[..., 0:3]
         l1, rgb, any_valid = self._set(stats, 0)
         loss = self._photometric(rgb, cur, l1)
@@ -160,9 +177,7 @@ class ReprojLossMonoMultiNew(_ReprojLoss):
         self.sdf_loss = sdf_loss
         self.sdf_loss_weight = sdf_loss_weight
 
-    def reproj_loss(self, curr_imgs, prev_imgs, next_imgs, ray_indices, weights, ts, metas, ms_rays, deltas=None,
-                    sample_sdfs=None):
-        stats, colours, num_cams = self._stats(curr_imgs, prev_imgs, next_imgs, ray_indices, weights, ts, metas, ms_rays, deltas)
+    def tail(self, stats, colours, num_cams):
         cur = colours[..., 0:3]
         cands = []
         for j in (0, 1):
@@ -196,11 +211,34 @@ class _Term(nn.Module):
         self.writer = None
 
     def forward(self, inputs):
-        return self.weight * self.loss_func(**{k: inputs[v] for k, v in self.input_dict.items()})
+        return self.weight * self.loss_func(**self._args(inputs))
+
+    def _args(self, inputs):
+        return {k: inputs[v] for k, v in self.input_dict.items()}
+
+    # ray-sharded evaluation (MultiLoss.forward with inputs['ray_shard']): local_payload(inputs, (rank, world, R_full)) ->
+    # [(this rank's [L, count, k] slice, its full length)]; from_gathered(full tensors, inputs) -> weight * loss
+    def local_payload(self, inputs, shard):
+        raise NotImplementedError('%s under ray sharding' % type(self).__name__)
+
+
+class _SampleMeanTerm(_Term):
+    """A per-sample mean over the rays' samples: under ray sharding each rank sends its mean times its element count and
+    that count (the full mean is the ratio of the sums; elements per sample cancel)."""
+
+    def local_payload(self, inputs, shard):
+        x, = self._args(inputs).values()
+        n = x.numel()
+        part = self.loss_func(x).double() * n if n else x.new_zeros((), dtype=torch.float64)
+        return [(torch.stack([part, part.new_full((), float(n))]).reshape(1, 1, 2), shard[1])]
+
+    def from_gathered(self, full, inputs):
+        s = full[0][0].sum(0)                                   # over the ranks: (sum, count)
+        return self.weight * (s[0] / s[1]).float()
 
 
 @LOSSES.register_module()
-class EikonalLoss(_Term):
+class EikonalLoss(_SampleMeanTerm):
     """mean over samples of (|eik_grad|_2 - 1)^2 (loss/eikonal_loss.py)."""
     DEFAULT_KEYS = ('eik_grad',)
 
@@ -212,7 +250,7 @@ class EikonalLoss(_Term):
 
 
 @LOSSES.register_module()
-class SecondGradLoss(_Term):
+class SecondGradLoss(_SampleMeanTerm):
     """mean |second_grad| (loss/second_grad_loss.py)."""
     DEFAULT_KEYS = ('second_grad',)
 
@@ -233,6 +271,17 @@ class SoftSparsityLoss(_Term):
 
     def loss_func(self, density):
         return ops.SampleMeanFunction.apply(density, 'neg_relu')
+
+    # under ray sharding the uniform_sdf lattice is the same on every rank: each rank computes the whole term, unscaled, and
+    # the average over the ranks of its (equal) gradients is the gradient
+    def local_payload(self, inputs, shard):
+        if self.input_dict['density'] != 'uniform_sdf':
+            raise NotImplementedError('SoftSparsityLoss under ray sharding takes the replicated uniform_sdf, got %r'
+                                      % self.input_dict['density'])
+        return []
+
+    def from_gathered(self, full, inputs):
+        return self(inputs)
 
 
 def sample_at_rays(imgs, rays, img_size, padding):
@@ -272,11 +321,27 @@ class RGBLossMS(_Term):
 
     def loss_func(self, ms_colors, ms_rays, gt_imgs):
         rays = _single_rays(ms_rays, 'RGBLossMS')
-        bs, num_cams = gt_imgs.shape[:2]
-        R = rays.shape[0]
         if not self.no_ssim:
-            _check_grid(self.ray_resize, R, 'RGBLossMS with SSIM')
-        gt = sample_at_rays(gt_imgs.flatten(0, 1), rays, self.img_size, 'zeros')          # [B*N, 3, R]
+            _check_grid(self.ray_resize, rays.shape[0], 'RGBLossMS with SSIM')
+        return self._tail(ms_colors, self._gt(rays, gt_imgs), gt_imgs)
+
+    def _gt(self, rays, gt_imgs):
+        return sample_at_rays(gt_imgs.flatten(0, 1), rays, self.img_size, 'zeros')          # [B*N, 3, R]
+
+    def local_payload(self, inputs, shard):
+        a = self._args(inputs)
+        gt = self._gt(_single_rays(a['ms_rays'], 'RGBLossMS'), a['gt_imgs'])
+        return [(c.flatten(0, 1), shard[2]) for c in a['ms_colors']] + [(gt.transpose(1, 2), shard[2])]
+
+    def from_gathered(self, full, inputs):
+        gt_imgs = self._args(inputs)['gt_imgs']
+        colors = [c.reshape(*gt_imgs.shape[:2], *c.shape[1:]) for c in full[:-1]]
+        return self.weight * self._tail(colors, full[-1].transpose(1, 2).contiguous(), gt_imgs)
+
+    def _tail(self, ms_colors, gt, gt_imgs):
+        """The loss from the colours [B, N, R, 3] and the ground truth at the ray pixels [B*N, 3, R] on the ray grid."""
+        bs, num_cams = gt_imgs.shape[:2]
+        R = gt.shape[-1]
         gt_grid = None if self.no_ssim else gt.reshape(bs * num_cams, 3, *self.ray_resize)
         gt = gt.reshape(bs, num_cams, 3, R).transpose(-1, -2)
         tot = 0.
@@ -320,6 +385,15 @@ class _SemTerm(_Term):
         gt = _sem_labels(metas, rays, sem[0].device)
         return sum(self.term(s, gt) for s in sem) / len(sem)
 
+    # under ray sharding: the elements the term averages, [B, N, count, k] per scale (per_ray), gathered, then their mean
+    def local_payload(self, inputs, shard):
+        a = self._args(inputs)
+        gt = _sem_labels(a['metas'], _single_rays(a['ms_rays'], type(self).__name__), a['sem'][0].device)
+        return [(self.per_ray(s, gt).flatten(0, 1), shard[2]) for s in a['sem']]
+
+    def from_gathered(self, full, inputs):
+        return self.weight * (sum(e[None].mean() for e in full) / len(full))
+
 
 @LOSSES.register_module()
 class SemLossMS(_SemTerm):
@@ -330,6 +404,10 @@ class SemLossMS(_SemTerm):
     def term(s, gt):
         return F.binary_cross_entropy(torch.clamp(s, 0, 1), F.one_hot(gt, num_classes=s.shape[-1]).to(s.dtype))
 
+    @staticmethod
+    def per_ray(s, gt):
+        return F.binary_cross_entropy(torch.clamp(s, 0, 1), F.one_hot(gt, num_classes=s.shape[-1]).to(s.dtype), reduction='none')
+
 
 @LOSSES.register_module()
 class SemCELossMS(_SemTerm):
@@ -338,7 +416,11 @@ class SemCELossMS(_SemTerm):
 
     @staticmethod
     def term(s, gt):
-        return -torch.log(torch.clamp(s.gather(-1, gt.unsqueeze(-1)), 1e-6, 1)).mean()
+        return SemCELossMS.per_ray(s, gt).mean()
+
+    @staticmethod
+    def per_ray(s, gt):
+        return -torch.log(torch.clamp(s.gather(-1, gt.unsqueeze(-1)), 1e-6, 1))
 
 
 def _smooth(disp, img):
@@ -364,22 +446,41 @@ class EdgeLoss3DMS(_Term):
         self.ray_resize = list(self.ray_resize)
 
     def loss_func(self, curr_imgs, ms_depths, ms_rays, ms_accs=None, max_depths=None):
+        _check_grid(self.ray_resize, ms_depths[0].shape[2], 'EdgeLoss3DMS')
+        return self._tail(self._rays(curr_imgs, ms_depths, ms_rays, ms_accs, max_depths))
+
+    def _rays(self, curr_imgs, ms_depths, ms_rays, ms_accs=None, max_depths=None):
+        """Per scale the depth [B, N, R] (blended by the inf mask) and the current image at the ray pixels [B*N, 3, R]."""
         if self.use_inf_mask:
             assert ms_accs is not None and max_depths is not None
         if not isinstance(ms_rays, (list, tuple)):
             ms_rays = [ms_rays] * len(ms_depths)
-        bs, num_cams, num_rays = ms_depths[0].shape
-        _check_grid(self.ray_resize, num_rays, 'EdgeLoss3DMS')
         imgs = curr_imgs.flatten(0, 1)
-        tot = 0.
+        out = []
         for scale, (depth, rays) in enumerate(zip(ms_depths, ms_rays)):
-            rgb = sample_at_rays(imgs, rays, self.img_size, 'border').reshape(bs * num_cams, -1, *self.ray_resize)
+            rgb = sample_at_rays(imgs, rays, self.img_size, 'border')
             if self.use_inf_mask:
                 depth = depth * ms_accs[scale] + max_depths[scale] * (1 - ms_accs[scale])
-            depth = depth.reshape(bs * num_cams, 1, *self.ray_resize)
+            out.append((depth, rgb))
+        return out
+
+    def _tail(self, per_scale):
+        tot = 0.
+        for depth, rgb in per_scale:
+            depth = depth.reshape(-1, 1, *self.ray_resize)
+            rgb = rgb.reshape(depth.shape[0], -1, *self.ray_resize)
             norm = depth / (depth.mean(2, True).mean(3, True) + 1e-6)
             tot = tot + _smooth(norm, rgb)
-        return tot / len(ms_depths)
+        return tot / len(per_scale)
+
+    def local_payload(self, inputs, shard):
+        pay = []
+        for depth, rgb in self._rays(**self._args(inputs)):
+            pay += [(depth.reshape(-1, depth.shape[-1], 1), shard[2]), (rgb.transpose(1, 2), shard[2])]
+        return pay
+
+    def from_gathered(self, full, inputs):
+        return self.weight * self._tail([(d, rgb.transpose(1, 2).contiguous()) for d, rgb in zip(full[0::2], full[1::2])])
 
 
 @LOSSES.register_module()
@@ -396,13 +497,43 @@ class MultiLoss(nn.Module):
         self.losses = nn.ModuleList([LOSSES.build(c) for c in loss_cfgs])
         self.iter_counter = 0
         self.writer = None
+        self.group = None             # process group of a ray-sharded step (None: the default group)
+        self.collective = None        # collective(out, buf) of dist.all_gather_ray_payload (None: all_gather_into_tensor)
 
     def forward(self, inputs):
+        """With inputs['ray_shard'] = (rank, world, R_full), world > 1 (NeuSHead under head.ray_shard), the inputs hold this
+        rank's slice of every camera's rays and the objective runs in two stages: local_payload (the per-ray quantities of
+        this rank's rays), ONE gather of every term's payload, and from_gathered (each term's formulas on the full ray grid).
+        Every rank then returns the unsharded loss values; the gradients follow dist.all_gather_ray_payload's contract
+        (averaged over the ranks, as DistributedDataParallel does, they are the unsharded gradients)."""
+        shard = inputs.get('ray_shard')
+        if shard is not None and shard[1] > 1:
+            return self.from_gathered(self.gather(self.local_payload(inputs), shard[0], shard[1]), inputs)
+        return self._total(loss_func(inputs) for loss_func in self.losses)
+
+    def local_payload(self, inputs):
+        """Stage 1 of a ray-sharded step: per term a list of (this rank's [L, count, k] slice, its full length)."""
+        shard = inputs['ray_shard']
+        return [loss_func.local_payload(inputs, shard) for loss_func in self.losses]
+
+    def gather(self, payload, rank, world):
+        """local_payload's slices of every rank -> per term the list of full tensors, in one collective."""
+        from .dist import all_gather_ray_payload
+        flat = [p for term in payload for p in term]
+        if not flat:
+            return payload
+        full = iter(all_gather_ray_payload([t for t, _ in flat], [n for _, n in flat], rank, world, self.collective, self.group))
+        return [[next(full) for _ in term] for term in payload]
+
+    def from_gathered(self, full, inputs):
+        """Stage 2 of a ray-sharded step: (tot_loss, loss_dict) from gather's full tensors."""
+        return self._total(loss_func.from_gathered(f, inputs) for loss_func, f in zip(self.losses, full))
+
+    def _total(self, losses):
         loss_dict = {}
         tot_loss = 0.
         log = self.writer is not None and self.iter_counter % 10 == 0
-        for loss_func in self.losses:
-            loss = loss_func(inputs)
+        for loss_func, loss in zip(self.losses, losses):
             tot_loss = tot_loss + loss
             name = loss_func.__class__.__name__
             loss_dict[name] = loss.detach()
