@@ -17,7 +17,14 @@ JSON line (ms per step, device timed; peak device memory of the timed steps).  n
 Under torchrun both objectives run ray-sharded: MultiLoss gathers the per-ray loss inputs of every rank (one collective per
 step), so its terms have the 1-GPU values, and each rank prints its last step's terms.  With --loss reproj the printed total
 also holds the toy terms (depth, eikonal and colour means), which stay per-rank means of the rank's own rays and differ
-between ranks and from the 1-GPU run; with --loss shipped the total is the MultiLoss total."""
+between ranks and from the 1-GPU run; with --loss shipped the total is the MultiLoss total.
+    --shard-encoder (under torchrun): the encoder's training pass is query-sharded too (encoder.query_shard, its exchange on
+    its own NCCL process group): each rank runs every layer on its 1/world of each plane, one all_gather per layer forward
+    and one reduce-scatter per layer backward.
+    --emulate-world W (one process): ONE rank's share of a W-rank step with both shardings on one GPU -- rank 0's rows
+    through every layer, a local stand-in for the exchange (it fills the other ranks' rows with this rank's buffer and returns
+    this rank's own gradient rows, talking to no one), the head on rank 0's ray slice.  Compute per rank, communication
+    excluded; the loss value is not the W-rank step's."""
 import json, os, sys, time
 import numpy as np
 import torch
@@ -36,6 +43,10 @@ if world > 1:
 margs = dict(synth.NUSC_MAPPING, h_size=[128, 0], h_range=[40.0, 0], w_size=[128, 0], w_range=[40.0, 0], d_size=[24, 0], d_range=[-1.0, 5.4, 5.4])
 rng = [-40.0, -40.0, -1.0, 40.0, 40.0, 5.4]
 loss_mode = sys.argv[sys.argv.index('--loss') + 1] if '--loss' in sys.argv else None
+emulate = int(sys.argv[sys.argv.index('--emulate-world') + 1]) if '--emulate-world' in sys.argv else 0
+shard_encoder = '--shard-encoder' in sys.argv
+if emulate and world > 1:
+    raise SystemExit('--emulate-world runs in one process (it emulates one rank of the W-rank step)')
 shipped = loss_mode == 'shipped'
 cfg = configs.hot_path_config(mapping_args=margs, pc_range=rng, ray_number=(48, 100), ray_img_size=(768, 1600), color_dims=24 if shipped else 3,
                               ray_sample_mode='cellular', render_bkgd='random', return_max_depth=False, dropout=0.1, return_sem=shipped)
@@ -75,13 +86,37 @@ if loss_mode == 'reproj':
 net = model
 if world > 1:
     model.head.ray_shard = (rank, world)
+    if shard_encoder:
+        model.encoder.query_shard = (rank, world)
+        model.encoder.query_shard_group = dist.new_group(backend='nccl')
     net = torch.nn.parallel.DistributedDataParallel(model, device_ids=[local], broadcast_buffers=False)
+
+
+def local_gather(out, buf):
+    """the stand-in all_gather of --emulate-world: every rank's slot gets this rank's buffer"""
+    out.view(emulate, -1).copy_(buf.reshape(1, -1).expand(emulate, -1))
+
+
+def local_reduce_scatter(out, buf):
+    """the stand-in reduce-scatter of --emulate-world: this rank's block of its own gradient"""
+    out.copy_(buf.view(emulate, -1)[0].view_as(out))
+
+
+if emulate:
+    model.head.ray_shard = (0, emulate)
+    for ml_ in (objective, reproj):
+        if ml_ is not None:
+            ml_.collective = local_gather
 
 
 class _Step(torch.nn.Module):
     """the whole hot path as ONE forward so that DDP sees a single module call"""
     def forward(self, feats, metas):
         r = model.lifter(ms_img_feats=feats)
+        if emulate:
+            rep = model.encoder.forward_query_sharded(r['representation'], feats, metas, 0, emulate, local_gather,
+                                                      local_reduce_scatter)
+            return model.head(representation=rep, metas=metas)
         r = model.encoder(representation=r['representation'], ms_img_feats=feats, metas=metas)
         return model.head(representation=r['representation'], metas=metas)
 
@@ -140,8 +175,14 @@ if '--profile' in sys.argv and world == 1:
 if world > 1 and terms:            # the last step's loss terms on every rank: ray sharding gives every rank the same values
     print(json.dumps({'rank': rank, 'terms': {k: float(v) for k, v in terms.items()}}), flush=True)
     dist.barrier()
+if emulate:
+    mode = ', ONE rank of %d emulated (query- and ray-sharded): compute per rank, communication excluded' % emulate
+elif world > 1:
+    mode = ' ray-sharded%s + DDP' % (' + query-sharded encoder' if shard_encoder else '')
+else:
+    mode = ''
 if rank == 0:
-  print(json.dumps({'workload': 'nuscenes_occ-like training step, %d GPU(s)%s, fp32, 6x48x100 rays x 256, TPV 257x257x25, colour%s' % (world, ' ray-sharded + DDP' if world > 1 else '', ', reprojection loss' if reproj is not None else ', nuscenes_occ MultiLoss (24 colour dims, semantics, second grad)' if shipped else ''), 'ms_per_step': ms,
+  print(json.dumps({'workload': 'nuscenes_occ-like training step, %d GPU(s)%s, fp32, 6x48x100 rays x 256, TPV 257x257x25, colour%s' % (world, mode, ', reprojection loss' if reproj is not None else ', nuscenes_occ MultiLoss (24 colour dims, semantics, second grad)' if shipped else ''), 'ms_per_step': ms,
                   'rays_per_s': 28800 / (ms * 1e-3), 'library_launches_per_step': (_lib.launch_count() - l0) / K, 'peak_mem_gb': peak_gb,
                   'loss': float(last), 'finite': bool(torch.isfinite(last))}))
 if world > 1:

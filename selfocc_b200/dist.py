@@ -117,6 +117,136 @@ def all_gather_ray_payload(tensors, totals, rank, world, collective=None, group=
     return list(_RayPayloadGather.apply((rank, world, list(totals), collective), *tensors))
 
 
+# ---------------------------------------------------------------------------------------- per-plane row slices of the TPV
+# A query-sharded rank owns the contiguous slice ray_slice(Q_i, world, rank) of EACH plane i (sizes = [Q_hw, Q_zh, Q_wz]);
+# its rows are those slices one after the other.  For the exchange every slice is padded to ceil(Q_i / world) rows, so all
+# ranks send buffers of per_rank_rows(sizes, world) rows.
+def plane_slices(sizes, rank, world):
+    """[(begin, count)] of this rank in each plane."""
+    return [ray_slice(n, world, rank) for n in sizes]
+
+
+def per_rank_rows(sizes, world):
+    return sum(-(-n // world) for n in sizes)
+
+
+def local_rows(full, sizes, rank, world):
+    """This rank's rows out of a [sum(sizes), ...] tensor laid out plane after plane."""
+    return local_rows_of(full, sizes, plane_slices(sizes, rank, world))
+
+
+def local_rows_of(full, sizes, slices):
+    """The rows slices [(begin, count)] per plane out of a [sum(sizes), ...] tensor laid out plane after plane."""
+    parts, off = [], 0
+    for (b, c), n in zip(slices, sizes):
+        parts.append(full[off + b:off + b + c])
+        off += n
+    return torch.cat(parts, 0)
+
+
+def pad_rows(local, sizes, rank, world):
+    """local rows -> [per_rank_rows, C] with each plane's slice padded to ceil(Q_i / world) rows (zeros)."""
+    buf = local.new_zeros(per_rank_rows(sizes, world), local.shape[1])
+    o_src = o_dst = 0
+    for (b, c), n in zip(plane_slices(sizes, rank, world), sizes):
+        buf[o_dst:o_dst + c] = local[o_src:o_src + c]
+        o_src += c
+        o_dst += -(-n // world)
+    return buf
+
+
+def unpad_rows(buf, sizes, rank, world):
+    """The inverse of pad_rows: [per_rank_rows, C] -> this rank's rows (padding dropped)."""
+    parts, off = [], 0
+    for (b, c), n in zip(plane_slices(sizes, rank, world), sizes):
+        parts.append(buf[off:off + c])
+        off += -(-n // world)
+    return torch.cat(parts, 0)
+
+
+def assemble_rows(gathered, sizes, world):
+    """Every rank's padded rows [world, per_rank_rows, C] -> the full planes [sum(sizes), C]."""
+    C = gathered.shape[-1]
+    out = gathered.new_empty(sum(sizes), C)
+    o_dst = o_src = 0
+    for n in sizes:
+        per = -(-n // world)
+        out[o_dst:o_dst + n] = gathered[:, o_src:o_src + per].reshape(world * per, C)[:n]
+        o_dst += n
+        o_src += per
+    return out
+
+
+def split_rows(full, sizes, world):
+    """The inverse of assemble_rows: [sum(sizes), C] -> [world, per_rank_rows, C], rank r's padded rows in block r."""
+    C = full.shape[-1]
+    out = full.new_zeros(world, per_rank_rows(sizes, world), C)
+    o_src = o_dst = 0
+    for n in sizes:
+        per = -(-n // world)
+        plane = full.new_zeros(world * per, C)
+        plane[:n] = full[o_src:o_src + n]
+        out[:, o_dst:o_dst + per] = plane.view(world, per, C)
+        o_src += n
+        o_dst += per
+    return out
+
+
+class _RowGather(torch.autograd.Function):
+    """forward: this rank's plane rows -> the full planes (one all_gather); backward: this rank's rows of the gradient summed
+    over the ranks (one reduce-scatter).  See all_gather_rows."""
+
+    @staticmethod
+    def forward(ctx, spec, local):
+        sizes, rank, world, collective, reduce_scatter = spec
+        buf = pad_rows(local, sizes, rank, world)
+        out = buf.new_empty(world * buf.shape[0], buf.shape[1])
+        collective(out, buf)
+        ctx.spec = spec
+        return assemble_rows(out.view(world, buf.shape[0], buf.shape[1]), sizes, world)
+
+    @staticmethod
+    @torch.autograd.function.once_differentiable
+    def backward(ctx, grad):
+        sizes, rank, world, collective, reduce_scatter = ctx.spec
+        buf = split_rows(grad.contiguous(), sizes, world)
+        out = buf.new_empty(buf.shape[1], buf.shape[2])
+        reduce_scatter(out, buf.view(-1, buf.shape[2]))
+        return None, unpad_rows(out, sizes, rank, world)
+
+
+def all_gather_rows(local, sizes, rank, world, collective=None, reduce_scatter=None, group=None):
+    """The exchange of the query-sharded encoder, differentiable: this rank's rows [sum(count_i), C] (each plane's slice
+    plane_slices(sizes, rank, world), plane after plane) -> the full planes [sum(sizes), C] on every rank.
+
+    Forward: ONE all_gather of the padded slices (pad_rows / assemble_rows).  Backward: ONE reduce-scatter (SUM) of the
+    padded incoming gradient (split_rows), whose block for this rank, padding dropped, is the gradient of its rows.
+    ``collective(out, buf)`` fills ``out`` [world * rows, C] with every rank's ``buf`` [rows, C] in rank order;
+    ``reduce_scatter(out, buf)`` fills ``out`` [rows, C] with the sum over the ranks of block ``rank`` of their ``buf``
+    [world * rows, C].  Defaults: dist.all_gather_into_tensor / dist.reduce_scatter_tensor over ``group``.
+
+    Gradient rule: every rank's head and loss give a gradient with respect to the full planes -- partial and already scaled
+    by world under head.ray_shard (all_gather_ray_payload), full and unscaled for replicated terms (the sparsity term on
+    uniform_sdf).  Either way the sum over the ranks is world x the full gradient, so the reduce-scatter hands rank r
+    world x the full gradient at its rows, and the layers below give parameter gradients that are world x rank r's share.
+    Everything a rank computes whole (layer 0's input planes, the self-attention value_proj over all rows, the image
+    value_projs, the positional-embedding Linear, the image features) receives a partial gradient from that rank's rows,
+    and by linearity these too sum to world x the full gradient.  DistributedDataParallel's mean over the ranks is then
+    the full gradient, with no extra factor."""
+    if collective is None:
+        def collective(out, buf):
+            dist.all_gather_into_tensor(out, buf, group=group)
+    if reduce_scatter is None:
+        def reduce_scatter(out, buf):
+            dist.reduce_scatter_tensor(out, buf, op=dist.ReduceOp.SUM, group=group)
+    sizes = [int(n) for n in sizes]
+    n_local = sum(c for _, c in plane_slices(sizes, rank, world))
+    if local.dim() != 2 or local.shape[0] != n_local:
+        raise ValueError('all_gather_rows: rank %d of %d holds %d rows of planes %s, got %s'
+                         % (rank, world, n_local, sizes, tuple(local.shape)))
+    return _RowGather.apply((sizes, rank, world, collective, reduce_scatter), local.contiguous())
+
+
 def _num_cams(head, metas):
     """Number of cameras the head will render, read from the metas' SHAPES (no copy: usable inside CUDA-graph capture)."""
     import os
@@ -201,18 +331,14 @@ class ShardedLifter:
     # ---- slices
     def slices(self, rank, world):
         """[(begin, count)] of this rank in each plane."""
-        return [ray_slice(n, world, rank) for n in self.sizes]
+        return plane_slices(self.sizes, rank, world)
 
     def per_rank_rows(self, world):
-        return sum(-(-n // world) for n in self.sizes)
+        return per_rank_rows(self.sizes, world)
 
     def _local_rows(self, full, rank, world):
         """rows of this rank out of a [Q_total, ...] tensor laid out hw | zh | wz."""
-        parts, off = [], 0
-        for (b, c), n in zip(self.slices(rank, world), self.sizes):
-            parts.append(full[off + b:off + b + c])
-            off += n
-        return torch.cat(parts, 0)
+        return local_rows(full, self.sizes, rank, world)
 
     # ---- per-frame replicated state
     @torch.no_grad()
@@ -239,26 +365,11 @@ class ShardedLifter:
     # ---- exchange
     def pad_local(self, local, rank, world):
         """local rows -> [per_rank_rows, C] with each plane's slice padded to ceil(Q_i / world) (all_gather needs equal sizes)."""
-        C = local.shape[1]
-        buf = local.new_zeros(self.per_rank_rows(world), C)
-        o_src = o_dst = 0
-        for (b, c), n in zip(self.slices(rank, world), self.sizes):
-            buf[o_dst:o_dst + c] = local[o_src:o_src + c]
-            o_src += c
-            o_dst += -(-n // world)
-        return buf
+        return pad_rows(local, self.sizes, rank, world)
 
     def assemble(self, gathered, world):
         """gathered [world, per_rank_rows, C] -> qfull [Q_total, C]."""
-        C = gathered.shape[-1]
-        out = gathered.new_empty(sum(self.sizes), C)
-        o_dst = o_src = 0
-        for n in self.sizes:
-            per = -(-n // world)
-            out[o_dst:o_dst + n] = gathered[:, o_src:o_src + per].reshape(world * per, C)[:n]
-            o_dst += n
-            o_src += per
-        return out
+        return assemble_rows(gathered, self.sizes, world)
 
     @torch.no_grad()
     def forward(self, representation, ms_img_feats, metas, group=None):

@@ -15,6 +15,8 @@ The arithmetic of the hot ops runs in ``libselfocc_b200.so``:
   (``ops.TPVSelfAttnFunction`` / ``ops.TPVCrossAttnFunction``: no host sync, no padded rebatch, no
   sampling-location tensor); the projections run forward and input gradient on the wgmma GEMM
   (``train_linear``), the weight gradients on cuBLAS;
+* query-sharded training (``TPVFormerEncoder.query_shard = (rank, world)``): the same training kernels on the rank's rows
+  of each plane (``TPVFormerLayer.forward_rows_train``), one ``dist.all_gather_rows`` per layer;
 * batch > 1 or a ``key_padding_mask``: the reference's formulation, the mmcv-contract op
   ``ops.MultiScaleDeformableAttnFunction`` fed by torch softmax / location arithmetic, with the image
   cross-attention's rebatch built from device-compacted index lists (``ops.visible_index_lists``).
@@ -635,6 +637,66 @@ class TPVFormerLayer(nn.Module):
         h = fast_linear(ffn.layers[0][0], x, relu=True)
         return fast_linear(ffn.layers[1], h, residual=x if ffn.add_identity else None, ln=self.norms[2])[0]
 
+    def forward_rows_train(self, q, q_full, pos, ref, slices, value, spatial_shapes, level_start_index, tpv_levels, uvs, vises):
+        """The layer's training forward (autograd, bs = 1, POST_NORM_ORDER, CUDA fp32) on a set of token rows: the twin of
+        forward_rows for the query-sharded training step (TPVFormerEncoder.query_shard), on the kernels of the module
+        forwards' training path (ops.TPVSelfAttnFunction, ops.TPVCrossAttnFunction, train_linear, nn.LayerNorm).  Arguments
+        as forward_rows; q_full must be the autograd-connected full planes.  Every row is computed as the unsharded training
+        forward computes it.  Each dropout draws its mask for the WHOLE tensor the unsharded forward drops out (same shape,
+        same order) and applies this set of rows' part of it (_row_dropout), so every rank advances the torch RNG exactly
+        as the unsharded forward does and a sharded step has one well-defined mask."""
+        from .dist import local_rows_of
+        sa, ca, ffn = self.attentions[0], self.attentions[1], self.ffns[0]
+        sizes = [v.shape[1] for v in vises]
+        Q, C = q_full.shape
+        n = q.shape[0]
+        rows = lambda full: local_rows_of(full, sizes, slices)
+        # self-attention: value = all tokens, queries = these rows (+ pos); the residual is the rows without pos
+        Hd, L, P = sa.num_heads, sa.num_levels, sa.num_points
+        v = train_linear(sa.value_proj, q_full).view(Q, Hd, -1)
+        qp = q + pos
+        offs = train_linear(sa.sampling_offsets, qp).view(n, Hd, L, P, 2)
+        logits = train_linear(sa.attention_weights, qp).view(n, Hd, L, P)
+        out = ops.TPVSelfAttnFunction.apply(v, tpv_levels[0], tpv_levels[1], offs, logits, ref)
+        out = train_linear(sa.output_proj, out)
+        q = self.norms[0](_row_dropout(sa.dropout, out, (Q, out.shape[1]), rows) + q)
+        # image cross-attention, one plane at a time, each on its own rows of q
+        n_cam, nv = value.shape[0], value.shape[1]
+        feat = value[:, :, 0]
+        parts, o0 = [], 0
+        for i, (b, c) in enumerate(slices):
+            att = ca.attns[i]
+            da = att.deformable_attention
+            qi = q[o0:o0 + c]
+            v = train_linear(da.value_proj, feat).view(n_cam, nv, da.num_heads, -1)
+            offs = train_linear(da.sampling_offsets, qi).view(c, da.num_heads, da.num_levels, da.num_points, 2)
+            logits = train_linear(da.attention_weights, qi).view(c, da.num_heads, da.num_levels, da.num_points)
+            slots = ops.TPVCrossAttnFunction.apply(v, spatial_shapes, level_start_index, offs, logits, uvs[i][:, 0, b:b + c],
+                                                   vises[i][:, b:b + c])
+            slots = train_linear(att.output_proj, slots)
+            parts.append(_row_dropout(att.dropout, slots, (sizes[i], slots.shape[1]), lambda m, b=b, c=c: m[b:b + c]) + qi)
+            o0 += c
+        q = self.norms[1](torch.cat(parts, 0))
+        # FFN (mmcv FFN: Linear, ReLU, Dropout, Linear, Dropout, + identity)
+        l0 = ffn.layers[0]
+        h = F.relu(train_linear(l0[0], q))
+        h = _row_dropout(l0[2], h, (Q, h.shape[1]), rows)
+        out = _row_dropout(ffn.layers[2], train_linear(ffn.layers[1], h), (Q, C), rows)
+        return self.norms[2](q + out if ffn.add_identity else out)
+
+
+def _row_dropout(drop, x, full_shape, rows):
+    """nn.Dropout ``drop`` on the rows ``x`` of a tensor of shape ``full_shape``.  The mask is drawn for the whole tensor
+    with the op the unsharded forward runs (nn.Dropout on a CUDA tensor is aten.native_dropout), and ``rows(mask)`` picks
+    the part that belongs to ``x``; x * scale * mask is what native_dropout computes."""
+    p = drop.p
+    if not drop.training or p == 0:
+        return x
+    if p == 1:
+        return x * 0
+    mask = torch.ops.aten.native_dropout(torch.empty(full_shape, device=x.device, dtype=x.dtype), p, True)[1]
+    return x * (rows(mask) * (1.0 / (1.0 - p)))
+
 
 @MODELS.register_module()
 class TPVFormerEncoder(nn.Module):
@@ -676,6 +738,10 @@ class TPVFormerEncoder(nn.Module):
         self.register_buffer('cross_view_ref_points', _cross_view_refs(H, W, Z, num_points_self[0]), False)
         self.register_buffer('tpv_spatial_shapes', torch.tensor([[H, W], [Z, H], [W, Z]], dtype=torch.int64), False)
         self.register_buffer('tpv_level_start', torch.tensor([0, H * W, H * W + Z * H], dtype=torch.int64), False)
+        # query-sharded training (forward_query_sharded): (rank, world) of this process, and the process group of the
+        # exchange (None: the default group)
+        self.query_shard = None
+        self.query_shard_group = None
 
     def init_weights(self):
         """tpvformer_encoder.py:174-190."""
@@ -772,7 +838,55 @@ class TPVFormerEncoder(nn.Module):
             tpv_pos = [p.unsqueeze(0).repeat(bs, 1, 1) if bs > 1 else p.unsqueeze(0) for p in pos]
         return (tpv_pos,) + self.flatten_features(ms_img_feats)
 
+    # ---- query-sharded training (query_shard = (rank, world)): each rank runs every layer on its own rows of each plane
+    def shard_state(self, ms_img_feats, metas):
+        """The per-frame inputs every rank of a query-sharded training step computes whole (under autograd): positional
+        embeddings [Q_total, C], flattened image features with their level tables, camera projections of every plane."""
+        tpv_pos, feat, shapes, lsi = self.frame_inputs(ms_img_feats)
+        pos = torch.cat([p[0] for p in tpv_pos], 0) if isinstance(tpv_pos, (list, tuple)) else tpv_pos[0]
+        uvs, _, vises = self.project_reference_points(metas, feat.device)
+        return dict(pos=pos, feat=feat, shapes=shapes, lsi=lsi, uvs=uvs, vises=vises)
+
+    def shard_layer(self, li, qfull, st, rank, world):
+        """Layer li of the query-sharded training step: the full planes qfull [Q_total, C] (autograd-connected) -> this
+        rank's updated rows (dist.plane_slices of each plane, plane after plane)."""
+        from .dist import local_rows, plane_slices
+        H, W, Z = self.tpv_size
+        sizes = [H * W, Z * H, W * Z]
+        rows = lambda t: local_rows(t, sizes, rank, world)
+        return self.layers[li].forward_rows_train(
+            rows(qfull), qfull, rows(st['pos']), rows(self.cross_view_ref_points), plane_slices(sizes, rank, world), st['feat'],
+            st['shapes'], st['lsi'], (self.tpv_spatial_shapes, self.tpv_level_start), st['uvs'], st['vises'])
+
+    def forward_query_sharded(self, representation, ms_img_feats, metas, rank, world, collective=None, reduce_scatter=None,
+                              group=None):
+        """The encoder's training forward with the queries sharded over ``world`` ranks: the shared set-up (shard_state),
+        then per layer this rank's rows (shard_layer) and ONE dist.all_gather_rows that rebuilds the planes (its backward
+        is one reduce-scatter).  Returns the full planes [1, Q_i, C] x 3 on every rank; the rows equal the unsharded
+        training forward's.  ``collective`` / ``reduce_scatter`` / ``group``: as dist.all_gather_rows."""
+        from .dist import all_gather_rows
+        H, W, Z = self.tpv_size
+        sizes = [H * W, Z * H, W * Z]
+        if min(sizes) < world:
+            raise ValueError('query_shard: a plane of %s rows cannot be split over %d ranks (a rank without rows would leave '
+                             'parameters without a gradient)' % (sizes, world))
+        if representation[0].shape[0] != 1 or not _cuda_fp32(representation[0], ms_img_feats[0]):
+            raise NotImplementedError('query_shard: batch 1, CUDA fp32 only')
+        for layer in self.layers:
+            if tuple(layer.operation_order) != POST_NORM_ORDER or not layer.batch_first:
+                raise NotImplementedError('query_shard: operation_order %r' % (layer.operation_order,))
+        st = self.shard_state(ms_img_feats, metas)
+        qfull = torch.cat([p[0] for p in representation], 0)
+        for li in range(len(self.layers)):
+            local = self.shard_layer(li, qfull, st, rank, world)
+            qfull = all_gather_rows(local, sizes, rank, world, collective, reduce_scatter, group)
+        return [t[None] for t in torch.split(qfull, sizes, 0)]
+
     def forward(self, representation, ms_img_feats=None, metas=None, **kwargs):
+        shard = getattr(self, 'query_shard', None)
+        if shard is not None and shard[1] > 1 and self.training and torch.is_grad_enabled():
+            return {'representation': self.forward_query_sharded(representation, ms_img_feats, metas, shard[0], shard[1],
+                                                                 group=getattr(self, 'query_shard_group', None))}
         tpv_pos, feat_flatten, spatial_shapes, level_start_index = self.frame_inputs(ms_img_feats)
         tpv_embed = self.forward_layers(representation, feat_flatten, feat_flatten, tpv_pos=tpv_pos,
                                         spatial_shapes=spatial_shapes, level_start_index=level_start_index, img_metas=metas)
