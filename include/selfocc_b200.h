@@ -81,8 +81,9 @@ typedef struct so_volume_desc {
  *     f[h,w,z,:] = hw[h,w,:] + zh[z,h,:] + wz[w,z,:]
  *     out        = W2 * softplus(W1 * softplus(f) + b1) + b2          (C -> C -> 1 + n_feat)
  * tpv_hw [H*W, C], tpv_zh [Z*H, C], tpv_wz [W*Z, C]; w1 [C, C], b1 [C], w2 [1+n_feat, C], b2.
- * Outputs: vol_sdf [H, W, zpitch] (channel 0; pad entries zeroed), vol_feat [H, W, Z, feat_pitch]
- * (channels 1.., may be NULL when n_feat == 0).  C must be a multiple of 32, C <= 128.
+ * Outputs: vol_sdf [H, W, zpitch] (channel 0; pad entries z in [Z, zpitch) written as 0), vol_feat [H, W, Z, feat_pitch]
+ * (channels 1.., may be NULL when n_feat == 0; the pad channels [n_feat, feat_pitch) are never written: a caller that reads
+ * them clears the buffer first).  C is 32, 64, 96 or 128 and 1 + n_feat <= 32, else SO_ERR_UNSUPPORTED before any launch.
  */
 int so_tpv_decode(const float* tpv_hw, const float* tpv_zh, const float* tpv_wz, int32_t C,
                   const float* w1, const float* b1, const float* w2, const float* b2,
@@ -100,7 +101,10 @@ int so_tpv_decode_rows(const float* tpv_hw, const float* tpv_zh, const float* tp
  *   hidden:   z1_a1[rows][C] holds z1 = a0 W1^T + b1 on entry and a1 = softplus(z1) on return;
  *             g1 = (W2^T g_out) * sigmoid(z1); g_out[rows][1 + n_feat] = the slab's output gradient gathered from
  *             g_vol_sdf [H][W][zpitch] (may be NULL = zero) and g_vol_feat [H][W][Z][feat_pitch] (may be NULL = zero)
- *   input:    g0[n] *= 1 - exp(-a0[n])   (= sigmoid of the pre-activation), n % 4 == 0                                   */
+ *   input:    g0[n] *= 1 - exp(-a0[n])   (= sigmoid of the pre-activation), n % 4 == 0
+ * The sdf pads and feature pad channels of g_vol_sdf / g_vol_feat are never read.  softplus and both sigmoid factors are
+ * accurate relative to their own value (1e-5 or better down to a pre-activation of -16 and below), not only absolutely:
+ * a channel whose activations are all small still gets a gradient that is right relative to itself.                      */
 int so_tpv_decode_bwd_features(const float* tpv_hw, const float* tpv_zh, const float* tpv_wz, int32_t C,
                                const so_volume_desc* vol_host, int32_t h_begin, int32_t h_count, float* a0, void* stream);
 int so_tpv_decode_bwd_hidden(float* z1_a1, const float* g_vol_sdf, const float* g_vol_feat, const float* w2, int32_t C,

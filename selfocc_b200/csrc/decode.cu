@@ -17,8 +17,49 @@ constexpr int kThreads = 256;
 constexpr int kMaxOut = 32;
 
 __device__ __forceinline__ float softplus_fast(float x) {
-  // F.softplus(beta=1, threshold=20): max(x,0) + log1p(exp(-|x|)); identical to x beyond the threshold in fp32
+  // F.softplus(beta=1, threshold=20): max(x,0) + log1p(exp(-|x|)); identical to x beyond the threshold in fp32.
+  // Forward kernels only.  1 + e is rounded to fp32 and __logf is accurate to 2^-21.4 absolute, so the ABSOLUTE error stays
+  // below 1e-6 everywhere, which is what the decoded volume needs (every consumer of an activation multiplies it by a
+  // weight and adds it to an O(1) sum), but the error RELATIVE to the value grows as the value shrinks (1e-2 at x = -10).
+  // The backward needs the relative kind (softplus_rel below) and does not share this function.
   return fmaxf(x, 0.f) + __logf(1.0f + __expf(-fabsf(x)));
+}
+
+// log1p(e) for e = exp(-|x|) in [0, 1], accurate relative to its value: 2 atanh(s) with s = e / (2 + e) <= 1/3 by the odd
+// series up to s^11 (next term 1.5e-7 relative at e = 1).  No 1 + e is formed and no logarithm taken, so a small e keeps all
+// its digits; one MUFU.RCP instead of softplus_fast's MUFU.LG2, plus five FMAs.
+__device__ __forceinline__ float log1p_small(float e) {
+  const float s = __fdividef(e, 2.0f + e), t = s * s;
+  float p = fmaf(t, 1.0f / 11.0f, 1.0f / 9.0f);
+  p = fmaf(t, p, 1.0f / 7.0f);
+  p = fmaf(t, p, 1.0f / 5.0f);
+  p = fmaf(t, p, 1.0f / 3.0f);
+  p = fmaf(t, p, 1.0f);
+  return 2.0f * s * p;
+}
+
+// Backward kernels: softplus and the sigmoid factors accurate RELATIVE to their values on the negative side too (a few
+// 1e-7 down to the underflow of exp at x = -87).  A plane channel or hidden unit whose pre-activation sits below about
+// -6 has activations and sigmoid factors of 1e-3 and less; its gradient is a sum of products with exactly those, and
+// Adam divides every gradient by its own running magnitude, so an error relative to the small value is an error of the
+// same size in the update.
+__device__ __forceinline__ float softplus_rel(float x) { return fmaxf(x, 0.f) + log1p_small(__expf(-fabsf(x))); }
+
+// softplus(z) and sigmoid(z) from one exponential: sigmoid = 1 / (1 + e) for z >= 0, e / (1 + e) below
+__device__ __forceinline__ float softplus_sigmoid(float z, float* sig) {
+  const float e = __expf(-fabsf(z)), r = __fdividef(1.0f, 1.0f + e);
+  *sig = z >= 0.f ? r : e * r;
+  return fmaxf(z, 0.f) + log1p_small(e);
+}
+
+// sigmoid(x) from a = softplus(x) alone: 1 - exp(-a).  Below 1/8 the subtraction would cancel (sigmoid ~ a), so -expm1(-a)
+// is taken by its series up to a^5 (next term 4e-8 relative at 1/8); above, the difference keeps 2e-6 relative or better.
+__device__ __forceinline__ float sigmoid_of_softplus(float a) {
+  float p = fmaf(a, 1.0f / 120.0f, -1.0f / 24.0f);
+  p = fmaf(a, p, 1.0f / 6.0f);
+  p = fmaf(a, p, -0.5f);
+  p = fmaf(a, p, 1.0f);
+  return a < 0.125f ? a * p : 1.0f - __expf(-a);
 }
 
 // C = channels (multiple of 32), LD = padded leading dimension (C + 4) in floats
@@ -385,6 +426,7 @@ extern "C" int so_tpv_decode_rows(const float* tpv_hw, const float* tpv_zh, cons
   if (h_count == 0) return SO_OK;
   if (d->n_feat > 0 && !vol_feat) return SO_ERR_INVALID_ARG;
   if (1 + d->n_feat > kMaxOut) return SO_ERR_UNSUPPORTED;
+  if (C != 32 && C != 64 && C != 96 && C != 128) return SO_ERR_UNSUPPORTED;   // before the pad kernel below is launched
   if (d->H > 65535) return SO_ERR_UNSUPPORTED;
   cudaStream_t st = (cudaStream_t)stream;
   if (d->zpitch > d->Z) {
@@ -443,7 +485,9 @@ extern "C" int so_tpv_decode_rows(const float* tpv_hw, const float* tpv_zh, cons
 //   features:  a0 = softplus(hw + zh + wz)                                       (recomputed, never stored by forward)
 //   hidden:    z1 -> a1 = softplus(z1);  g1 = (W2^T g_out) * sigmoid(z1);  g_out packed [rows][n_out]
 //   input:     g0 *= sigmoid(f) = 1 - exp(-a0)
-// sigmoid(x) = 1 - exp(-softplus(x)) lets the activations be reused without keeping the pre-activations.
+// sigmoid(x) = 1 - exp(-softplus(x)) lets the input kernel reuse a0 without keeping the pre-activation; the hidden kernel
+// has z1 in hand and takes its sigmoid from the same exponential as the softplus.  All three use the relative-accuracy
+// forms above (softplus_rel, softplus_sigmoid, sigmoid_of_softplus).
 __global__ void __launch_bounds__(256) decode_bwd_features_kernel(const float* __restrict__ hw, const float* __restrict__ zh,
                                                                   const float* __restrict__ wz, int C4, int H, int W, int Z,
                                                                   int h_begin, long long n_vec, float4* __restrict__ a0) {
@@ -456,8 +500,8 @@ __global__ void __launch_bounds__(256) decode_bwd_features_kernel(const float* _
     float4 a = __ldg(reinterpret_cast<const float4*>(hw + ((size_t)h * W + w) * C4 * 4) + c4);
     float4 b = __ldg(reinterpret_cast<const float4*>(zh + ((size_t)z * H + h) * C4 * 4) + c4);
     float4 c = __ldg(reinterpret_cast<const float4*>(wz + ((size_t)w * Z + z) * C4 * 4) + c4);
-    a0[i] = make_float4(softplus_fast(a.x + b.x + c.x), softplus_fast(a.y + b.y + c.y), softplus_fast(a.z + b.z + c.z),
-                        softplus_fast(a.w + b.w + c.w));
+    a0[i] = make_float4(softplus_rel(a.x + b.x + c.x), softplus_rel(a.y + b.y + c.y), softplus_rel(a.z + b.z + c.z),
+                        softplus_rel(a.w + b.w + c.w));
   }
 }
 
@@ -490,17 +534,19 @@ __global__ void __launch_bounds__(256) decode_bwd_hidden_kernel(float4* __restri
       if (c4 == 0) g_out[v * n_out + o] = g;
     }
     float4 zv = z1_a1[i];
-    float4 a = make_float4(softplus_fast(zv.x), softplus_fast(zv.y), softplus_fast(zv.z), softplus_fast(zv.w));
+    float4 a, sg;
+    a.x = softplus_sigmoid(zv.x, &sg.x); a.y = softplus_sigmoid(zv.y, &sg.y);
+    a.z = softplus_sigmoid(zv.z, &sg.z); a.w = softplus_sigmoid(zv.w, &sg.w);
     z1_a1[i] = a;
-    g1[i] = make_float4(acc.x * (1.f - __expf(-a.x)), acc.y * (1.f - __expf(-a.y)), acc.z * (1.f - __expf(-a.z)),
-                        acc.w * (1.f - __expf(-a.w)));
+    g1[i] = make_float4(acc.x * sg.x, acc.y * sg.y, acc.z * sg.z, acc.w * sg.w);
   }
 }
 
 __global__ void __launch_bounds__(256) decode_bwd_input_kernel(float4* __restrict__ g0, const float4* __restrict__ a0, long long n_vec) {
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n_vec; i += (long long)gridDim.x * blockDim.x) {
     float4 g = g0[i], a = __ldg(a0 + i);
-    g0[i] = make_float4(g.x * (1.f - __expf(-a.x)), g.y * (1.f - __expf(-a.y)), g.z * (1.f - __expf(-a.z)), g.w * (1.f - __expf(-a.w)));
+    g0[i] = make_float4(g.x * sigmoid_of_softplus(a.x), g.y * sigmoid_of_softplus(a.y), g.z * sigmoid_of_softplus(a.z),
+                        g.w * sigmoid_of_softplus(a.w));
   }
 }
 

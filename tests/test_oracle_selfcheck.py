@@ -117,3 +117,42 @@ def test_train_parity_reproduces_itself_and_masks_exactly_the_flip_rays():
     with pytest.raises(AssertionError, match='not zero on a flip ray'):
         tp.train_parity(got, {'vol': gvol, 'inv_s': ginv}, cot, vol, m, o, d, nrm, aabb, 12.0, S, moved, jitter=jitter,
                         color_dims=3, bkgd_rand=bk, chunk=5)
+
+
+def test_slabwise_decode_equals_the_whole_volume_oracle_and_its_autograd():
+    """oracle/decode_parity.py restates tpv_decode_ref slab by slab (ragged last slab, H != W): same volume, same gradients
+    of every plane and MLP tensor, fp64, 1e-12; and its per-slice and per-bucket error reports on planted errors."""
+    from oracle import decode_parity as dp
+    g = torch.Generator().manual_seed(5)
+    H, W, Z, C, n_out = 11, 6, 5, 32, 4
+    planes = [torch.randn(n, C, generator=g, dtype=torch.float64) for n in (H * W, Z * H, W * Z)]
+    mlp = [t.double() for t in synth.random_mlp(C, n_out, seed=5)]
+    cot = torch.randn(H, W, Z, n_out, generator=g, dtype=torch.float64)
+    ins = [t.clone().requires_grad_(True) for t in (*planes, *mlp)]
+    ref = orender.tpv_decode_ref(*ins[:3], (H, W, Z), *ins[3:]).permute(1, 2, 3, 0)       # [H, W, Z, n_out]
+    gref = torch.autograd.grad((ref * cot).sum(), ins)
+    for slab in (3, 4, 11, 32):
+        vol = dp.decode_slabwise(*planes, (H, W, Z), *mlp, slab=slab)
+        assert vol.shape == ref.shape and (vol - ref.detach()).abs().max() < 1e-12
+        grads, b1_mass = dp.decode_grads_slabwise(*planes, (H, W, Z), *mlp, cot, slab=slab)
+        for name, a, b in zip(dp.GRAD_NAMES, grads, gref):
+            assert a.shape == b.shape and (a - b).abs().max() < 1e-12 * max(1.0, b.abs().max().item()), (slab, name)
+        # the un-cancelled sum behind d/d b1: the same gradient with every voxel's term taken positive
+        assert (b1_mass >= gref[4].abs() * (1 - 1e-12)).all() and b1_mass.max() > 3 * gref[4].abs().max()
+    f = dp.preactivation(*planes, (H, W, Z), 2, 5)
+    assert f.shape == (3, W, Z, C)
+    assert f[1, 4, 3, 7] == planes[0].view(H, W, C)[3, 4, 7] + planes[1].view(Z, H, C)[3, 3, 7] + planes[2].view(W, Z, C)[4, 3, 7]
+    # slice_errors: an error planted in one small column is invisible relative to the tensor's max-abs, not to its own slice
+    w = torch.ones(4, 3, dtype=torch.float64)
+    w[:, 1] = 1e-6
+    bad = w.clone()
+    bad[2, 1] = 2e-6
+    assert (bad - w).abs().max() / w.abs().max() < 1e-5
+    assert dp.slice_errors(bad, w, 1).tolist() == [0.0, 1.0, 0.0]
+    assert dp.slice_errors(torch.ones(3, dtype=torch.float64), torch.tensor([2.0, 0.0, 1.0], dtype=torch.float64), 0).tolist() == [0.5, 0.0, 0.0]
+    # bucket_errors: the relative error is taken per element, inside the bucket of its pre-activation
+    pre = torch.tensor([-13.0, -9.0, -9.5, 1.0, 25.0], dtype=torch.float64)
+    val = torch.nn.functional.softplus(pre)
+    rows = dp.bucket_errors(val * torch.tensor([1.5, 1.0, 1.01, 1.0, 1.0], dtype=torch.float64), val, pre)
+    assert [r[0] for r in rows] == [0, 1, 2, 0, 0, 1, 1]
+    assert abs(rows[1][2] - 0.5) < 1e-12 and abs(rows[2][2] - 0.01) < 1e-12 and rows[5][2] == 0 and rows[6][1] == 0
