@@ -11,13 +11,13 @@ The arithmetic of the hot ops runs in ``libselfocc_b200.so``:
   ``ops.tpv_cross_attn_forward_rows``); every dense projection (value / offset / weight / output Linear, FFN) runs on
   the wgmma split-precision GEMM (``ops.linear_3xtf32``, fp32-level accuracy), projections of the same input are
   fused into one GEMM, and each LayerNorm is folded into the epilogue of the GEMM before it;
-* training (autograd), batch 1: the same fused attention cores with their backward kernels
-  (``ops.TPVSelfAttnFunction`` / ``ops.TPVCrossAttnFunction``: no host sync, no padded rebatch, no
-  sampling-location tensor); the projections run forward and input gradient on the wgmma GEMM
-  (``train_linear``), the weight gradients on cuBLAS;
-* query-sharded training (``TPVFormerEncoder.query_shard = (rank, world)``): the same training kernels on the rank's rows
-  of each plane (``TPVFormerLayer.forward_rows_train``), one ``dist.all_gather_rows`` per layer;
-* batch > 1 or a ``key_padding_mask``: the reference's formulation, the mmcv-contract op
+* training (autograd, or train mode), batch 1, post-norm layers: ``TPVFormerLayer.forward_rows_train``, one routine per
+  layer on all rows, or on the rank's rows of each plane in the query-sharded step (``TPVFormerEncoder.query_shard =
+  (rank, world)``, one ``dist.all_gather_rows`` per layer).  The same fused attention cores with their backward kernels
+  (``ops.TPVSelfAttnFunction`` / ``ops.TPVCrossAttnFunction``: no host sync, no padded rebatch, no sampling-location
+  tensor); the projections run forward and input gradient on the wgmma GEMM (``train_linear``), the weight gradients on
+  cuBLAS;
+* batch > 1 or a ``key_padding_mask``: the attention modules' own forwards, the reference's formulation: the mmcv-contract op
   ``ops.MultiScaleDeformableAttnFunction`` fed by torch softmax / location arithmetic, with the image
   cross-attention's rebatch built from device-compacted index lists (``ops.visible_index_lists``).
 """
@@ -189,17 +189,12 @@ def _fast_linear_impl(lin, x, relu, residual, out, ln):
 
 def train_linear(lin, x):
     """nn.Linear inside the autograd (training) path: forward and input gradient on the wgmma 3xTF32 GEMM
-    (ops.TCLinearFunction) when the shape allows it; SELFOCC_B200_TRAIN_LINEAR=cublas keeps the stock nn.Linear."""
+    (ops.TCLinearFunction) when the shape allows it, the stock nn.Linear otherwise."""
     w = lin.weight
     if x.is_cuda and x.dtype == torch.float32 and w.dtype == torch.float32 and x.numel() > 0 \
-            and ops.linear_supported(w.shape[1], w.shape[0]) and _needs_grad(x, w) and not _train_linear_off():
+            and ops.linear_supported(w.shape[1], w.shape[0]) and _needs_grad(x, w):
         return ops.TCLinearFunction.apply(x, w, lin.bias)
     return lin(x)
-
-
-def _train_linear_off():
-    import os
-    return os.environ.get('SELFOCC_B200_TRAIN_LINEAR', 'tc') == 'cublas'
 
 
 def fast_linear_cat(owner, key, lins, x):
@@ -247,7 +242,8 @@ def _cuda_fp32(*tensors):
 class CrossViewHybridAttention(_DeformBase):
     """A8.  cross_view_hybrid_attention.py:11-124 (subclass of mmcv MultiScaleDeformableAttention whose
     only change is the per-point reference broadcast, :96-99).  Parameters: sampling_offsets,
-    attention_weights, value_proj, output_proj."""
+    attention_weights, value_proj, output_proj.  forward is the reference's formulation, for the layers that do not run a
+    row routine (batch > 1, a key_padding_mask); TPVFormerLayer runs this attention's batch-1 arithmetic itself."""
 
     def __init__(self, embed_dims=256, num_heads=8, num_levels=4, num_points=4, im2col_step=64, dropout=0.1,
                  batch_first=False, norm_cfg=None, init_cfg=None, value_proj_ratio=1.0, **kwargs):
@@ -277,16 +273,6 @@ class CrossViewHybridAttention(_DeformBase):
         Hd, L, P = self.num_heads, self.num_levels, self.num_points
         if reference_points.shape[-1] != 2:
             raise ValueError('Last dim of reference_points must be 2, but get %d instead.' % reference_points.shape[-1])
-        if bs == 1 and key_padding_mask is None and _cuda_fp32(query, value):
-            # the fused core with its backward kernel; projections on the autograd GEMM
-            v = train_linear(self.value_proj, value[0]).view(num_value, Hd, -1)
-            offsets = train_linear(self.sampling_offsets, query[0]).view(num_query, Hd, L, P, 2)
-            logits = train_linear(self.attention_weights, query[0]).view(num_query, Hd, L, P)
-            ref = reference_points[0] if reference_points.dim() == 5 else reference_points
-            out = ops.TPVSelfAttnFunction.apply(v, spatial_shapes, level_start_index, offsets, logits, ref)
-            out = train_linear(self.output_proj, out)
-            out = out[None] if self.batch_first else out[:, None]
-            return self.dropout(out) + identity
         value = train_linear(self.value_proj, value)
         if key_padding_mask is not None:
             value = value.masked_fill(key_padding_mask[..., None], 0.0)
@@ -348,9 +334,9 @@ class BEVDeformableAttention(_DeformBase):
 
 @MODELS.register_module()
 class BEVCrossAttention(nn.Module):
-    """A5.  image_cross_attention.py:11-139.  Batch 1 runs the rebatch-free fused core, with autograd through
-    its backward kernel; batch > 1 or a key_padding_mask reproduce the reference's rebatch with
-    device-compacted index lists."""
+    """A5.  image_cross_attention.py:11-139.  forward reproduces the reference's rebatch with device-compacted index
+    lists, for the layers that do not run a row routine (batch > 1, a key_padding_mask); TPVFormerLayer runs this
+    attention's batch-1 arithmetic itself, on the rebatch-free fused core."""
 
     def __init__(self, embed_dims=256, num_cams=6, dropout=0.1, init_cfg=None, batch_first=True,
                  deformable_attention=dict(type='BEVDeformableAttention', embed_dims=256, num_levels=4), **kwargs):
@@ -366,31 +352,16 @@ class BEVCrossAttention(nn.Module):
         nn.init.constant_(self.output_proj.bias, 0.)
 
     def forward(self, query, key, value, residual=None, spatial_shapes=None, reference_points_cams=None,
-                bev_masks=None, level_start_index=None, bev_vis=None, **kwargs):
+                bev_masks=None, level_start_index=None, **kwargs):
         """query [B,Q,C]; key/value [N, sum(hw), B, C]; reference_points_cams [N,B,Q,D,2];
-        bev_masks [N,B,Q,D] (bool/uint8); bev_vis optional uint8 [N,Q] = any_D(mask) from so_point_sampling."""
+        bev_masks [N,B,Q,D] (bool/uint8)."""
         if key is None:
             key = query
         if value is None:
             value = key
         if residual is None:
             residual = query
-        bs, num_query, C = query.shape
-        da = self.deformable_attention
-        Hd, L, D = da.num_heads, da.num_levels, da.num_points
-        assert reference_points_cams.size(3) == D
-        if bs == 1 and kwargs.get('key_padding_mask') is None and _cuda_fp32(query, value):
-            # the rebatch-free core with its backward kernel (no host sync, no padded per-camera copies)
-            n_cam, nv = value.shape[0], value.shape[1]
-            if bev_vis is None:
-                bev_vis = (bev_masks[:, 0].sum(-1) > 0).to(torch.uint8)
-            v = train_linear(da.value_proj, value[:, :, 0]).view(n_cam, nv, Hd, -1)
-            offsets = train_linear(da.sampling_offsets, query[0]).view(num_query, Hd, L, D, 2)
-            logits = train_linear(da.attention_weights, query[0]).view(num_query, Hd, L, D)
-            slots = ops.TPVCrossAttnFunction.apply(v, spatial_shapes, level_start_index, offsets, logits,
-                                                   reference_points_cams[:, 0], bev_vis)
-            slots = train_linear(self.output_proj, slots)
-            return self.dropout(slots)[None] + residual
+        assert reference_points_cams.size(3) == self.deformable_attention.num_points
         slots = self._rebatch_forward(query, value, spatial_shapes, reference_points_cams, bev_masks, level_start_index)
         slots = train_linear(self.output_proj, slots)
         return self.dropout(slots) + residual
@@ -439,11 +410,10 @@ class TPVCrossAttention(nn.Module):
         self.attns = [self.attn_hw, self.attn_zh, self.attn_wz]
 
     def forward(self, query, key, value, residual=None, spatial_shapes=None, reference_points_cams=None, tpv_masks=None,
-                level_start_index=None, tpv_vis=None, **kwargs):
+                level_start_index=None, **kwargs):
         return [self.attns[i](query[i], key, value, residual[i] if residual is not None else None,
                               spatial_shapes=spatial_shapes, level_start_index=level_start_index,
-                              reference_points_cams=reference_points_cams[i], bev_masks=tpv_masks[i],
-                              bev_vis=None if tpv_vis is None else tpv_vis[i])
+                              reference_points_cams=reference_points_cams[i], bev_masks=tpv_masks[i])
                 for i in range(3)]
 
 
@@ -543,57 +513,56 @@ class TPVFormerLayer(nn.Module):
             ss = torch.tensor([[H, W], [Z, H], [W, Z]], device=dev)
             tpv_levels = (ss, torch.tensor([0, H * W, H * W + Z * H], device=dev))
         pos_cat = torch.cat(tpv_pos, dim=1) if isinstance(tpv_pos, (list, tuple)) else tpv_pos
-        # `qc` is the concatenated [B, Q_hw + Q_zh + Q_wz, C] token buffer; `query` are its per-plane views.  Keeping both
-        # avoids the reference's torch.cat before every self-attention / norm / ffn step (5 x 31 MB copies per layer).
-        qc = _whole(query, split)
-        if self._takes_rows(query[0], kwargs):
+        routine = self._row_routine(query[0], value, kwargs)
+        if routine is not None:
             if tpv_vis is None:
                 tpv_vis = [(m[:, 0].sum(-1) > 0).to(torch.uint8) for m in tpv_masks]
+            # the previous layer's output is torch.split views of one token buffer: take it whole, no 31 MB torch.cat
+            qc = _whole(query, split)
             q = (qc if qc is not None else torch.cat(query, dim=1))[0]
-            out = self.forward_rows(q, q, pos_cat[0], ref_2d[0] if ref_2d.dim() == 5 else ref_2d, [(0, n) for n in split], value,
-                                    spatial_shapes, level_start_index, tpv_levels, reference_points_cams, tpv_vis)
+            out = routine(q, q, pos_cat[0], ref_2d[0] if ref_2d.dim() == 5 else ref_2d, [(0, n) for n in split], value,
+                          spatial_shapes, level_start_index, tpv_levels, reference_points_cams, tpv_vis)
             return torch.split(out[None], split, 1)
         norm_i = attn_i = ffn_i = 0
         identity = query
-        cat = lambda views, whole: whole if whole is not None else torch.cat(views, dim=1)
         for op in self.operation_order:
             if op == 'self_attn':
-                q = cat(query, qc)
+                q = torch.cat(query, dim=1)
                 idt = (q if identity is query else torch.cat(identity, dim=1)) if self.pre_norm else None
-                qc = self.attentions[attn_i](q, q, q, idt, query_pos=pos_cat, reference_points=ref_2d,
-                                             spatial_shapes=tpv_levels[0], level_start_index=tpv_levels[1], **kwargs)
-                query = torch.split(qc, split, 1)
+                query = torch.split(self.attentions[attn_i](q, q, q, idt, query_pos=pos_cat, reference_points=ref_2d,
+                                                            spatial_shapes=tpv_levels[0], level_start_index=tpv_levels[1],
+                                                            **kwargs), split, 1)
                 attn_i += 1
                 identity = query
             elif op == 'norm':
-                q = cat(query, qc)
+                q = torch.cat(query, dim=1)
                 ln = self.norms[norm_i]
                 if q.is_cuda and q.dtype == torch.float32 and q.shape[-1] <= 256 and not _needs_grad(q, ln.weight):
-                    qc = ops.layer_norm(q.contiguous(), ln.weight.detach(), ln.bias.detach(), ln.eps)
+                    q = ops.layer_norm(q.contiguous(), ln.weight.detach(), ln.bias.detach(), ln.eps)
                 else:
-                    qc = ln(q)
-                query = torch.split(qc, split, 1)
+                    q = ln(q)
+                query = torch.split(q, split, 1)
                 norm_i += 1
             elif op == 'cross_attn':
                 query = self.attentions[attn_i](query, key, value, identity if self.pre_norm else None,
                                                 spatial_shapes=spatial_shapes, level_start_index=level_start_index,
-                                                reference_points_cams=reference_points_cams, tpv_masks=tpv_masks,
-                                                tpv_vis=tpv_vis, **kwargs)
-                qc = None
+                                                reference_points_cams=reference_points_cams, tpv_masks=tpv_masks, **kwargs)
                 attn_i += 1
                 identity = query
             elif op == 'ffn':
-                q = cat(query, qc)
+                q = torch.cat(query, dim=1)
                 idt = (q if identity is query else torch.cat(identity, dim=1)) if self.pre_norm else None
-                qc = self.ffns[ffn_i](q, idt)
-                query = torch.split(qc, split, 1)
+                query = torch.split(self.ffns[ffn_i](q, idt), split, 1)
                 ffn_i += 1
         return query
 
-    def _takes_rows(self, q, kwargs):
-        """Whether forward runs as forward_rows: inference at batch 1 in CUDA fp32, batch_first, post-norm order, no mask."""
-        return not self.training and not torch.is_grad_enabled() and q.shape[0] == 1 and _cuda_fp32(q) and self.batch_first \
-            and tuple(self.operation_order) == POST_NORM_ORDER and kwargs.get('key_padding_mask') is None
+    def _row_routine(self, q, value, kwargs):
+        """The routine forward runs on all rows at batch 1 in CUDA fp32, batch_first, post-norm order, no mask:
+        forward_rows for inference (eval, no autograd), forward_rows_train otherwise.  None: the op-order loop."""
+        if q.shape[0] != 1 or not _cuda_fp32(q, value) or not self.batch_first \
+                or tuple(self.operation_order) != POST_NORM_ORDER or kwargs.get('key_padding_mask') is not None:
+            return None
+        return self.forward_rows if not self.training and not torch.is_grad_enabled() else self.forward_rows_train
 
     def forward_rows(self, q, q_full, pos, ref, slices, value, spatial_shapes, level_start_index, tpv_levels, uvs, vises):
         """The layer's inference (eval, no autograd, bs = 1, POST_NORM_ORDER) on a set of token rows.
@@ -638,13 +607,14 @@ class TPVFormerLayer(nn.Module):
         return fast_linear(ffn.layers[1], h, residual=x if ffn.add_identity else None, ln=self.norms[2])[0]
 
     def forward_rows_train(self, q, q_full, pos, ref, slices, value, spatial_shapes, level_start_index, tpv_levels, uvs, vises):
-        """The layer's training forward (autograd, bs = 1, POST_NORM_ORDER, CUDA fp32) on a set of token rows: the twin of
-        forward_rows for the query-sharded training step (TPVFormerEncoder.query_shard), on the kernels of the module
-        forwards' training path (ops.TPVSelfAttnFunction, ops.TPVCrossAttnFunction, train_linear, nn.LayerNorm).  Arguments
-        as forward_rows; q_full must be the autograd-connected full planes.  Every row is computed as the unsharded training
-        forward computes it.  Each dropout draws its mask for the WHOLE tensor the unsharded forward drops out (same shape,
-        same order) and applies this set of rows' part of it (_row_dropout), so every rank advances the torch RNG exactly
-        as the unsharded forward does and a sharded step has one well-defined mask."""
+        """The layer's training forward (autograd or train mode, bs = 1, POST_NORM_ORDER, CUDA fp32) on a set of token rows,
+        the autograd twin of forward_rows: all rows for forward, a rank's rows for the query-sharded training step
+        (TPVFormerEncoder.query_shard).  The fused attention cores with their backward kernels (ops.TPVSelfAttnFunction,
+        ops.TPVCrossAttnFunction), train_linear, nn.LayerNorm.  Arguments as forward_rows; q_full must be the
+        autograd-connected full planes.  Any split of the rows computes every row as the call on all rows does.  Each
+        dropout draws its mask for the WHOLE tensor (same shape, same order) and applies this set of rows' part of it
+        (_row_dropout), so every rank advances the torch RNG exactly as the call on all rows does and a sharded step has
+        one well-defined mask."""
         from .dist import local_rows_of
         sa, ca, ffn = self.attentions[0], self.attentions[1], self.ffns[0]
         sizes = [v.shape[1] for v in vises]
@@ -658,8 +628,9 @@ class TPVFormerLayer(nn.Module):
         offs = train_linear(sa.sampling_offsets, qp).view(n, Hd, L, P, 2)
         logits = train_linear(sa.attention_weights, qp).view(n, Hd, L, P)
         out = ops.TPVSelfAttnFunction.apply(v, tpv_levels[0], tpv_levels[1], offs, logits, ref)
-        out = train_linear(sa.output_proj, out)
-        q = self.norms[0](_row_dropout(sa.dropout, out, (Q, out.shape[1]), rows) + q)
+        # no name holds a [rows, C] tensor that backward does not keep (a projection before its dropout, a dropout before its
+        # residual): the forward's peak is what backward saves plus one step's temporaries
+        q = self.norms[0](_row_dropout(sa.dropout, train_linear(sa.output_proj, out), (Q, C), rows) + q)
         # image cross-attention, one plane at a time, each on its own rows of q
         n_cam, nv = value.shape[0], value.shape[1]
         feat = value[:, :, 0]
@@ -673,8 +644,8 @@ class TPVFormerLayer(nn.Module):
             logits = train_linear(da.attention_weights, qi).view(c, da.num_heads, da.num_levels, da.num_points)
             slots = ops.TPVCrossAttnFunction.apply(v, spatial_shapes, level_start_index, offs, logits, uvs[i][:, 0, b:b + c],
                                                    vises[i][:, b:b + c])
-            slots = train_linear(att.output_proj, slots)
-            parts.append(_row_dropout(att.dropout, slots, (sizes[i], slots.shape[1]), lambda m, b=b, c=c: m[b:b + c]) + qi)
+            parts.append(_row_dropout(att.dropout, train_linear(att.output_proj, slots), (sizes[i], C),
+                                      lambda m, b=b, c=c: m[b:b + c]) + qi)
             o0 += c
         q = self.norms[1](torch.cat(parts, 0))
         # FFN (mmcv FFN: Linear, ReLU, Dropout, Linear, Dropout, + identity)
@@ -682,13 +653,20 @@ class TPVFormerLayer(nn.Module):
         h = F.relu(train_linear(l0[0], q))
         h = _row_dropout(l0[2], h, (Q, h.shape[1]), rows)
         out = _row_dropout(ffn.layers[2], train_linear(ffn.layers[1], h), (Q, C), rows)
-        return self.norms[2](q + out if ffn.add_identity else out)
+        if ffn.add_identity:
+            out = q + out
+        # normed as [1, n, C]: the layer's forward returns torch.split views of this one token buffer, which the next layer
+        # takes whole (`_whole`) instead of concatenating the planes again
+        return self.norms[2](out[None])[0]
 
 
 def _row_dropout(drop, x, full_shape, rows):
-    """nn.Dropout ``drop`` on the rows ``x`` of a tensor of shape ``full_shape``.  The mask is drawn for the whole tensor
-    with the op the unsharded forward runs (nn.Dropout on a CUDA tensor is aten.native_dropout), and ``rows(mask)`` picks
-    the part that belongs to ``x``; x * scale * mask is what native_dropout computes."""
+    """nn.Dropout ``drop`` on the rows ``x`` of a tensor of shape ``full_shape``.  When ``x`` is the whole tensor this is
+    ``drop(x)``.  Otherwise the mask is drawn for the whole tensor with the op nn.Dropout runs on a CUDA tensor
+    (aten.native_dropout), so the RNG advances as for the whole tensor, and ``rows(mask)`` picks the part that belongs to
+    ``x``; x * scale * mask is what native_dropout computes."""
+    if tuple(x.shape) == tuple(full_shape):
+        return drop(x)
     p = drop.p
     if not drop.training or p == 0:
         return x

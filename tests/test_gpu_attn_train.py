@@ -1,6 +1,7 @@
 """Training through the fused attention cores: the backward kernels (so_tpv_cross_attn_backward / so_tpv_self_attn_backward)
-against fp64 autograd of the oracle, their determinism, the attention modules' training path against the fp64 oracle
-modules, the full-size cores against the reference-contract composition, and the training step's freedom from host syncs.
+against fp64 autograd of the oracle, their determinism, the encoder layer's training routine (forward_rows_train) and the
+attention modules' reference formulation (the MSDA op's backward) against the fp64 oracle, which path a training forward
+takes, the full-size cores against the reference-contract composition, and the training step's freedom from host syncs.
 The C-ABI argument checks run without a GPU."""
 import importlib.util
 import os
@@ -249,8 +250,7 @@ def test_image_cross_attention_training_matches_fp64_oracle():
     qd = [q.to(dev).requires_grad_(True) for q in queries]
     fd = feat.to(dev).requires_grad_(True)
     ss, lsi = _levels(shapes, dev)
-    outs = att(qd, fd, fd, None, spatial_shapes=ss, level_start_index=lsi, reference_points_cams=uvs, tpv_masks=masks,
-               tpv_vis=vises)
+    outs = att(qd, fd, fd, None, spatial_shapes=ss, level_start_index=lsi, reference_points_cams=uvs, tpv_masks=masks)
     sum((o * go.to(dev)).sum() for o, go in zip(outs, gouts)).backward()
     f64 = feat.double().requires_grad_(True)
     names = ('attn_hw', 'attn_zh', 'attn_wz')
@@ -302,6 +302,125 @@ def test_cross_view_hybrid_attention_training_matches_fp64_oracle():
         e = (a.grad.cpu().double() - b.grad).abs().max().item() / b.grad.abs().max().item()
         print('%s grad %.2e of max-abs' % (name, e))
         assert e < 1e-3, name
+
+
+# --------------------------------------------------------------------------------------------- the layer's training routine
+def _small_encoder(dev, num_layers, seed):
+    """The encoder of test_tpv_layer_training_step_runs_without_host_sync's geometry at dropout 0, weights `_perturb`ed, in
+    train(); returns it with a frame's FPN features and metas."""
+    from selfocc_b200 import configs
+    from selfocc_b200.registry import build_head
+    import selfocc_b200.segmentor  # noqa: F401
+    torch.manual_seed(seed)
+    margs, rng = synth.small_mapping(8, 4, rng=20.0, z0=-2.0, z1=4.0)
+    cfg = configs.hot_path_config(mapping_args=margs, pc_range=rng, num_cams=6, num_layers=num_layers,
+                                  num_points_cross=(6, 6, 4), num_points_self=4, dropout=0.0)
+    enc = build_head(cfg['encoder'])
+    enc.init_weights()
+    g = torch.Generator().manual_seed(seed + 1)
+    _perturb(enc, g)
+    enc.to(dev).train()
+    l2i, _ = synth.camera_rig(synth.NUSC_YAWS, f=126.6, cx=80., cy=45., height=0.5, radius=0.2)
+    metas = [dict(lidar2img=list(l2i), img_shape=(90, 160))]
+    feats = [torch.randn(1, 6, 96, h, w, generator=g).to(dev) for h, w in [(12, 20), (6, 10), (3, 5), (2, 3)]]
+    return enc, feats, metas
+
+
+def _layer_inputs(enc, feats, metas, g):
+    """One layer's operands as leaves: planes and positional embeddings [1, Q_i, C] x 3, image features [N, sum(hw), 1, C];
+    the layer's keyword arguments; the camera projections and masks."""
+    dev = feats[0].device
+    feat, ss, lsi = enc.flatten_features(feats)
+    H, W, Z = enc.tpv_size
+    C = feat.shape[-1]
+    planes = [torch.randn(1, n, C, generator=g).to(dev).requires_grad_(True) for n in (H * W, Z * H, W * Z)]
+    pos = [torch.randn(1, n, C, generator=g).to(dev).requires_grad_(True) for n in (H * W, Z * H, W * Z)]
+    feat = feat.detach().requires_grad_(True)
+    uvs, masks, vises = enc.project_reference_points(metas, dev)
+    kw = dict(tpv_pos=pos, ref_2d=enc.cross_view_ref_points[None], spatial_shapes=ss, level_start_index=lsi,
+              reference_points_cams=uvs, tpv_masks=masks, tpv_size=enc.tpv_size, tpv_vis=vises,
+              tpv_levels=(enc.tpv_spatial_shapes, enc.tpv_level_start))
+    return planes, pos, feat, kw
+
+
+@gpu
+def test_tpv_layer_training_matches_fp64_oracle():
+    """One TPVFormerLayer in train() at dropout 0 through its training routine (forward_rows_train: the fused cores with their
+    backward kernels, train_linear, nn.LayerNorm) against fp64 autograd of oracle.lifting.tpv_layer_ref: the layer's
+    outputs, every parameter's gradient and the gradients of the input planes, positional embeddings and image features,
+    at the module tests' bars."""
+    dev = _dev()
+    from oracle import lifting as ol
+    enc, feats, metas = _small_encoder(dev, 1, seed=23)
+    layer = enc.layers[0]
+    g = torch.Generator().manual_seed(24)
+    planes, pos, feat, kw = _layer_inputs(enc, feats, metas, g)
+    outs = layer(planes, feat, feat, **kw)
+    gouts = [torch.randn(o.shape, generator=g) for o in outs]
+    sum((o * go.to(dev)).sum() for o, go in zip(outs, gouts)).backward()
+    p64 = _leaf64(layer, 'l.')
+    planes64, pos64 = ([t.detach().cpu().double().requires_grad_(True) for t in ts] for ts in (planes, pos))
+    f64 = feat.detach().cpu().double().requires_grad_(True)
+    shapes = [tuple(s) for s in kw['spatial_shapes'].tolist()]
+    ocfg = dict(num_heads=layer.attentions[0].num_heads, num_points_self=layer.attentions[0].num_points, num_cams=6)
+    ref = ol.tpv_layer_ref(p64, 'l.', planes64, pos64, f64, shapes, kw['ref_2d'].cpu().double(),
+                           [uv.cpu().double() for uv in kw['reference_points_cams']], [m.cpu().bool() for m in kw['tpv_masks']],
+                           enc.tpv_size, ocfg)
+    for i, (o, r) in enumerate(zip(outs, ref)):
+        err = (o.detach().cpu().double() - r.detach()).abs().max().item()
+        print('plane %d output max abs err %.2e' % (i, err))
+        assert err < 1e-4, i
+    sum((r * go.double()).sum() for r, go in zip(ref, gouts)).backward()
+    _assert_grads_match(layer, p64, 'l.', _tol)
+    for name, got, want, tol in [('plane %d' % i, a, b, 1e-3) for i, (a, b) in enumerate(zip(planes, planes64))] + \
+            [('pos %d' % i, a, b, 1e-3) for i, (a, b) in enumerate(zip(pos, pos64))] + [('image features', feat, f64, 2e-4)]:
+        e = (got.grad.cpu().double() - want.grad).abs().max().item() / want.grad.abs().max().item()
+        print('%s grad %.2e of max-abs' % (name, e))
+        assert e < tol, name
+
+
+@gpu
+def test_training_forward_takes_the_row_routine(monkeypatch):
+    """A training forward through TPVFormerEncoder.forward runs forward_rows_train once per layer and never the MSDA op; a
+    layer called with a key_padding_mask (all False) runs its op-order loop, the attention modules' reference formulation,
+    and computes what the routine computes."""
+    dev = _dev()
+    from selfocc_b200 import ops
+    from selfocc_b200.encoder import TPVFormerLayer
+    enc, feats, metas = _small_encoder(dev, 2, seed=25)
+    rows, msda = TPVFormerLayer.forward_rows_train, ops.MultiScaleDeformableAttnFunction
+    calls = dict(rows=[], msda=0)
+
+    def rows_spy(layer, *a, **k):
+        calls['rows'].append(layer)
+        return rows(layer, *a, **k)
+
+    class MsdaSpy:
+        @staticmethod
+        def apply(*a):
+            calls['msda'] += 1
+            return msda.apply(*a)
+
+    monkeypatch.setattr(TPVFormerLayer, 'forward_rows_train', rows_spy)
+    monkeypatch.setattr(ops, 'MultiScaleDeformableAttnFunction', MsdaSpy)
+    H, W, Z = enc.tpv_size
+    g = torch.Generator().manual_seed(26)
+    rep = [torch.randn(1, n, 96, generator=g).to(dev).requires_grad_(True) for n in (H * W, Z * H, W * Z)]
+    assert torch.is_grad_enabled() and enc.training
+    out = enc(representation=rep, ms_img_feats=feats, metas=metas)['representation']
+    sum(o.sum() for o in out).backward()
+    assert calls['rows'] == list(enc.layers) and calls['msda'] == 0
+    layer = enc.layers[0]
+    planes, _, feat, kw = _layer_inputs(enc, feats, metas, g)
+    calls['rows'].clear()
+    routine = layer(planes, feat, feat, **kw)
+    assert calls['rows'] == [layer]
+    calls['rows'].clear()
+    mask = torch.zeros(1, sum(p.shape[1] for p in planes), dtype=torch.bool, device=dev)
+    loop = layer(planes, feat, feat, key_padding_mask=mask, **kw)
+    assert calls['rows'] == [] and calls['msda'] == 4        # the self-attention and the three planes' cross-attention
+    for a, b in zip(loop, routine):
+        assert (a - b).abs().max().item() < 1e-4
 
 
 # --------------------------------------------------------------------------------------------- full size
