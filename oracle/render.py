@@ -197,8 +197,10 @@ def neus_render_chunk(vol, mapping, o, d, dnorm, aabb, inv_s, S=256, near_plane=
 
 
 def max_depth_ref(weights, ts, deltas):
-    """neus_head.py:430-438 / 579-587.  weights, ts, deltas [..., S] -> (max_depth, index int64)."""
-    eps = torch.finfo(deltas.dtype).eps
+    """neus_head.py:430-438 / 579-587.  weights, ts, deltas [..., S] -> (max_depth, index int64).  The reference renders in
+    fp32, so a sample is dropped below fp32's eps whatever dtype the oracle runs in: a ray that misses the ROI has
+    zero-length samples (far - near = 1e-6), all dropped, and takes index 0."""
+    eps = torch.finfo(torch.float32).eps
     w = weights.clone()
     w[deltas < eps] = 0.
     idx = (w / deltas.clamp_min(eps)).argmax(-1, keepdim=True)
@@ -207,14 +209,17 @@ def max_depth_ref(weights, ts, deltas):
 
 def head_render_ref(vol, mapping, origin, direction, aabb, inv_s, batch=0, max_depth_on_cpu=False, grid_override=None, **kw):
     """NeuSHead.render (neus_head.py:308-471) after ray generation: origin [1,N,3], direction
-    [1,N,R,3] un-normalised.  Serial chunk loop with ``torch.chunk`` sizes when batch > 0."""
+    [1,N,R,3] un-normalised.  Serial chunk loop with ``torch.chunk`` sizes when batch > 0.  ``bkgd_rand`` (bkgd='random')
+    holds one row per ray, [N*R, 3] in the flat (cam, ray) order, and is chunked with the rays."""
     from .rays import flatten_rays, num_chunks
     bs, n_cam, n_ray = direction.shape[:3]
     o, d, nrm = flatten_rays(origin, direction)
     n = num_chunks(o.shape[0], batch)
     go = [None] * n if grid_override is None else torch.chunk(grid_override.reshape(o.shape[0], -1, 3), n)
-    outs = [neus_render_chunk(vol, mapping, oc, dc, nc, aabb, inv_s, grid_override=gc, **kw)
-            for oc, dc, nc, gc in zip(torch.chunk(o, n), torch.chunk(d, n), torch.chunk(nrm, n), go)]
+    bk = kw.pop('bkgd_rand', None)
+    bk = [None] * n if bk is None else torch.chunk(bk.reshape(o.shape[0], 3), n)
+    outs = [neus_render_chunk(vol, mapping, oc, dc, nc, aabb, inv_s, grid_override=gc, bkgd_rand=bc, **kw)
+            for oc, dc, nc, gc, bc in zip(torch.chunk(o, n), torch.chunk(d, n), torch.chunk(nrm, n), go, bk)]
     cat = lambda k: torch.cat([c[k] for c in outs])
     weights = cat('weights')
     ts = (cat('starts') + cat('ends')) / 2 / nrm

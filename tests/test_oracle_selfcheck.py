@@ -119,6 +119,60 @@ def test_train_parity_reproduces_itself_and_masks_exactly_the_flip_rays():
                         color_dims=3, bkgd_rand=bk, chunk=5)
 
 
+def _random_bkgd_scene(n_feat=7):
+    """Small analytic scene with 3 colour + (n_feat - 3) semantic channels, 2 cameras x 3 x 4 rays, one background row per ray."""
+    m, aabb = _map(10, 6)
+    g = torch.Generator().manual_seed(3)
+    sdf = synth.analytic_sdf_volume(m, ground_z=-1.0, spheres=((3., 5., 0., 1.5),), boxes=(), noise=0.05, seed=1)
+    vol = torch.cat([sdf[None], 2.5 * torch.randn(n_feat, *sdf.shape, generator=g)], 0).double()
+    _, i2l = synth.camera_rig(synth.NUSC_YAWS[:2], f=126.6, cx=80., cy=45., height=0.5, radius=0.2)
+    origin, direction = orays.img2lidar_rays(torch.tensor(i2l, dtype=torch.float32)[None], orays.fixed_ray_grid([3, 4], [90, 160]))
+    bk = torch.rand(origin.shape[1] * direction.shape[2], 3, generator=g, dtype=torch.float64)
+    return m, aabb, vol, origin, direction, bk
+
+
+def test_render_parity_passes_the_oracle_itself_and_gates_max_depth_rgb_and_semantics():
+    """oracle/parity.py on the fp64 oracle's own outputs, its grid as the probe, random background: every comparison is at
+    rounding level and the report is ok.  Each planted error in max_depth, in rgb (the background of the next ray) and in
+    one semantic channel fails the report."""
+    from oracle.parity import render_parity
+    m, aabb, vol, origin, direction, bk = _random_bkgd_scene()
+    S, inv_s = 32, 12.0
+    kw = dict(color_dims=7, bkgd='random', bkgd_rand=bk)
+    ref = orender.head_render_ref(vol, m, origin.double(), direction.double(), aabb, inv_s, S=S, **kw)
+    n = bk.shape[0]
+    got = dict(depth=ref['depth'].reshape(n), acc=ref['acc'].reshape(n), max_idx=ref['max_idx'].reshape(n),
+               max_depth=ref['max_depth'].reshape(n), grid=ref['grid'].reshape(n, S, 3), rgb=ref['rgb'].reshape(n, 3),
+               normal_vis=ref['vis_normal'].reshape(n, 3), sem=ref['sem'].reshape(n, -1))
+    assert got['sem'].shape == (n, 4) and (ref['acc'] < 0.5).any()
+    rep = render_parity(got, vol, m, origin, direction, aabb, inv_s, S, **kw)
+    print(rep)
+    b = rep['same_cells']
+    assert rep['ok'] and rep['geometry']['max_abs_grid_units'] == 0 and rep['independent']['rays_with_cell_flip'] == 0
+    for k in ('depth_max_rel', 'acc_max_abs', 'max_depth_max_rel', 'normal_max_abs', 'rgb_max_abs', 'sem_max_abs'):
+        assert b[k] < 1e-12, (k, b[k])
+    low = (ref['acc'].reshape(n) < 0.5).nonzero()[0, 0]
+    bad_bk = got['rgb'].clone()
+    bad_bk[low] += (bk[(low + 1) % n] - bk[low]) * (1 - got['acc'][low])
+    for k, v in (('max_depth', got['max_depth'] * (1 + 2e-5)), ('rgb', bad_bk), ('sem', got['sem'] + 2e-4 * (torch.arange(4) == 2))):
+        assert not render_parity(dict(got, **{k: v}), vol, m, origin, direction, aabb, inv_s, S, **kw)['ok'], k
+
+
+def test_chunked_random_background_render_equals_the_per_chunk_restatement():
+    """head_render_ref with batch > 0 hands every chunk the background rows of its own rays (torch.chunk sizes)."""
+    m, aabb, vol, origin, direction, bk = _random_bkgd_scene()
+    S, inv_s, batch = 32, 12.0, 7
+    out = orender.head_render_ref(vol, m, origin.double(), direction.double(), aabb, inv_s, batch=batch, S=S, color_dims=7,
+                                  bkgd='random', bkgd_rand=bk)
+    o, d, nrm = orays.flatten_rays(origin.double(), direction.double())
+    n = orays.num_chunks(o.shape[0], batch)
+    assert n == 4
+    parts = [orender.neus_render_chunk(vol, m, oc, dc, nc, aabb, inv_s, S=S, color_dims=7, bkgd='random', bkgd_rand=bc)
+             for oc, dc, nc, bc in zip(torch.chunk(o, n), torch.chunk(d, n), torch.chunk(nrm, n), torch.chunk(bk, n))]
+    for k, pk in (('rgb', 'rgb'), ('depth', 'depth'), ('sem', 'sem')):
+        assert torch.equal(out[k].reshape(o.shape[0], -1), torch.cat([p[pk] for p in parts]).reshape(o.shape[0], -1)), k
+
+
 def test_slabwise_decode_equals_the_whole_volume_oracle_and_its_autograd():
     """oracle/decode_parity.py restates tpv_decode_ref slab by slab (ragged last slab, H != W): same volume, same gradients
     of every plane and MLP tensor, fp64, 1e-12; and its per-slice and per-bucket error reports on planted errors."""
