@@ -349,15 +349,28 @@ int so_flatten_level(const float* feat, const float* cams_embeds, const float* l
                      int32_t hw, int64_t level_start, int64_t total, void* stream);
 
 /* A4  projection of pillar reference points into the cameras.  Replaces point_sampling
- * (model/encoder/bevformer/utils.py:116-206, no post_rots / focal_ratios branch).
+ * (model/encoder/bevformer/utils.py:116-206, including the focal_ratios branch through
+ * so_point_sampling_scaled; the post_rots branch, which no shipped pipeline produces, is not covered).
  *   ref_3d [D, Q, 3] metres, lidar2img [N, 4, 4], img_h/img_w = metas[0]['img_shape']
  *   -> uv [N, Q, D, 2] normalised (x, y), mask uint8 [N, Q, D] (1 = in frustum),
  *      vis uint8 [N, Q] = any_d mask (the per-camera query visibility of
  *      image_cross_attention.py:92; NULL ok).
  * Arithmetic order is fixed (plain fp32 mul/add, no FMA contraction) so that `mask`, an index-
- * generating quantity, is reproducible bit for bit. */
+ * generating quantity, is reproducible bit for bit.  Same as so_point_sampling_scaled with scale_xy = NULL. */
 int so_point_sampling(const float* ref_3d, const float* lidar2img, int32_t D, int32_t Q, int32_t N,
                       float img_h, float img_w, float* uv, uint8_t* mask, uint8_t* vis, void* stream);
+
+/* A4 with the focal-ratio rescale of bevformer/utils.py:198-204 (metas[0]['focal_ratios_x' / '_y'],
+ * written by RandomScaleImageMultiViewImage).  scale_xy [N, 2] fp32 device memory holds
+ * (ratio_x, ratio_y) per camera, or NULL for none (bit-identical to so_point_sampling).  After the
+ * frustum test, uv[cam, ..., 0] *= ratio_x[cam] and uv[cam, ..., 1] *= ratio_y[cam], each one fp32
+ * multiply; mask and vis are those of the unscaled coordinates, as in the reference, so a visible
+ * sample may lie outside [0, 1] when a ratio exceeds 1.  The ratios are read on the device when the
+ * kernel runs (a captured graph picks up new values written into scale_xy).  Same error returns as
+ * so_point_sampling. */
+int so_point_sampling_scaled(const float* ref_3d, const float* lidar2img, const float* scale_xy, int32_t D,
+                             int32_t Q, int32_t N, float img_h, float img_w, float* uv, uint8_t* mask,
+                             uint8_t* vis, void* stream);
 
 /* A5+A6+A7  rebatch-free image cross-attention core for one TPV plane.  Replaces the
  * nonzero()/rebatch/scatter-add/count machinery of BEVCrossAttention.forward together with the

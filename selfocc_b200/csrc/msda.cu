@@ -681,11 +681,13 @@ __global__ void __launch_bounds__(256) tpv_self_attn_backward_kernel(
 // ---- A4 point_sampling (bevformer/utils.py:116-206) ---------------------------------------------------------
 // One thread per (camera, query, pillar point): fully coalesced uv / mask stores.  The projection uses plain fp32
 // mul/add in a fixed left-to-right order (no FMA contraction): `mask` generates index lists.  `vis` (any over the
-// pillar) is zero-filled first and set with idempotent byte stores.
+// pillar) is zero-filled first and set with idempotent byte stores.  `scale_xy` [N, 2] (NULL: none) is the per-camera
+// focal-ratio rescale of bevformer/utils.py:198-204: it multiplies uv AFTER the frustum test, so mask / vis are those of
+// the unscaled coordinates, as in the reference.  It is read from device memory so a graph replay sees the current ratios.
 __global__ void __launch_bounds__(256) point_sampling_kernel(const float* __restrict__ ref3d, const float* __restrict__ l2i,
-                                                             int D, int Q, int N, float img_h, float img_w,
-                                                             float* __restrict__ uv, unsigned char* __restrict__ mask,
-                                                             unsigned char* __restrict__ vis) {
+                                                             const float* __restrict__ scale_xy, int D, int Q, int N,
+                                                             float img_h, float img_w, float* __restrict__ uv,
+                                                             unsigned char* __restrict__ mask, unsigned char* __restrict__ vis) {
   long long t = blockIdx.x * (long long)blockDim.x + threadIdx.x;
   if (t >= (long long)N * Q * D) return;
   int d = (int)(t % D);
@@ -703,6 +705,10 @@ __global__ void __launch_bounds__(256) point_sampling_kernel(const float* __rest
   float u = __fdiv_rn(__fdiv_rn(cx, den), img_w);
   float v = __fdiv_rn(__fdiv_rn(cy, den), img_h);
   ok = ok && (v > 0.f) && (v < 1.f) && (u < 1.f) && (u > 0.f);
+  if (scale_xy) {
+    u = __fmul_rn(u, __ldg(scale_xy + 2 * cam));
+    v = __fmul_rn(v, __ldg(scale_xy + 2 * cam + 1));
+  }
   reinterpret_cast<float2*>(uv)[t] = make_float2(u, v);
   if (mask) mask[t] = ok ? 1 : 0;
   if (vis && ok) vis[cq] = 1;
@@ -804,8 +810,9 @@ extern "C" int so_msda_backward(const float* value, const int64_t* spatial_shape
   return check_launch();
 }
 
-extern "C" int so_point_sampling(const float* ref_3d, const float* lidar2img, int32_t D, int32_t Q, int32_t N, float img_h,
-                                 float img_w, float* uv, uint8_t* mask, uint8_t* vis, void* stream) {
+extern "C" int so_point_sampling_scaled(const float* ref_3d, const float* lidar2img, const float* scale_xy, int32_t D,
+                                        int32_t Q, int32_t N, float img_h, float img_w, float* uv, uint8_t* mask, uint8_t* vis,
+                                        void* stream) {
   if (!ref_3d || !lidar2img || !uv) return SO_ERR_INVALID_ARG;
   if (D < 1 || Q < 1 || N < 1 || !(img_h > 0.f) || !(img_w > 0.f)) return SO_ERR_INVALID_ARG;
   cudaStream_t st = (cudaStream_t)stream;
@@ -814,9 +821,15 @@ extern "C" int so_point_sampling(const float* ref_3d, const float* lidar2img, in
     note_launch(1);
   }
   long long n = (long long)N * Q * D;
-  point_sampling_kernel<<<(unsigned)ceil_div64(n, 256), 256, 0, st>>>(ref_3d, lidar2img, D, Q, N, img_h, img_w, uv, mask, vis);
+  point_sampling_kernel<<<(unsigned)ceil_div64(n, 256), 256, 0, st>>>(ref_3d, lidar2img, scale_xy, D, Q, N, img_h, img_w, uv,
+                                                                      mask, vis);
   note_launch(1);
   return check_launch();
+}
+
+extern "C" int so_point_sampling(const float* ref_3d, const float* lidar2img, int32_t D, int32_t Q, int32_t N, float img_h,
+                                 float img_w, float* uv, uint8_t* mask, uint8_t* vis, void* stream) {
+  return so_point_sampling_scaled(ref_3d, lidar2img, nullptr, D, Q, N, img_h, img_w, uv, mask, vis, stream);
 }
 
 extern "C" int so_tpv_cross_attn_forward_strided(const float* value, const int64_t* spatial_shapes, const int64_t* level_start_index,

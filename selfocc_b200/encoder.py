@@ -88,6 +88,37 @@ def _metas_matrix(metas, key, device):
     return torch.stack(mats)
 
 
+_FOCAL_KEYS = ('focal_ratios_x', 'focal_ratios_y')
+
+
+def _focal_scale(metas, n_cam, device):
+    """metas[0]['focal_ratios_x' / '_y'] -> scale_xy [n_cam, 2] fp32 on ``device``, or None when the metas carry neither.
+
+    RandomScaleImageMultiViewImage (dataset/transform_3d.py:362-363) writes both as lists of Python floats; numpy arrays and
+    tensors are taken too.  Like the reference (bevformer/utils.py:198-204) only metas[0]'s ratios are read, rounded to fp32
+    as ``new_tensor`` does, and a length of 1 broadcasts over the cameras.  A tensor already on ``device`` is used without
+    a host copy, so a captured graph (dist.GraphedFrame) reads whatever ratios were written into it before a replay.
+    Raises ValueError, before any kernel launch, for one key without the other or a length other than 1 or n_cam."""
+    m = metas[0]
+    present = [k in m for k in _FOCAL_KEYS]
+    if not any(present):
+        return None
+    if not all(present):
+        raise ValueError('metas[0] has %s without %s: the focal-ratio rescale needs both'
+                         % (_FOCAL_KEYS[present.index(True)], _FOCAL_KEYS[present.index(False)]))
+    cols = []
+    for k in _FOCAL_KEYS:
+        v = m[k]
+        if isinstance(v, torch.Tensor):
+            t = v.reshape(-1)
+        else:
+            t = torch.as_tensor(np.asarray(v, dtype=np.float64).reshape(-1))
+        if t.numel() not in (1, n_cam):
+            raise ValueError('metas[0][%r] holds %d ratios for %d cameras (expected 1 or %d)' % (k, t.numel(), n_cam, n_cam))
+        cols.append(t.to(device=device, dtype=torch.float32).expand(n_cam))
+    return torch.stack(cols, -1)
+
+
 # --------------------------------------------------------------------------- positional encoding (A10)
 @MODELS.register_module()
 class TPVPositionalEncoding(nn.Module):
@@ -736,15 +767,19 @@ class TPVFormerEncoder(nn.Module):
 
     def project_reference_points(self, metas, device):
         """A4: three point_sampling calls (tpvformer_encoder.py:205-210) -> per plane uv [N,B,Q,D,2],
-        mask [N,B,Q,D] uint8, vis [N,Q] uint8.  B must be 1 (as everywhere in the reference head)."""
-        if 'img_augmentation' in metas[0] or 'focal_ratios_x' in metas[0]:
-            raise NotImplementedError('post_rots / focal_ratios branches of point_sampling are not implemented')
+        mask [N,B,Q,D] uint8, vis [N,Q] uint8.  B must be 1 (as everywhere in the reference head).  Frames from the
+        reference's data wrapper carry metas[0]['focal_ratios_x' / '_y'] (RandomScaleImageMultiViewImage): uv is rescaled
+        per camera after the frustum test (bevformer/utils.py:198-204), see _focal_scale."""
+        if 'img_augmentation' in metas[0]:
+            raise NotImplementedError("the post_rots / post_trans branch of point_sampling (metas['img_augmentation']) is not "
+                                      'implemented: no shipped data pipeline produces it')
         l2i = _metas_matrix(metas, 'lidar2img', device)
         assert l2i.shape[0] == 1, 'only bs = 1 is supported (the reference head asserts the same)'
+        scale_xy = _focal_scale(metas, l2i.shape[1], device)
         shp = metas[0]['img_shape']
         uvs, masks, vises = [], [], []
         for ref in (self.ref_3d_hw, self.ref_3d_zh, self.ref_3d_wz):
-            uv, mask, vis = ops.point_sampling(ref, l2i[0].contiguous(), (shp[0], shp[1]))
+            uv, mask, vis = ops.point_sampling(ref, l2i[0].contiguous(), (shp[0], shp[1]), scale_xy)
             uvs.append(uv[:, None])
             masks.append(mask[:, None])
             vises.append(vis)

@@ -204,18 +204,22 @@ class MultiScaleDeformableAttnFunction(torch.autograd.Function):
         return gv, None, None, gl, gw, None
 
 
-def point_sampling(ref_3d, lidar2img, img_shape):
-    """ref_3d [D,Q,3], lidar2img [N,4,4] -> uv [N,Q,D,2], mask uint8 [N,Q,D], vis uint8 [N,Q]."""
+def point_sampling(ref_3d, lidar2img, img_shape, scale_xy=None):
+    """ref_3d [D,Q,3], lidar2img [N,4,4] -> uv [N,Q,D,2], mask uint8 [N,Q,D], vis uint8 [N,Q].
+    scale_xy [N,2] (per camera: focal_ratios_x, focal_ratios_y) multiplies uv after the frustum test; mask / vis stay those
+    of the unscaled uv (bevformer/utils.py:198-204)."""
     lib = _lib.load()
-    _chk(ref_3d, name='ref_3d'); _chk(lidar2img, name='lidar2img')
+    _chk(ref_3d, name='ref_3d'); _chk(lidar2img, name='lidar2img'); _chk(scale_xy, name='scale_xy')
     D, Q, _ = ref_3d.shape
     N = lidar2img.shape[0]
+    if scale_xy is not None and tuple(scale_xy.shape) != (N, 2):
+        raise ValueError('scale_xy must have shape [%d, 2] (one (x, y) ratio pair per camera), got %s' % (N, tuple(scale_xy.shape)))
     dev = ref_3d.device
     uv = torch.empty(N, Q, D, 2, device=dev)
     mask = torch.empty(N, Q, D, device=dev, dtype=torch.uint8)
     vis = torch.empty(N, Q, device=dev, dtype=torch.uint8)
-    _lib.check(lib.so_point_sampling(_p(ref_3d), _p(lidar2img), D, Q, N, float(img_shape[0]), float(img_shape[1]),
-                                     _p(uv), _p(mask), _p(vis), _stream()), 'so_point_sampling')
+    _lib.check(lib.so_point_sampling_scaled(_p(ref_3d), _p(lidar2img), _p(scale_xy), D, Q, N, float(img_shape[0]),
+                                            float(img_shape[1]), _p(uv), _p(mask), _p(vis), _stream()), 'so_point_sampling_scaled')
     return uv, mask, vis
 
 
