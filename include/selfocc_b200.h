@@ -112,6 +112,27 @@ int so_tpv_decode_bwd_hidden(float* z1_a1, const float* g_vol_sdf, const float* 
                              void* stream);
 int so_tpv_decode_bwd_input(float* g0, const float* a0, int64_t n, void* stream);
 
+/* B5 for tpv=False heads (the BEV-only model; bev_nerf.py:62-81, density_layers=2):
+ *     out[r][z * Cf + c] = W2 * softplus(W1 * softplus(bev[r]) + b1) + b2          (C -> C -> Z * Cf), Cf = 1 + n_feat
+ * bev [H*W, C] (row r = h * W + w); w1 [C, C], b1 [C], w2 [Z * Cf, C], b2 [Z * Cf].  Column z * Cf + c of row r is voxel
+ * (h, w, z), channel c: c = 0 -> vol_sdf [H, W, zpitch] (pads z in [Z, zpitch) written as 0), c >= 1 -> vol_feat
+ * [H, W, Z, feat_pitch] channel c - 1 (may be NULL when n_feat == 0; pad channels never written, as so_tpv_decode).
+ * One persistent wgmma kernel with the 3xTF32 split; the hidden and output matrices never reach global memory, and every
+ * voxel is computed the same way whatever the SM count.  C == 96 and Z * Cf <= 2048, else SO_ERR_UNSUPPORTED before any
+ * launch; bev, w1 and w2 16-byte aligned. */
+int so_bev_decode(const float* bev, int32_t C, const float* w1, const float* b1, const float* w2, const float* b2,
+                  const so_volume_desc* vol_host, float* vol_sdf, float* vol_feat, void* stream);
+/* Element-wise pieces of its backward (training), around the products on so_linear_3xtf32 / cuBLAS:
+ *   gather:   g_out[row_count][Z * Cf] of rows [row_begin, row_begin + row_count) from g_vol_sdf / g_vol_feat (NULL = zero;
+ *             sdf pads and feature pad channels never read)
+ *   features: a0[n] = softplus(bev[n])
+ *   hidden:   z1_a1[n] holds z1 on entry and a1 = softplus(z1) on return; g1[n] *= sigmoid(z1)
+ * with the relative-accuracy softplus / sigmoid forms of so_tpv_decode_bwd_*; the input side is so_tpv_decode_bwd_input. */
+int so_bev_decode_bwd_gather(const float* g_vol_sdf, const float* g_vol_feat, const so_volume_desc* vol_host, int64_t row_begin,
+                             int64_t row_count, float* g_out, void* stream);
+int so_bev_decode_bwd_features(const float* bev, int64_t n, float* a0, void* stream);
+int so_bev_decode_bwd_hidden(float* z1_a1, float* g1, int64_t n, void* stream);
+
 /* Test hook: force the fp32 SIMT decode kernel (default: the wgmma 3xTF32 kernel whenever C % 32 == 0). */
 int so_tpv_decode_force_simt(int on);
 

@@ -53,6 +53,10 @@ SIGNATURES = {
     'so_tpv_decode_bwd_hidden': (C.c_int, [_P, _P, _P, _P, _I, C.POINTER(VolumeDesc), _I, _I, _P, _P, _P]),
     'so_tpv_decode_bwd_input': (C.c_int, [_P, _P, _L, _P]),
     'so_tpv_decode_force_simt': (C.c_int, [C.c_int]),
+    'so_bev_decode': (C.c_int, [_P, _I, _P, _P, _P, _P, C.POINTER(VolumeDesc), _P, _P, _P]),
+    'so_bev_decode_bwd_gather': (C.c_int, [_P, _P, C.POINTER(VolumeDesc), _L, _L, _P, _P]),
+    'so_bev_decode_bwd_features': (C.c_int, [_P, _L, _P, _P]),
+    'so_bev_decode_bwd_hidden': (C.c_int, [_P, _P, _L, _P]),
     'so_render_train_force_fwd32': (C.c_int, [C.c_int]),
     'so_render_train_force_sem_generic': (C.c_int, [C.c_int]),
     'so_render_workspace_floats': (C.c_int64, [_L]),

@@ -62,6 +62,26 @@ __device__ __forceinline__ float sigmoid_of_softplus(float a) {
   return a < 0.125f ? a * p : 1.0f - __expf(-a);
 }
 
+// Split v into TF32 hi / lo (hi + lo == v exactly) and store both at byte offset off of the hi and lo operand atoms.
+__device__ __forceinline__ void store_split_tf32(uint8_t* hi, uint8_t* lo, uint32_t off, float4 v) {
+  float4 h, l;
+  h.x = tf32_rn(v.x); l.x = v.x - h.x; h.y = tf32_rn(v.y); l.y = v.y - h.y;
+  h.z = tf32_rn(v.z); l.z = v.z - h.z; h.w = tf32_rn(v.w); l.w = v.w - h.w;
+  *reinterpret_cast<float4*>(hi + off) = h;
+  *reinterpret_cast<float4*>(lo + off) = l;
+}
+
+// Builder step of the tensor-core decodes (TPV and BEV): softplus of one 16-byte chunk x of a row's pre-activations, split
+// into TF32 hi / lo and stored at (row, chunk c4) of the 128B-swizzled K-major A atoms.  Rows past the end (ok false) are 0.
+__device__ __forceinline__ void build_a_chunk(uint8_t* hi, uint8_t* lo, int row, int c4, float4 x, bool ok) {
+  float4 f = make_float4(0.f, 0.f, 0.f, 0.f);
+  if (ok) {
+    f.x = softplus_fast(x.x); f.y = softplus_fast(x.y);
+    f.z = softplus_fast(x.z); f.w = softplus_fast(x.w);
+  }
+  store_split_tf32(hi, lo, swz_off(row, c4), f);
+}
+
 // C = channels (multiple of 32), LD = padded leading dimension (C + 4) in floats
 template <int C>
 __global__ void __launch_bounds__(kThreads) tpv_decode_kernel(
@@ -225,12 +245,8 @@ tpv_decode_tc_kernel(const float* __restrict__ hw, const float* __restrict__ zh,
   // W1 [out j][in k] is K-major already: split it and lay it out as KA swizzled atoms of [C rows x 32 k]
   for (int i = tid; i < C * C / 4; i += kDecThreads) {
     int j = (i * 4) / C, k = (i * 4) % C;
-    float4 v = __ldg(reinterpret_cast<const float4*>(w1) + i), h, l;
-    h.x = tf32_rn(v.x); l.x = v.x - h.x; h.y = tf32_rn(v.y); l.y = v.y - h.y;
-    h.z = tf32_rn(v.z); l.z = v.z - h.z; h.w = tf32_rn(v.w); l.w = v.w - h.w;
-    uint32_t off = (uint32_t)((k / kAtomK) * C * 128) + swz_off(j, (k % kAtomK) / 4);
-    *reinterpret_cast<float4*>(w_hi + off) = h;
-    *reinterpret_cast<float4*>(w_lo + off) = l;
+    store_split_tf32(w_hi, w_lo, (uint32_t)((k / kAtomK) * C * 128) + swz_off(j, (k % kAtomK) / 4),
+                     __ldg(reinterpret_cast<const float4*>(w1) + i));
   }
   for (int i = tid; i < n_out * C; i += kDecThreads) W2s[i] = __ldg(w2 + i);
   for (int i = tid; i < C; i += kDecThreads) b1s[i] = __ldg(b1 + i);
@@ -268,19 +284,10 @@ tpv_decode_tc_kernel(const float* __restrict__ hw, const float* __restrict__ zh,
           u[j] = ok ? __ldg(reinterpret_cast<const float4*>(wz + (size_t)vv[j] * C + kc)) : make_float4(0.f, 0.f, 0.f, 0.f);
         }
 #pragma unroll
-        for (int j = 0; j < 4; ++j) {
-          float4 f = make_float4(0.f, 0.f, 0.f, 0.f);
-          if (vv[j] < WZ) {
-            f.x = softplus_fast(x[j].x + y[j].x + u[j].x); f.y = softplus_fast(x[j].y + y[j].y + u[j].y);
-            f.z = softplus_fast(x[j].z + y[j].z + u[j].z); f.w = softplus_fast(x[j].w + y[j].w + u[j].w);
-          }
-          float4 hh, ll;
-          hh.x = tf32_rn(f.x); ll.x = f.x - hh.x; hh.y = tf32_rn(f.y); ll.y = f.y - hh.y;
-          hh.z = tf32_rn(f.z); ll.z = f.z - hh.z; hh.w = tf32_rn(f.w); ll.w = f.w - hh.w;
-          const uint32_t off = swz_off(r0 + 32 * j, c4);
-          *reinterpret_cast<float4*>(hi + off) = hh;
-          *reinterpret_cast<float4*>(lo + off) = ll;
-        }
+        for (int j = 0; j < 4; ++j)
+          build_a_chunk(hi, lo, r0 + 32 * j, c4,
+                        make_float4(x[j].x + y[j].x + u[j].x, x[j].y + y[j].y + u[j].y, x[j].z + y[j].z + u[j].z,
+                                    x[j].w + y[j].w + u[j].w), vv[j] < WZ);
         asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
         mbar_arrive(conv + s);
         if (++s == stages) { s = 0; ph ^= 1; }
@@ -369,6 +376,296 @@ tpv_decode_tc_kernel(const float* __restrict__ hw, const float* __restrict__ zh,
         }
       }
     }
+  }
+}
+
+// ---------------------------------------------------------------------------------------------------------------------
+// BEV decode (tpv=False heads, bev_nerf.py:62-81): one row per BEV cell, N = Z * Cf outputs per row,
+//   a0 = softplus(bev[r])     a1 = softplus(a0 W1^T + b1)     out[r][z * Cf + c] = a1 W2[z * Cf + c]^T + b2   -> voxel (r, z), c
+// N is far beyond a register-resident second layer (625 at the shipped geometry), so both layers run on the tensor cores
+// with the 3xTF32 split.  Persistent CTA per SM, 12 warps:
+//   warps 0-3   builders  per 128-row tile: the A atoms of a0 (build_a_chunk, shared with the TPV decode), then every
+//                         n-tile of W2 split into hi / lo, read from L2 (every CTA splits the same 240 KB, so no split copy
+//                         of the weights has to live in global memory); the next n-tile's loads are in flight while one
+//                         is split and stored
+//   warps 4-11  two consumer warpgroups, 64 rows each: GEMM 1 with resident W1 hi / lo, + b1, softplus; the hidden tile
+//                         stays in registers as the A operand of GEMM 2 (wgmma with A from registers), one n-tile of W2 at a
+//                         time from the ring, + b2, staged in shared memory and written out row by row.  Neither the
+//                         [rows, C] hidden nor the [rows, N] output matrix reaches HBM.
+// GEMM 2's A fragment holds hidden columns (8j + 2t, 8j + 2t + 1) where wgmma reads k = (t, t + 4) of the k-block: the
+// builders store W2's k in the same order (even columns in the first four positions of each 8-column block, odd in the
+// last four), so the contraction is unchanged.  Every output takes the same products in the same order whatever the grid.
+constexpr int kBevBuilders = 128;
+constexpr int kBevThreads = kBevBuilders + 256;
+constexpr int kBevBN = 64;            // GEMM 2 n-tile
+constexpr int kBevStagesA = 1, kBevStagesW = 2;   // 72 KB W1 + 32 KB A (also the output staging) + 2 x 48 KB W2
+constexpr int kBevMaxCols = 2048;     // Z * Cf: every CTA splits all of W2 per tile; beyond this that outweighs the tile's output
+
+struct BevSmem {
+  int w1, ring_a, ring_w, b1, bars, total;
+};
+__host__ __device__ inline BevSmem bev_smem(int C) {
+  BevSmem m;
+  m.w1 = 0;                                                        // W1 hi + lo: (C / 32) atoms x [C rows x 128 B] each
+  m.ring_a = 2 * C * C * 4;
+  m.ring_w = m.ring_a + kBevStagesA * 2 * kAtomBytesA;             // A stage: hi + lo atom of 128 rows
+  m.b1 = m.ring_w + kBevStagesW * 2 * C * kBevBN * 4;              // W2 stage: hi + lo, (C / 32) atoms x [BN rows x 128 B]
+  m.bars = m.b1 + C * 4;
+  m.total = m.bars + 256 + 1024;
+  return m;
+}
+
+template <int C>
+__global__ void __launch_bounds__(kBevThreads, 1)
+bev_decode_tc_kernel(const float* __restrict__ bev, const float* __restrict__ w1, const float* __restrict__ b1,
+                     const float* __restrict__ w2, const float* __restrict__ b2, int rows, int Z, int Cf, int zpitch,
+                     int feat_pitch, float* __restrict__ vol_sdf, float* __restrict__ vol_feat, int n_tiles) {
+  extern __shared__ uint8_t smem_raw[];
+  uint8_t* sm = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
+  constexpr int KA = C / kAtomK;
+  constexpr int kWAtom = kBevBN * 128;                             // bytes of one W2 atom (BN rows)
+  const BevSmem L = bev_smem(C);
+  uint8_t* w_hi = sm + L.w1;
+  uint8_t* w_lo = w_hi + KA * C * 128;
+  uint8_t* ring_a = sm + L.ring_a;
+  uint8_t* ring_w = sm + L.ring_w;
+  float* b1s = reinterpret_cast<float*>(sm + L.b1);
+  uint64_t* full_a = reinterpret_cast<uint64_t*>(sm + L.bars);
+  uint64_t* empty_a = full_a + kBevStagesA;
+  uint64_t* full_w = empty_a + kBevStagesA;
+  uint64_t* empty_w = full_w + kBevStagesW;
+  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  const int N = Z * Cf, n_tiles_w = (N + kBevBN - 1) / kBevBN;
+
+  if (tid == 0) {
+    for (int s = 0; s < kBevStagesA; ++s) { mbar_init(full_a + s, kBevBuilders); mbar_init(empty_a + s, 8); }
+    for (int s = 0; s < kBevStagesW; ++s) { mbar_init(full_w + s, kBevBuilders); mbar_init(empty_w + s, 8); }
+    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+  }
+  for (int i = tid; i < C * C / 4; i += kBevThreads) {
+    const int j = (i * 4) / C, k = (i * 4) % C;
+    store_split_tf32(w_hi, w_lo, (uint32_t)((k / kAtomK) * C * 128) + swz_off(j, (k % kAtomK) / 4),
+                     __ldg(reinterpret_cast<const float4*>(w1) + i));
+  }
+  for (int i = tid; i < C; i += kBevThreads) b1s[i] = __ldg(b1 + i);
+  asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+  __syncthreads();
+
+  if (warp < kBevBuilders / 32) {
+    // ===== builders =====
+    const int c4 = tid & 7, r0 = tid >> 3;                         // A: 16-byte chunk c4 of rows r0 + 16 j
+    const int wr = tid >> 2, wq = tid & 3;       // W2: rows wr + 32 i of the n-tile, 8-column block wq of every atom
+    constexpr int WR = kBevBN / 32;
+    int sa = 0, sw = 0;
+    uint32_t pa = 0, pw = 0;
+    float4 w[WR][KA][2];                         // the n-tile being loaded: [row][atom][even / odd half of the block]
+    auto load_w2 = [&](int nt) {
+#pragma unroll
+      for (int i = 0; i < WR; ++i) {
+        const int n = nt * kBevBN + wr + 32 * i;
+#pragma unroll
+        for (int a = 0; a < KA; ++a) {
+          const float4* src = reinterpret_cast<const float4*>(w2 + (size_t)n * C + a * kAtomK + wq * 8);
+          w[i][a][0] = n < N ? __ldg(src) : make_float4(0.f, 0.f, 0.f, 0.f);
+          w[i][a][1] = n < N ? __ldg(src + 1) : make_float4(0.f, 0.f, 0.f, 0.f);
+        }
+      }
+    };
+    for (int t = blockIdx.x; t < n_tiles; t += gridDim.x) {
+      const int row0 = t * kBM;
+      for (int a = 0; a < KA; ++a) {
+        float4 x[kBM / 16];
+#pragma unroll
+        for (int j = 0; j < kBM / 16; ++j) {
+          const int r = row0 + r0 + 16 * j;
+          x[j] = r < rows ? __ldg(reinterpret_cast<const float4*>(bev + (size_t)r * C + a * kAtomK + c4 * 4)) : make_float4(0.f, 0.f, 0.f, 0.f);
+        }
+        mbar_wait(empty_a + sa, pa ^ 1);
+        uint8_t* hi = ring_a + sa * 2 * kAtomBytesA;
+#pragma unroll
+        for (int j = 0; j < kBM / 16; ++j) build_a_chunk(hi, hi + kAtomBytesA, r0 + 16 * j, c4, x[j], row0 + r0 + 16 * j < rows);
+        asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+        mbar_arrive(full_a + sa);
+        if (++sa == kBevStagesA) { sa = 0; pa ^= 1; }
+      }
+      load_w2(0);
+      for (int nt = 0; nt < n_tiles_w; ++nt) {
+        float4 cur[WR][KA][2];
+#pragma unroll
+        for (int i = 0; i < WR; ++i)
+#pragma unroll
+          for (int a = 0; a < KA; ++a) { cur[i][a][0] = w[i][a][0]; cur[i][a][1] = w[i][a][1]; }
+        if (nt + 1 < n_tiles_w) load_w2(nt + 1);
+        mbar_wait(empty_w + sw, pw ^ 1);
+        uint8_t* hi = ring_w + sw * 2 * KA * kWAtom;
+#pragma unroll
+        for (int i = 0; i < WR; ++i)
+#pragma unroll
+          for (int a = 0; a < KA; ++a) {
+            const float4 u = cur[i][a][0], v = cur[i][a][1];
+            uint8_t* ah = hi + a * kWAtom;
+            store_split_tf32(ah, ah + KA * kWAtom, swz_off(wr + 32 * i, 2 * wq), make_float4(u.x, u.z, v.x, v.z));      // even
+            store_split_tf32(ah, ah + KA * kWAtom, swz_off(wr + 32 * i, 2 * wq + 1), make_float4(u.y, u.w, v.y, v.w));  // odd
+          }
+        asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+        mbar_arrive(full_w + sw);
+        if (++sw == kBevStagesW) { sw = 0; pw ^= 1; }
+      }
+    }
+  } else {
+    // ===== consumers: warpgroup wg owns rows 64 wg .. 64 wg + 63 of every tile =====
+    const int wg = (warp - kBevBuilders / 32) >> 2, wl = warp & 3, g = lane >> 2, t4 = lane & 3;
+    const int frag_row = wg * kWgRows + wl * 16 + g;               // this thread's rows: frag_row and frag_row + 8
+    const uint32_t whi = smem_u32(w_hi), wlo = smem_u32(w_lo);
+    const float inv_cf = 1.0f / (float)Cf;
+    const int wrow0 = wg * kWgRows + wl * 16;                       // the warp's 16 rows of every tile
+    // the warp's staging: its rows of the A stage's hi (warps 0, 1 of the warpgroup) or lo (warps 2, 3) atom
+    float* stage = reinterpret_cast<float*>(ring_a + (wl >> 1) * kAtomBytesA + wg * kWgRows * 128 + (wl & 1) * 32 * 128);
+    int sa = 0, sw = 0;
+    uint32_t pa = 0, pw = 0;
+    for (int t = blockIdx.x; t < n_tiles; t += gridDim.x) {
+      const int row0 = t * kBM;
+      // ---- GEMM 1: z1 = a0 W1^T ----
+      float acc[C / 2];
+#pragma unroll
+      for (int i = 0; i < C / 2; ++i) acc[i] = 0.f;
+      uint32_t accum = 0;
+      for (int a = 0; a < KA; ++a) {
+        mbar_wait(full_a + sa, pa);
+        const uint32_t ahi = smem_u32(ring_a + sa * 2 * kAtomBytesA) + wg * kWgRows * 128, alo = ahi + kAtomBytesA;
+        const uint32_t bhi = whi + a * C * 128, blo = wlo + a * C * 128;
+#pragma unroll
+        for (int i = 0; i < C / 2; ++i) asm volatile("" : "+f"(acc[i])::"memory");
+        wg_fence();
+#pragma unroll
+        for (int prod = 0; prod < 3; ++prod) {
+          const uint32_t ab = prod == 1 ? alo : ahi;
+          const uint32_t bb = prod == 2 ? blo : bhi;
+#pragma unroll
+          for (int k = 0; k < kAtomK / 8; ++k) {
+            Wgmma<C>::ss(acc, make_desc(ab + k * 32), make_desc(bb + k * 32), accum);
+            accum = 1u;
+          }
+        }
+        wg_commit();
+        wg_wait0();
+#pragma unroll
+        for (int i = 0; i < C / 2; ++i) asm volatile("" : "+f"(acc[i])::"memory");
+        __syncwarp();
+        if (lane == 0 && a < KA - 1) mbar_arrive(empty_a + sa);      // the last atom's rows stage the output (below)
+        if (a < KA - 1 && ++sa == kBevStagesA) { sa = 0; pa ^= 1; }
+      }
+      // ---- a1 = softplus(z1 + b1) as GEMM 2's A fragments, split into TF32 hi / lo ----
+      uint32_t fh[C / 8][4], fl[C / 8][4];
+#pragma unroll
+      for (int j = 0; j < C / 8; ++j) {
+        const int col = 8 * j + 2 * t4;
+        const float h[4] = {softplus_fast(acc[4 * j] + b1s[col]), softplus_fast(acc[4 * j + 2] + b1s[col]),
+                            softplus_fast(acc[4 * j + 1] + b1s[col + 1]), softplus_fast(acc[4 * j + 3] + b1s[col + 1])};
+#pragma unroll
+        for (int q = 0; q < 4; ++q) {
+          const float hh = tf32_rn(h[q]);
+          fh[j][q] = __float_as_uint(hh);
+          fl[j][q] = __float_as_uint(h[q] - hh);
+        }
+      }
+      // ---- GEMM 2, one n-tile of W2 at a time.  Epilogue: the warp's 16 rows x BN columns go through its own 4 KB of the A
+      // stage (rows this warpgroup read in GEMM 1, free until the next tile's A), then out row by row while the next
+      // n-tile's products run: column n = z * Cf + c -> voxel (r, z), channel c, so 32 lanes write 32 consecutive columns,
+      // one contiguous run of vol_feat (and the few sdf entries among them).
+      auto write_out = [&](int nt) {
+        int zq[2], cq[2];
+        float bq[2];
+#pragma unroll
+        for (int q = 0; q < 2; ++q) {
+          const int n = nt * kBevBN + lane + 32 * q;
+          // (n + 1/2) / Cf is at least 1/(2 Cf) away from an integer, far beyond the product's rounding: the floor is exact
+          zq[q] = __float2int_rd(((float)n + 0.5f) * inv_cf);
+          cq[q] = n < N ? n - zq[q] * Cf : -1;
+          bq[q] = n < N ? __ldg(b2 + n) : 0.f;
+        }
+#pragma unroll 4
+        for (int lr = 0; lr < 16; ++lr) {
+          const int r = row0 + wrow0 + lr;
+#pragma unroll
+          for (int q = 0; q < 2; ++q) {
+            const float o = stage[lr * kBevBN + ((lane + 32 * q) ^ ((lr & 7) << 3))] + bq[q];
+            if (r >= rows) continue;
+            if (cq[q] == 0) vol_sdf[(size_t)r * zpitch + zq[q]] = o;
+            else if (cq[q] > 0) vol_feat[((size_t)r * Z + zq[q]) * feat_pitch + (cq[q] - 1)] = o;
+          }
+        }
+      };
+      for (int nt = 0; nt < n_tiles_w; ++nt) {
+        mbar_wait(full_w + sw, pw);
+        const uint32_t bhi = smem_u32(ring_w + sw * 2 * KA * kWAtom), blo = bhi + KA * kWAtom;
+        float acc2[kBevBN / 2];
+#pragma unroll
+        for (int i = 0; i < kBevBN / 2; ++i) acc2[i] = 0.f;
+#pragma unroll
+        for (int j = 0; j < C / 8; ++j)
+#pragma unroll
+          for (int q = 0; q < 4; ++q) asm volatile("" : "+r"(fh[j][q]), "+r"(fl[j][q])::"memory");
+        wg_fence();
+#pragma unroll
+        for (int j = 0; j < C / 8; ++j) {
+          const uint32_t off = (j / 4) * kWAtom + (j % 4) * 32;
+          Wgmma<kBevBN>::rs(acc2, fh[j], make_desc(bhi + off), j ? 1u : 0u);
+          Wgmma<kBevBN>::rs(acc2, fl[j], make_desc(bhi + off), 1u);
+          Wgmma<kBevBN>::rs(acc2, fh[j], make_desc(blo + off), 1u);
+        }
+        wg_commit();
+        if (nt > 0) write_out(nt - 1);
+        wg_wait0();
+#pragma unroll
+        for (int i = 0; i < kBevBN / 2; ++i) asm volatile("" : "+f"(acc2[i])::"memory");
+        __syncwarp();
+        if (lane == 0) mbar_arrive(empty_w + sw);
+        if (++sw == kBevStagesW) { sw = 0; pw ^= 1; }
+#pragma unroll
+        for (int jb = 0; jb < kBevBN / 8; ++jb)
+#pragma unroll
+          for (int hr = 0; hr < 2; ++hr)
+            *reinterpret_cast<float2*>(stage + (g + 8 * hr) * kBevBN + ((8 * jb + 2 * t4) ^ (g << 3))) =
+                make_float2(acc2[4 * jb + 2 * hr], acc2[4 * jb + 2 * hr + 1]);
+        __syncwarp();
+      }
+      write_out(n_tiles_w - 1);
+      __syncwarp();
+      if (lane == 0) mbar_arrive(empty_a + sa);                     // the staging rows are free for the next tile's A
+      if (++sa == kBevStagesA) { sa = 0; pa ^= 1; }
+    }
+  }
+}
+
+// ---- BEV decode backward pieces (BEVDecodeFunction: the products run on the 3xTF32 GEMM / cuBLAS between them) ----
+// g_out[r][z * Cf + c] of rows [row_begin, row_begin + n / N) gathered from the volume gradients (NULL: zero; pads ignored)
+__global__ void __launch_bounds__(256) bev_decode_bwd_gather_kernel(const float* __restrict__ g_vs, const float* __restrict__ g_vf,
+                                                                    int Z, int zpitch, int Cf, int feat_pitch, long long row_begin,
+                                                                    long long n, float* __restrict__ g_out) {
+  const int N = Z * Cf;
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
+    const long long r = row_begin + i / N;
+    const int col = (int)(i % N), z = col / Cf, c = col - z * Cf;
+    float g = 0.f;
+    if (c == 0) { if (g_vs) g = __ldg(g_vs + r * zpitch + z); }
+    else if (g_vf) g = __ldg(g_vf + (r * Z + z) * feat_pitch + c - 1);
+    g_out[i] = g;
+  }
+}
+
+// a0 = softplus(x), accurate relative to its value (softplus_rel)
+__global__ void __launch_bounds__(256) bev_decode_bwd_features_kernel(const float* __restrict__ x, long long n, float* __restrict__ a0) {
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x)
+    a0[i] = softplus_rel(__ldg(x + i));
+}
+
+// z1 -> a1 = softplus(z1) in place, g1 *= sigmoid(z1) (one exponential: softplus_sigmoid)
+__global__ void __launch_bounds__(256) bev_decode_bwd_hidden_kernel(float* __restrict__ z1_a1, float* __restrict__ g1, long long n) {
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
+    float sg;
+    z1_a1[i] = softplus_sigmoid(z1_a1[i], &sg);
+    g1[i] *= sg;
   }
 }
 
@@ -602,6 +899,65 @@ extern "C" int so_tpv_decode_bwd_input(float* g0, const float* a0, int64_t n, vo
   if (misaligned16(g0) || misaligned16(a0)) return SO_ERR_INVALID_ARG;
   if (n == 0) return SO_OK;
   decode_bwd_input_kernel<<<bwd_grid(n / 4), 256, 0, (cudaStream_t)stream>>>(reinterpret_cast<float4*>(g0), reinterpret_cast<const float4*>(a0), n / 4);
+  note_launch(1);
+  return check_launch();
+}
+
+extern "C" int so_bev_decode(const float* bev, int32_t C, const float* w1, const float* b1, const float* w2, const float* b2,
+                             const so_volume_desc* d, float* vol_sdf, float* vol_feat, void* stream) {
+  if (!bev || !w1 || !b1 || !w2 || !b2 || !vol_sdf) return SO_ERR_INVALID_ARG;
+  int rc = validate_volume(d);
+  if (rc) return rc;
+  if (d->n_feat > 0 && !vol_feat) return SO_ERR_INVALID_ARG;
+  if (C != 96) return SO_ERR_UNSUPPORTED;
+  if ((int64_t)d->Z * (1 + d->n_feat) > kBevMaxCols) return SO_ERR_UNSUPPORTED;
+  if (misaligned16(bev) || misaligned16(w1) || misaligned16(w2)) return SO_ERR_INVALID_ARG;
+  cudaStream_t st = (cudaStream_t)stream;
+  const long long cols = (long long)d->H * d->W;
+  if (d->zpitch > d->Z) {
+    long long n = cols * (d->zpitch - d->Z);
+    zero_pad_kernel<<<(unsigned)ceil_div64(n, 256), 256, 0, st>>>(vol_sdf, cols, d->Z, d->zpitch);
+    note_launch(1);
+  }
+  const BevSmem L = bev_smem(96);
+  static PerDeviceOnce attr;
+  if ((rc = attr.run([&L] {
+         return check_cuda(cudaFuncSetAttribute(bev_decode_tc_kernel<96>, cudaFuncAttributeMaxDynamicSharedMemorySize, L.total));
+       })))
+    return rc;
+  const int n_tiles = (int)ceil_div64(cols, kBM), sms = num_sms(), grid = n_tiles < sms ? n_tiles : sms;
+  bev_decode_tc_kernel<96><<<grid, kBevThreads, L.total, st>>>(bev, w1, b1, w2, b2, (int)cols, d->Z, 1 + d->n_feat, d->zpitch,
+                                                              d->feat_pitch, vol_sdf, vol_feat, n_tiles);
+  note_launch(1);
+  return check_launch();
+}
+
+extern "C" int so_bev_decode_bwd_gather(const float* g_vol_sdf, const float* g_vol_feat, const so_volume_desc* d, int64_t row_begin,
+                                        int64_t row_count, float* g_out, void* stream) {
+  if (!g_out) return SO_ERR_INVALID_ARG;
+  int rc = validate_volume(d);
+  if (rc) return rc;
+  if (row_begin < 0 || row_count < 0 || row_begin + row_count > (int64_t)d->H * d->W) return SO_ERR_INVALID_ARG;
+  const long long n = row_count * (long long)d->Z * (1 + d->n_feat);
+  if (n == 0) return SO_OK;
+  bev_decode_bwd_gather_kernel<<<bwd_grid(n), 256, 0, (cudaStream_t)stream>>>(g_vol_sdf, d->n_feat ? g_vol_feat : nullptr, d->Z,
+                                                                             d->zpitch, 1 + d->n_feat, d->feat_pitch, row_begin, n, g_out);
+  note_launch(1);
+  return check_launch();
+}
+
+extern "C" int so_bev_decode_bwd_features(const float* bev, int64_t n, float* a0, void* stream) {
+  if (!bev || !a0 || n < 0) return SO_ERR_INVALID_ARG;
+  if (n == 0) return SO_OK;
+  bev_decode_bwd_features_kernel<<<bwd_grid(n), 256, 0, (cudaStream_t)stream>>>(bev, n, a0);
+  note_launch(1);
+  return check_launch();
+}
+
+extern "C" int so_bev_decode_bwd_hidden(float* z1_a1, float* g1, int64_t n, void* stream) {
+  if (!z1_a1 || !g1 || n < 0) return SO_ERR_INVALID_ARG;
+  if (n == 0) return SO_OK;
+  bev_decode_bwd_hidden_kernel<<<bwd_grid(n), 256, 0, (cudaStream_t)stream>>>(z1_a1, g1, n);
   note_launch(1);
   return check_launch();
 }

@@ -265,32 +265,45 @@ linear_3xtf32_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_con
       uint32_t ah0[16], al0[16], ah1_[kTwoSets ? 16 : 1], al1_[kTwoSets ? 16 : 1];
       uint32_t* ah1 = kTwoSets ? ah1_ : ah0;
       uint32_t* al1 = kTwoSets ? al1_ : al0;
-      mbar_wait(my_full + s, ph);
-      load_split_frag(my_ring + s * kStageBytes, frag_row, g, t, ah0, al0);
-      __syncwarp();
-      if (lane == 0) mbar_arrive(my_empty + s);            // the stage is in registers: the producer may refill it
-      ring_advance(s, ph, half);
+      // A stage goes back to the producer only once the MMAs that took their A fragments from it have completed.  The
+      // fragments are read with generic loads and the next TMA write into the stage is an async-proxy write: releasing
+      // the stage right after the loads were issued let that write overtake loads still in flight (wrong rows in a few
+      // m-tiles of long runs).  An MMA cannot complete before its register operands have arrived.
+      int pending = -1;                                    // two sets: the stage of the MMA group still in flight
+      auto release = [&](int slot) {
+        if (slot < 0) return;
+        __syncwarp();
+        if (lane == 0) mbar_arrive(my_empty + slot);
+      };
+      auto fetch = [&](uint32_t* ah, uint32_t* al) {
+        mbar_wait(my_full + s, ph);
+        load_split_frag(my_ring + s * kStageBytes, frag_row, g, t, ah, al);
+        const int slot = s;
+        ring_advance(s, ph, half);
+        return slot;
+      };
+      auto issue = [&](uint32_t* ah, uint32_t* al, int a, int slot) {
+        mma_atom_rs<BN>(acc, ah, al, whi + a * BN * 128, wlo + a * BN * 128, accum);
+        if constexpr (kTwoSets) {
+          wg_wait1();                                      // atom a - 1 is done: its set and its stage are free
+          release(pending);
+          pending = slot;
+        } else {
+          wg_wait0();                                      // atom a is done: the one set and its stage are free
+          release(slot);
+        }
+      };
+      int cur = fetch(ah0, al0);
       for (int a = 0; a < KA; a += 2) {
-        mma_atom_rs<BN>(acc, ah0, al0, whi + a * BN * 128, wlo + a * BN * 128, accum);
-        if constexpr (kTwoSets) wg_wait1(); else wg_wait0();   // atom a - 1 is done: set 1 is free
+        issue(ah0, al0, a, cur);
         if (a + 1 < KA) {
-          mbar_wait(my_full + s, ph);
-          load_split_frag(my_ring + s * kStageBytes, frag_row, g, t, ah1, al1);
-          __syncwarp();
-          if (lane == 0) mbar_arrive(my_empty + s);
-          ring_advance(s, ph, half);
-          mma_atom_rs<BN>(acc, ah1, al1, whi + (a + 1) * BN * 128, wlo + (a + 1) * BN * 128, accum);
-          if constexpr (kTwoSets) wg_wait1(); else wg_wait0();  // atom a is done: set 0 is free
-          if (a + 2 < KA) {
-            mbar_wait(my_full + s, ph);
-            load_split_frag(my_ring + s * kStageBytes, frag_row, g, t, ah0, al0);
-            __syncwarp();
-            if (lane == 0) mbar_arrive(my_empty + s);
-            ring_advance(s, ph, half);
-          }
+          cur = fetch(ah1, al1);
+          issue(ah1, al1, a + 1, cur);
+          if (a + 2 < KA) cur = fetch(ah0, al0);
         }
       }
       wg_wait0();
+      release(pending);
       fence_regs<BN / 2>(acc);
     } else {
       for (int a = 0; a < KA; ++a) {

@@ -321,6 +321,9 @@ class ShardedLifter:
 
     def __init__(self, encoder):
         from .encoder import POST_NORM_ORDER
+        if not hasattr(encoder, 'tpv_size'):
+            raise NotImplementedError('ShardedLifter: query-sharded lifting covers the TPV encoder; %s is not sharded'
+                                      % type(encoder).__name__)
         self.enc = encoder
         H, W, Z = encoder.tpv_size
         self.sizes = [H * W, Z * H, W * Z]
@@ -397,6 +400,8 @@ def decode_sharded(head, representation, group=None):
     block); the field then holds the first H rows as usual."""
     from . import ops as ops_
     f = head.model.field
+    if not f.tpv:
+        raise NotImplementedError('decode_sharded: the voxel-sharded decode covers the TPV field; tpv=False is not sharded')
     world = dist.get_world_size(group) if dist.is_initialized() else 1
     rank = dist.get_rank(group) if dist.is_initialized() else 0
     hw, zh, wz = representation

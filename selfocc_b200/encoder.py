@@ -120,6 +120,14 @@ def _focal_scale(metas, n_cam, device):
 
 
 # --------------------------------------------------------------------------- positional encoding (A10)
+def _freq_features(m, nf):
+    """[A, B, 2] range-normalised plane coordinates -> [A*B, 4 nf]: sin / cos at pi 2^-1 .. pi 2^(nf-2), channel order of
+    stack([sin, cos], -1).flatten(-3) (tpvformer_pos_embed.py:16-58, bevformer_pos_embed.py:20-28)."""
+    freqs = math.pi * (2.0 ** torch.arange(-1, nf - 1, dtype=torch.float))
+    ang = m.unsqueeze(-1) * freqs                                          # [A, B, 2, nf]
+    return torch.stack([ang.sin(), ang.cos()], -1).flatten(-3).flatten(0, 1)
+
+
 @MODELS.register_module()
 class TPVPositionalEncoding(nn.Module):
     """tpvformer_pos_embed.py:16-58: sin/cos of range-normalised plane metres -> Linear per plane."""
@@ -131,15 +139,29 @@ class TPVPositionalEncoding(nn.Module):
         norm = {'x': (r[0], r[3] - r[0]), 'y': (r[1], r[4] - r[1]), 'z': (r[2], r[5] - r[2])}
         for name, meter, axes, nf in zip(('hw', 'zh', 'wz'), tpv_meters, ('xy', 'yz', 'xz'), num_freqs):
             m = torch.stack([(meter[..., i] - norm[a][0]) / norm[a][1] for i, a in enumerate(axes)], -1)
-            freqs = math.pi * (2.0 ** torch.arange(-1, nf - 1, dtype=torch.float))
-            ang = m.unsqueeze(-1) * freqs                                  # [A, B, 2, nf]
-            feat = torch.stack([ang.sin(), ang.cos()], -1).flatten(-3).flatten(0, 1)
-            self.register_buffer(name + '_freq_feat', feat, False)
+            self.register_buffer(name + '_freq_feat', _freq_features(m, nf), False)
             setattr(self, 'position_layer_' + name, nn.Linear(4 * nf, embed_dims))
 
     def forward(self):
         return [self.position_layer_hw(self.hw_freq_feat), self.position_layer_zh(self.zh_freq_feat),
                 self.position_layer_wz(self.wz_freq_feat)]
+
+
+@MODELS.register_module()
+class BEVPositionalEncoding(nn.Module):
+    """bevformer_pos_embed.py:7-35: sin/cos of the range-normalised BEV cell metres -> Linear.  ``bev_meter`` [H, W, 2]
+    (x, y) metres; ``tot_range`` the point-cloud range (a scalar t stands for [-t, -t, 0, t, t, 0])."""
+
+    def __init__(self, num_freqs, embed_dims, bev_meter, tot_range, init_cfg=None):
+        super().__init__()
+        r = [float(v) for v in tot_range] if isinstance(tot_range, (list, tuple)) else \
+            [-1.0 * tot_range, -1.0 * tot_range, 0., tot_range, tot_range, 0.]
+        m = torch.stack([(bev_meter[..., 0] - r[0]) / (r[3] - r[0]), (bev_meter[..., 1] - r[1]) / (r[4] - r[1])], -1)
+        self.register_buffer('freq_feat', _freq_features(m, num_freqs), False)
+        self.position_layer = nn.Linear(4 * num_freqs, embed_dims)
+
+    def forward(self):
+        return self.position_layer(self.freq_feat)
 
 
 # --------------------------------------------------------------------------- attention modules
@@ -318,6 +340,24 @@ class CrossViewHybridAttention(_DeformBase):
         if not self.batch_first:
             out = out.permute(1, 0, 2)
         return self.dropout(out) + identity
+
+
+class MultiScaleDeformableAttention(CrossViewHybridAttention):
+    """mmcv.ops.MultiScaleDeformableAttention (the BEV layer's self-attention): parameter names, init (point i of the ring
+    scaled by i + 1) and ``dropout(output_proj(.)) + identity`` are CrossViewHybridAttention's, which differs from it only in
+    taking one reference point per point; here reference_points [bs, Q, L, 2] is one per query and level, broadcast over the
+    points.  BEVFormerLayer runs this attention's batch-1 arithmetic itself (TPVFormerLayer.forward_rows)."""
+
+    def forward(self, query, key=None, value=None, identity=None, query_pos=None, key_padding_mask=None,
+                reference_points=None, spatial_shapes=None, level_start_index=None, **kwargs):
+        if reference_points.shape[-1] != 2:
+            raise ValueError('Last dim of reference_points must be 2, but get %d instead.' % reference_points.shape[-1])
+        return super().forward(query, key, value, identity, query_pos, key_padding_mask, reference_points[..., None, :],
+                               spatial_shapes, level_start_index, **kwargs)
+
+
+if not HAVE_MMENGINE:  # mmcv registers its own MultiScaleDeformableAttention when present
+    MODELS.register_module(name='MultiScaleDeformableAttention', module=MultiScaleDeformableAttention)
 
 
 @MODELS.register_module()
@@ -614,14 +654,15 @@ class TPVFormerLayer(nn.Module):
         # image cross-attention, one plane at a time (tpvformer/attention/image_cross_attention.py:83-93); the three planes
         # project the same image features with their own value_proj: one GEMM, three column slices
         feat = value[:, :, 0].reshape(-1, value.shape[-1])
-        vps = [a.deformable_attention.value_proj for a in ca.attns]
+        attns = getattr(ca, 'attns', (ca,))                 # TPVCrossAttention: one per plane; BEVCrossAttention: itself
+        vps = [a.deformable_attention.value_proj for a in attns]
         vrows = fast_linear_cat(ca, '_so_value3', vps, feat)[1] if _fusable(vps, feat) else None
         x = q.new_empty(q.shape)                      # each plane's output_proj writes its own row range: no torch.cat
         o0 = 0
         for i, (b, c) in enumerate(slices):
             if c == 0:
                 continue
-            att = ca.attns[i]
+            att = attns[i]
             da = att.deformable_attention
             qi = q[o0:o0 + c]
             v = vrows[i] if vrows is not None else fast_linear(da.value_proj, feat)
@@ -665,9 +706,10 @@ class TPVFormerLayer(nn.Module):
         # image cross-attention, one plane at a time, each on its own rows of q
         n_cam, nv = value.shape[0], value.shape[1]
         feat = value[:, :, 0]
+        attns = getattr(ca, 'attns', (ca,))
         parts, o0 = [], 0
         for i, (b, c) in enumerate(slices):
-            att = ca.attns[i]
+            att = attns[i]
             da = att.deformable_attention
             qi = q[o0:o0 + c]
             v = train_linear(da.value_proj, feat).view(n_cam, nv, da.num_heads, -1)
@@ -691,6 +733,52 @@ class TPVFormerLayer(nn.Module):
         return self.norms[2](out[None])[0]
 
 
+@MODELS.register_module()
+class BEVFormerLayer(TPVFormerLayer):
+    """bevformer_encoder_layer.py:10-216: the TPV layer on one plane.  At batch 1 in CUDA fp32 (post-norm, no mask) it runs
+    TPVFormerLayer.forward_rows / forward_rows_train with the BEV plane as the only plane and the BEVCrossAttention as the
+    only image cross-attention; otherwise the modules' own forwards in operation order, as the reference."""
+
+    def forward(self, query, key=None, value=None, bev_pos=None, ref_2d=None, spatial_shapes=None, level_start_index=None,
+                reference_points_cams=None, bev_masks=None, bev_size=None, bev_vis=None, **kwargs):
+        """query [bs, H*W, C]; ref_2d [bs, H*W, 1, 2] (the self-attention's reference point per query); reference_points_cams
+        [N, bs, H*W, D, 2] / bev_masks [N, bs, H*W, D]; bev_vis [N, H*W] uint8 (optional: derived from bev_masks)."""
+        H, W = bev_size
+        dev = query.device
+        ss = torch.tensor([[H, W]], device=dev)                     # bevformer_encoder_layer.py:168-169
+        lsi = torch.tensor([0], device=dev)
+        routine = self._row_routine(query, value, kwargs)
+        if routine is not None:
+            if bev_vis is None:
+                bev_vis = (bev_masks[:, 0].sum(-1) > 0).to(torch.uint8)
+            sa = self.attentions[0]
+            ref = ref_2d[0][:, :, None, :].expand(-1, -1, sa.num_points, -1)     # [HW, 1, P, 2]: the point of every sample
+            out = routine(query[0], query[0], bev_pos[0], ref, [(0, H * W)], value, spatial_shapes, level_start_index,
+                          (ss, lsi), [reference_points_cams], [bev_vis])
+            return out[None]
+        norm_i = attn_i = ffn_i = 0
+        identity = query
+        for op in self.operation_order:
+            if op == 'self_attn':
+                query = self.attentions[attn_i](query, query, query, identity if self.pre_norm else None, query_pos=bev_pos,
+                                                reference_points=ref_2d, spatial_shapes=ss, level_start_index=lsi, **kwargs)
+                attn_i += 1
+                identity = query
+            elif op == 'norm':
+                query = self.norms[norm_i](query)
+                norm_i += 1
+            elif op == 'cross_attn':
+                query = self.attentions[attn_i](query, key, value, identity if self.pre_norm else None,
+                                                spatial_shapes=spatial_shapes, level_start_index=level_start_index,
+                                                reference_points_cams=reference_points_cams, bev_masks=bev_masks, **kwargs)
+                attn_i += 1
+                identity = query
+            elif op == 'ffn':
+                query = self.ffns[ffn_i](query, identity if self.pre_norm else None)
+                ffn_i += 1
+        return query
+
+
 def _row_dropout(drop, x, full_shape, rows):
     """nn.Dropout ``drop`` on the rows ``x`` of a tensor of shape ``full_shape``.  When ``x`` is the whole tensor this is
     ``drop(x)``.  Otherwise the mask is drawn for the whole tensor with the op nn.Dropout runs on a CUDA tensor
@@ -707,8 +795,58 @@ def _row_dropout(drop, x, full_shape, rows):
     return x * (rows(mask) * (1.0 / (1.0 - p)))
 
 
+class _LiftingEncoder(nn.Module):
+    """The image side the TPV and BEV encoders share: flattening the multi-scale features with their camera / level
+    embeddings (``cams_embeds``, ``level_embeds``) and projecting pillar tables of 3-D reference points into the cameras."""
+
+    def project_tables(self, tables, metas, device):
+        """point_sampling of each [D, Q, 3] metre table (bevformer/utils.py:116-206) -> lists of uv [N,B,Q,D,2],
+        mask [N,B,Q,D] uint8, vis [N,Q] uint8.  B must be 1 (as everywhere in the reference head).  Frames from the
+        reference's data wrapper carry metas[0]['focal_ratios_x' / '_y'] (RandomScaleImageMultiViewImage): uv is rescaled
+        per camera after the frustum test (bevformer/utils.py:198-204), see _focal_scale."""
+        if 'img_augmentation' in metas[0]:
+            raise NotImplementedError("the post_rots / post_trans branch of point_sampling (metas['img_augmentation']) is not "
+                                      'implemented: no shipped data pipeline produces it')
+        l2i = _metas_matrix(metas, 'lidar2img', device)
+        assert l2i.shape[0] == 1, 'only bs = 1 is supported (the reference head asserts the same)'
+        scale_xy = _focal_scale(metas, l2i.shape[1], device)
+        shp = metas[0]['img_shape']
+        uvs, masks, vises = [], [], []
+        for ref in tables:
+            uv, mask, vis = ops.point_sampling(ref, l2i[0].contiguous(), (shp[0], shp[1]), scale_xy)
+            uvs.append(uv[:, None])
+            masks.append(mask[:, None])
+            vises.append(vis)
+        return uvs, masks, vises
+
+    def flatten_features(self, img_feats):
+        """A3: [B,N,C,h,w] x L -> [N, sum(hw), B, C] with camera + level embeddings (tpvformer_encoder.py:261-277)."""
+        f0 = img_feats[0]
+        if f0.is_cuda and f0.dtype == torch.float32 and f0.shape[0] == 1 and all(f.is_contiguous() for f in img_feats) \
+                and not _needs_grad(self.cams_embeds, *img_feats):
+            shapes = tuple((f.shape[3], f.shape[4]) for f in img_feats)  # fused transposing pass (so_flatten_level)
+            key = (shapes, f0.device)
+            if getattr(self, '_shape_key', None) != key:                 # the two tiny int64 tables are per-resolution constants
+                spatial_shapes = torch.as_tensor(shapes, dtype=torch.long, device=f0.device)
+                level_start_index = torch.cat((spatial_shapes.new_zeros((1,)), spatial_shapes.prod(1).cumsum(0)[:-1]))
+                self._shape_key, self._shape_val = key, (spatial_shapes, level_start_index)
+            spatial_shapes, level_start_index = self._shape_val
+            return ops.flatten_levels(img_feats, self.cams_embeds.detach().contiguous(), self.level_embeds.detach().contiguous()), \
+                spatial_shapes, level_start_index
+        feats, shapes = [], []
+        for lvl, feat in enumerate(img_feats):
+            bs, num_cam, c, h, w = feat.shape
+            shapes.append((h, w))
+            f = feat.flatten(3).permute(1, 0, 3, 2)
+            feats.append(f + self.cams_embeds[:, None, None, :] + self.level_embeds[None, None, lvl:lvl + 1, :])
+        dev = img_feats[0].device
+        spatial_shapes = torch.as_tensor(shapes, dtype=torch.long, device=dev)
+        level_start_index = torch.cat((spatial_shapes.new_zeros((1,)), spatial_shapes.prod(1).cumsum(0)[:-1]))
+        return torch.cat(feats, 2).permute(0, 2, 1, 3).contiguous(), spatial_shapes, level_start_index
+
+
 @MODELS.register_module()
-class TPVFormerEncoder(nn.Module):
+class TPVFormerEncoder(_LiftingEncoder):
     """A2/A3.  tpvformer_encoder.py:19-290."""
 
     def __init__(self, mapping_args, embed_dims=128, num_cams=6, num_feature_levels=4, positional_encoding=None,
@@ -766,24 +904,9 @@ class TPVFormerEncoder(nn.Module):
         nn.init.normal_(self.cams_embeds)
 
     def project_reference_points(self, metas, device):
-        """A4: three point_sampling calls (tpvformer_encoder.py:205-210) -> per plane uv [N,B,Q,D,2],
-        mask [N,B,Q,D] uint8, vis [N,Q] uint8.  B must be 1 (as everywhere in the reference head).  Frames from the
-        reference's data wrapper carry metas[0]['focal_ratios_x' / '_y'] (RandomScaleImageMultiViewImage): uv is rescaled
-        per camera after the frustum test (bevformer/utils.py:198-204), see _focal_scale."""
-        if 'img_augmentation' in metas[0]:
-            raise NotImplementedError("the post_rots / post_trans branch of point_sampling (metas['img_augmentation']) is not "
-                                      'implemented: no shipped data pipeline produces it')
-        l2i = _metas_matrix(metas, 'lidar2img', device)
-        assert l2i.shape[0] == 1, 'only bs = 1 is supported (the reference head asserts the same)'
-        scale_xy = _focal_scale(metas, l2i.shape[1], device)
-        shp = metas[0]['img_shape']
-        uvs, masks, vises = [], [], []
-        for ref in (self.ref_3d_hw, self.ref_3d_zh, self.ref_3d_wz):
-            uv, mask, vis = ops.point_sampling(ref, l2i[0].contiguous(), (shp[0], shp[1]), scale_xy)
-            uvs.append(uv[:, None])
-            masks.append(mask[:, None])
-            vises.append(vis)
-        return uvs, masks, vises
+        """A4: three point_sampling calls (tpvformer_encoder.py:205-210) -> per plane uv [N,B,Q,D,2], mask [N,B,Q,D] uint8,
+        vis [N,Q] uint8 (project_tables)."""
+        return self.project_tables((self.ref_3d_hw, self.ref_3d_zh, self.ref_3d_wz), metas, device)
 
     def forward_layers(self, tpv_query, key, value, tpv_pos=None, spatial_shapes=None, level_start_index=None,
                        img_metas=None, **kwargs):
@@ -797,31 +920,6 @@ class TPVFormerEncoder(nn.Module):
                               tpv_size=self.tpv_size, tpv_vis=vises,
                               tpv_levels=(self.tpv_spatial_shapes, self.tpv_level_start), **kwargs)
         return tpv_query
-
-    def flatten_features(self, img_feats):
-        """A3: [B,N,C,h,w] x L -> [N, sum(hw), B, C] with camera + level embeddings (tpvformer_encoder.py:261-277)."""
-        f0 = img_feats[0]
-        if f0.is_cuda and f0.dtype == torch.float32 and f0.shape[0] == 1 and all(f.is_contiguous() for f in img_feats) \
-                and not _needs_grad(self.cams_embeds, *img_feats):
-            shapes = tuple((f.shape[3], f.shape[4]) for f in img_feats)  # fused transposing pass (so_flatten_level)
-            key = (shapes, f0.device)
-            if getattr(self, '_shape_key', None) != key:                 # the two tiny int64 tables are per-resolution constants
-                spatial_shapes = torch.as_tensor(shapes, dtype=torch.long, device=f0.device)
-                level_start_index = torch.cat((spatial_shapes.new_zeros((1,)), spatial_shapes.prod(1).cumsum(0)[:-1]))
-                self._shape_key, self._shape_val = key, (spatial_shapes, level_start_index)
-            spatial_shapes, level_start_index = self._shape_val
-            return ops.flatten_levels(img_feats, self.cams_embeds.detach().contiguous(), self.level_embeds.detach().contiguous()), \
-                spatial_shapes, level_start_index
-        feats, shapes = [], []
-        for lvl, feat in enumerate(img_feats):
-            bs, num_cam, c, h, w = feat.shape
-            shapes.append((h, w))
-            f = feat.flatten(3).permute(1, 0, 3, 2)
-            feats.append(f + self.cams_embeds[:, None, None, :] + self.level_embeds[None, None, lvl:lvl + 1, :])
-        dev = img_feats[0].device
-        spatial_shapes = torch.as_tensor(shapes, dtype=torch.long, device=dev)
-        level_start_index = torch.cat((spatial_shapes.new_zeros((1,)), spatial_shapes.prod(1).cumsum(0)[:-1]))
-        return torch.cat(feats, 2).permute(0, 2, 1, 3).contiguous(), spatial_shapes, level_start_index
 
     def _tpv_pos(self):
         """Positional embeddings depend on the weights only: recomputed per call under autograd (training), cached per
@@ -904,3 +1002,77 @@ class TPVFormerEncoder(nn.Module):
         tpv_embed = self.forward_layers(representation, feat_flatten, feat_flatten, tpv_pos=tpv_pos,
                                         spatial_shapes=spatial_shapes, level_start_index=level_start_index, img_metas=metas)
         return {'representation': list(tpv_embed)}
+
+
+@MODELS.register_module()
+class BEVFormerEncoder(_LiftingEncoder):
+    """bevformer_encoder.py:17-223: one BEV plane of H*W queries, BEVFormerLayer layers."""
+
+    def __init__(self, mapping_args, embed_dims=128, num_cams=6, num_feature_levels=4, positional_encoding=None,
+                 num_points_cross=32, num_points_self=16, transformerlayers=None, num_layers=None, init_cfg=None):
+        super().__init__()
+        self.embed_dims, self.num_feature_levels, self.num_cams = embed_dims, num_feature_levels, num_cams
+        self.mapping = GridMeterMapping(**mapping_args)
+        H, W = self.mapping.size_h, self.mapping.size_w
+        f = lambda n: torch.arange(n, dtype=torch.float)
+        bev_grid = torch.stack([f(H)[:, None].expand(-1, W), f(W)[None].expand(H, -1)], -1)     # [H, W, (h, w)]
+        pe = dict(positional_encoding)
+        pe['bev_meter'] = self.mapping.grid2meter(bev_grid)
+        self.positional_encoding = build_positional_encoding(pe)
+        self.bev_size = [H, W]
+        if isinstance(transformerlayers, dict):
+            transformerlayers = [copy.deepcopy(transformerlayers) for _ in range(num_layers)]
+        assert isinstance(transformerlayers, (list, tuple)) and len(transformerlayers) == num_layers
+        self.num_layers = num_layers
+        self.layers = nn.ModuleList([build_transformer_layer(copy.deepcopy(c)) for c in transformerlayers])
+        self.pre_norm = self.layers[0].pre_norm
+        self.level_embeds = nn.Parameter(torch.randn(num_feature_levels, embed_dims))
+        self.cams_embeds = nn.Parameter(torch.randn(num_cams, embed_dims))
+        self.num_points_cross, self.num_points_self = num_points_cross, num_points_self
+        # pillars of the image cross-attention: the TPV hw plane's table (bevformer_encoder.py:106-112)
+        self.register_buffer('ref_3d', _pillar_tables(self.mapping, [num_points_cross] * 3)[0], False)
+        # the self-attention's reference point, (h / (H - 1), w / (W - 1)) as mmcv's (x, y) (bevformer_encoder.py:114-117)
+        self.register_buffer('ref_2d', torch.stack([bev_grid[..., 0] / (H - 1), bev_grid[..., 1] / (W - 1)], -1), False)
+        self.query_shard = None
+
+    def init_weights(self):
+        """bevformer_encoder.py:119-133."""
+        for p in self.parameters():
+            if p.dim() > 1:
+                nn.init.xavier_uniform_(p)
+        for m in self.modules():
+            if isinstance(m, BEVCrossAttention):
+                m.init_weight()
+            elif isinstance(m, (BEVDeformableAttention, CrossViewHybridAttention)):
+                m.init_weights()
+        nn.init.normal_(self.level_embeds)
+        nn.init.normal_(self.cams_embeds)
+
+    def _bev_pos(self):
+        """The positional embedding [H*W, C]: recomputed under autograd, cached per parameter version otherwise."""
+        pe = self.positional_encoding
+        ws = [pe.position_layer.weight, pe.position_layer.bias]
+        if torch.is_grad_enabled() and any(w.requires_grad for w in ws):
+            return pe()
+        key = tuple((w._version, w.data_ptr()) for w in ws)
+        if getattr(self, '_pos_key', None) != key:
+            with torch.no_grad():
+                self._pos_key, self._pos_val = key, pe()
+        return self._pos_val
+
+    def forward(self, representation, ms_img_feats=None, metas=None, **kwargs):
+        if getattr(self, 'query_shard', None) is not None and self.query_shard[1] > 1:
+            raise NotImplementedError('query_shard: the query-sharded training step covers the TPV encoder; BEVFormerEncoder '
+                                      'is not sharded')
+        bs = representation.shape[0]
+        pos = self._bev_pos()[None]
+        bev_pos = pos if bs == 1 else pos.repeat(bs, 1, 1)
+        feat, spatial_shapes, level_start_index = self.flatten_features(ms_img_feats)
+        uvs, masks, vises = self.project_tables((self.ref_3d,), metas, feat.device)
+        ref_2d = self.ref_2d.reshape(1, -1, 1, 2).expand(bs, -1, -1, -1)
+        q = representation
+        for layer in self.layers:
+            q = layer(q, feat, feat, bev_pos=bev_pos, ref_2d=ref_2d, spatial_shapes=spatial_shapes,
+                      level_start_index=level_start_index, reference_points_cams=uvs[0], bev_masks=masks[0],
+                      bev_size=self.bev_size, bev_vis=vises[0], **kwargs)
+        return {'representation': q}

@@ -127,13 +127,16 @@ class _Deviation(nn.Module):
 
 
 class _SDFField(nn.Module):
-    """TPV SDF field: per-frame decoded volume + trilinear queries (SURVEY.md rows B5, B7, B8, B12).
-    Parameter layout follows the in-repo analogue bev_nerf.py:62-71 (``density_net.{1,3}``)."""
+    """SDF field: per-frame decoded volume + trilinear queries (SURVEY.md rows B5, B7, B8, B12).
+    Parameter layout follows the in-repo analogue bev_nerf.py:62-71 (``density_net.{1,3}``).  ``tpv``: the representation
+    is the three TPV planes (one MLP output row per voxel) or, False, one BEV plane [1, H*W, C] whose MLP emits the
+    Z * (1 + color_dims) values of a whole pillar (column z * Cf + c = voxel z, channel c).  Both decode into the same
+    volume layout, so everything downstream of the decode is shared."""
 
     def __init__(self, mapping_args, embed_dims, color_dims, density_layers, sh_deg, sh_act, beta_init, tpv):
         super().__init__()
-        if not tpv:
-            raise NotImplementedError('tpv=False (single BEV plane decode) is not used by the target configs')
+        if not tpv and embed_dims != 96:
+            raise NotImplementedError('tpv=False: the BEV decode kernel implements embed_dims = 96, got %d' % embed_dims)
         if density_layers != 2:
             raise NotImplementedError('density_layers=%d: the fused decode kernel implements the 2-layer MLP' % density_layers)
         if sh_deg != 0:
@@ -141,20 +144,35 @@ class _SDFField(nn.Module):
         if color_dims not in (0,) and color_dims < 3:
             raise ValueError('color_dims must be 0 or >= 3')
         self.mapping = GridMeterMapping(**mapping_args)
-        self.embed_dims, self.color_dims, self.sh_act = embed_dims, color_dims, sh_act
+        self.embed_dims, self.color_dims, self.sh_act, self.tpv = embed_dims, color_dims, sh_act, tpv
+        n_out = (1 + color_dims) * (1 if tpv else self.mapping.size_d)
         self.density_net = nn.Sequential(nn.Softplus(), nn.Linear(embed_dims, embed_dims), nn.Softplus(),
-                                         nn.Linear(embed_dims, 1 + color_dims))
+                                         nn.Linear(embed_dims, n_out))
         self.deviation_network = _Deviation(beta_init)
         self.desc = self.mapping.volume_desc(color_dims)
         self.vol_sdf = self.vol_feat = None
         self._pack = None
 
-    def pre_compute_density_color(self, representation):
-        hw, zh, wz = representation
-        assert hw.shape[0] == 1, 'only support bs = 1 currently'
+    def decode(self, representation, train=False):
+        """The representation -> (vol_sdf, vol_feat): the fused decode for prepare / forward_occ, its autograd form for the
+        training forward (``train``; vol_feat is then an empty tensor when no features are decoded)."""
         l1, l2 = self.density_net[1], self.density_net[3]
-        self.vol_sdf, self.vol_feat = ops.tpv_decode(hw[0].contiguous(), zh[0].contiguous(), wz[0].contiguous(),
-                                                     l1.weight, l1.bias, l2.weight, l2.bias, self.desc)
+        w = (l1.weight, l1.bias, l2.weight, l2.bias)
+        if self.tpv:
+            hw, zh, wz = representation
+            assert hw.shape[0] == 1, 'only support bs = 1 currently'
+            if train:
+                return ops.TPVDecodeFunction.apply(hw[0], zh[0], wz[0], *w, self.desc)
+            return ops.tpv_decode(hw[0].contiguous(), zh[0].contiguous(), wz[0].contiguous(), *w, self.desc)
+        bev = representation
+        assert torch.is_tensor(bev) and bev.dim() == 3, 'tpv=False: the representation is one BEV plane [bs, H*W, C]'
+        assert bev.shape[0] == 1, 'only support bs = 1 currently'
+        if train:
+            return ops.BEVDecodeFunction.apply(bev[0], *w, self.desc)
+        return ops.bev_decode(bev[0].contiguous(), *w, self.desc)
+
+    def pre_compute_density_color(self, representation):
+        self.vol_sdf, self.vol_feat = self.decode(representation)
         self._pack = None
 
     def render_pack(self):

@@ -23,10 +23,7 @@ def forward_train(head, representation, metas=None, jitter=None, bkgd_rand=None,
     jitter and the random background are drawn for all rays and sliced; the uniform_sdf lattice shift and the encoder's
     dropout masks are then drawn identically.  An explicit ``jitter`` / ``bkgd_rand`` is this rank's slice."""
     f = head.model.field
-    hw, zh, wz = representation
-    assert hw.shape[0] == 1, 'only support bs = 1 currently'
-    l1, l2 = f.density_net[1], f.density_net[3]
-    vol_sdf, vol_feat = ops.TPVDecodeFunction.apply(hw[0], zh[0], wz[0], l1.weight, l1.bias, l2.weight, l2.bias, f.desc)
+    vol_sdf, vol_feat = f.decode(representation, train=True)
     vol_feat = vol_feat if f.desc.n_feat else None
     f.vol_sdf, f.vol_feat = vol_sdf.detach(), (vol_feat.detach() if vol_feat is not None else None)
     f.vol_sdf_live, f.vol_feat_live = vol_sdf, vol_feat           # autograd-connected views for get_uniform_sdf

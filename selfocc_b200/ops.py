@@ -57,6 +57,26 @@ def tpv_decode(tpv_hw, tpv_zh, tpv_wz, w1, b1, w2, b2, desc, rows=None, out=None
     return vol_sdf, vol_feat
 
 
+def bev_decode(bev, w1, b1, w2, b2, desc):
+    """tpv=False decode: bev [H*W, C] + MLP (w2 [Z * (1 + n_feat), C]) -> (vol_sdf [H,W,zpitch], vol_feat [H,W,Z,feat_pitch] | None),
+    the layout tpv_decode writes."""
+    lib = _lib.load()
+    for n, t in (('bev', bev), ('w1', w1), ('b1', b1), ('w2', w2), ('b2', b2)):
+        _chk(t, name=n)
+    Cc = bev.shape[-1]
+    assert bev.numel() == desc.H * desc.W * Cc, 'bev shape does not match the mapping'
+    assert w1.shape == (Cc, Cc) and w2.shape == (desc.Z * (1 + desc.n_feat), Cc)
+    dev = bev.device
+    vol_sdf = torch.empty(desc.H, desc.W, desc.zpitch, device=dev, dtype=torch.float32)
+    vol_feat = None
+    if desc.n_feat:
+        vol_feat = (torch.zeros if desc.feat_pitch > desc.n_feat else torch.empty)(
+            desc.H, desc.W, desc.Z, desc.feat_pitch, device=dev, dtype=torch.float32)
+    _lib.check(lib.so_bev_decode(_p(bev), Cc, _p(w1), _p(b1), _p(w2), _p(b2), C.byref(desc), _p(vol_sdf), _p(vol_feat), _stream()),
+               'so_bev_decode')
+    return vol_sdf, vol_feat
+
+
 # --------------------------------------------------------------------------------------- B1-B11
 def make_ray_desc(n_cam, grid=None, n_pix=None, ray_begin=0, ray_count=None, chunk_len=0):
     """grid = (ny, nx, sx, ox, sy, oy) for the in-kernel strided pixel grid, or n_pix with a pixel table."""
@@ -563,6 +583,61 @@ class TPVDecodeFunction(torch.autograd.Function):
             for i in range(4):
                 grads[3 + i] += gs[3 + i]
         return tuple(grads)
+
+
+def _matmul_wt(x, w):
+    """x @ w^T: the 3xTF32 GEMM where linear_supported allows the shape, cuBLAS otherwise."""
+    if linear_supported(w.shape[1], w.shape[0]):
+        hi, lo = split_tf32(w.contiguous())
+        return linear_3xtf32(x.contiguous(), hi, lo)
+    return x @ w.t()
+
+
+class BEVDecodeFunction(torch.autograd.Function):
+    """bev_decode with autograd (training form of the tpv=False field): (bev [H*W, C], w1, b1, w2, b2, desc) ->
+    (vol_sdf, vol_feat or an empty tensor).  Backward recomputes a0 / z1 / a1 in slabs of rows (nothing of the forward's
+    MLP is kept) and gathers the slab's [rows, Z * Cf] output gradient from the volume gradients (so_bev_decode_bwd_gather);
+    the products run through _matmul_wt, the weight-gradient reductions over the rows on cuBLAS (as TPVDecodeFunction)."""
+
+    SLAB_ROWS = 8192
+
+    @staticmethod
+    def forward(ctx, bev, w1, b1, w2, b2, desc):
+        ctx.desc = desc
+        ctx.save_for_backward(bev, w1, b1, w2, b2)
+        vs, vf = bev_decode(bev.contiguous(), w1.contiguous(), b1.contiguous(), w2.contiguous(), b2.contiguous(), desc)
+        return vs, (vf if vf is not None else vs.new_empty(0))
+
+    @staticmethod
+    @torch.autograd.function.once_differentiable
+    def backward(ctx, g_vs, g_vf):
+        lib = _lib.load()
+        bev, w1, b1, w2, b2 = [t.detach().contiguous() for t in ctx.saved_tensors]
+        d = ctx.desc
+        rows_total, Cc = bev.shape
+        g_vs = _chk(g_vs.contiguous(), name='g_vol_sdf') if g_vs is not None else None
+        g_vf = _chk(g_vf.contiguous(), name='g_vol_feat') if (g_vf is not None and d.n_feat) else None
+        w1_hi, w1_lo = split_tf32(w1)
+        g_bev = torch.empty_like(bev)
+        g_w1, g_b1, g_w2, g_b2 = (torch.zeros_like(t) for t in (w1, b1, w2, b2))
+        st = _stream()
+        for r0 in range(0, rows_total, BEVDecodeFunction.SLAB_ROWS):
+            n = min(rows_total, r0 + BEVDecodeFunction.SLAB_ROWS) - r0
+            a0 = torch.empty(n, Cc, device=bev.device)
+            _lib.check(lib.so_bev_decode_bwd_features(_p(bev[r0:r0 + n]), a0.numel(), _p(a0), st), 'so_bev_decode_bwd_features')
+            z1 = linear_3xtf32(a0, w1_hi, w1_lo, b1)
+            go = torch.empty(n, w2.shape[0], device=bev.device)
+            _lib.check(lib.so_bev_decode_bwd_gather(_p(g_vs), _p(g_vf), C.byref(d), r0, n, _p(go), st), 'so_bev_decode_bwd_gather')
+            g1 = _matmul_wt(go, w2.t())
+            _lib.check(lib.so_bev_decode_bwd_hidden(_p(z1), _p(g1), z1.numel(), st), 'so_bev_decode_bwd_hidden')
+            g_w2.addmm_(go.t(), z1)                                   # z1 now holds a1
+            g_b2.add_(go.sum(0))
+            g_w1.addmm_(g1.t(), a0)
+            g_b1.add_(g1.sum(0))
+            g0 = _matmul_wt(g1, w1.t())
+            _lib.check(lib.so_tpv_decode_bwd_input(_p(g0), _p(a0), g0.numel(), st), 'so_tpv_decode_bwd_input')
+            g_bev[r0:r0 + n] = g0
+        return g_bev, g_w1, g_b1, g_w2, g_b2, None
 
 
 # --------------------------------------------------------------------------------------- A6/A9 tensor-core projections
