@@ -28,10 +28,11 @@ extern "C" {
 #define SO_ERR_CUDA (-3)          /* a CUDA runtime call or launch failed; see so_last_cuda_error */
 #define SO_ERR_NO_DEVICE (-4)
 
-#define SO_ABI_VERSION 9   /* 2: so_render_train_forward gained pair_workspace; 3: packed render volume entry points;
+#define SO_ABI_VERSION 10  /* 2: so_render_train_forward gained pair_workspace; 3: packed render volume entry points;
                               4: backward of the fused attention cores; 5: the colour pack holds the SH-0 colour;
                               6: reprojection-loss statistics; 7: training-render sample probe;
-                              8: occupancy labels and confusion matrix; 9: per-sample loss-term means */
+                              8: occupancy labels and confusion matrix; 9: per-sample loss-term means;
+                              10: test hooks so_linear_force_ss / so_tpv_decode_force_simt removed */
 
 /* ABI version of the loaded library (compare with SO_ABI_VERSION). */
 int so_abi_version(void);
@@ -132,9 +133,6 @@ int so_bev_decode_bwd_gather(const float* g_vol_sdf, const float* g_vol_feat, co
                              int64_t row_count, float* g_out, void* stream);
 int so_bev_decode_bwd_features(const float* bev, int64_t n, float* a0, void* stream);
 int so_bev_decode_bwd_hidden(float* z1_a1, float* g1, int64_t n, void* stream);
-
-/* Test hook: force the fp32 SIMT decode kernel (default: the wgmma 3xTF32 kernel whenever C % 32 == 0). */
-int so_tpv_decode_force_simt(int on);
 
 /* ---------------------------------------------------------------------------------------
  * Ray set of one frame: n_cam cameras x rays_per_cam pixel rays, flattened (cam, ray)-major
@@ -343,9 +341,6 @@ int so_msda_backward(const float* value, const int64_t* spatial_shapes, const in
  * cross_view_hybrid_attention.py:79-86,118, tpvformer_encoder_layer.py:198-206).  w_hi / w_lo = so_split_tf32(w)
  * (w_hi = w with the low 13 mantissa bits cleared, w_lo = w - w_hi), computed once per weight.  K % 96 == 0, N even;
  * x, w_hi, w_lo 16-byte aligned (TMA), y and residual 8-byte aligned; relu: 0/1; bias / residual may be NULL. */
-/* Test hook: 1 = so_linear_3xtf32 with both MMA operands in shared memory; 0 (default) = the X operand split in
- * registers.  Both are parity-tested. */
-int so_linear_force_ss(int on);
 int so_split_tf32(const float* w, float* w_hi, float* w_lo, int64_t n, void* stream);
 int so_linear_3xtf32(const float* x, const float* w_hi, const float* w_lo, const float* bias, const float* residual,
                      float* y, int64_t M, int32_t N, int32_t K, int32_t relu, void* stream);

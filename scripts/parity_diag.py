@@ -5,7 +5,6 @@ Renders a strided sub-grid of the bench frame with the CUDA kernels and with the
 combinations so that a kernel bug, a decode (3xTF32) error and an ill-conditioned ray can be told apart:
 
   K(tc)    kernel render of the tensor-core-decoded volume          (what bench.py's parity block measured)
-  K(simt)  kernel render of the SIMT-decoded volume
   O64      fp64 oracle decode + fp64 oracle render              (the tolerance anchor)
   O64(tc)  fp64 oracle render of the kernel's own decoded volume (isolates the render kernel)
   O32      fp32 oracle decode + render                          (the reference's own arithmetic precision)
@@ -36,11 +35,10 @@ def main():
     ap.add_argument('--scene', default='lifted', choices=['lifted', 'analytic'])
     ap.add_argument('--out', default=os.path.join(ROOT, 'gpurun_out', 'parity_diag.json'))
     a = ap.parse_args()
-    from selfocc_b200 import ops, synth, _lib
+    from selfocc_b200 import ops, synth
     from oracle.mapping import GridMeterMappingRef
     from oracle import render as orender, rays as orays
     dev = torch.device('cuda:0')
-    lib = _lib.load()
     model, cfg = bench.build_model(a.workload, dev)
     feats, metas, _ = bench.make_frame(a.workload, seed=100)
     feats = [f.to(dev) for f in feats]
@@ -55,12 +53,8 @@ def main():
         r = model.lifter(ms_img_feats=feats)
         r = model.encoder(representation=r['representation'], ms_img_feats=feats, metas=metas)
         planes = r['representation']
-        vols = {}
-        for name, simt in (('tc', 0), ('simt', 1)):
-            lib.so_tpv_decode_force_simt(simt)
-            head.prepare(representation=planes, metas=metas)
-            vols[name] = (f.vol_sdf.clone(), None if f.vol_feat is None else f.vol_feat.clone())
-        lib.so_tpv_decode_force_simt(0)
+        head.prepare(representation=planes, metas=metas)
+        vols = {'tc': (f.vol_sdf.clone(), None if f.vol_feat is None else f.vol_feat.clone())}
     ny, nx = max(w['ray_number'][0] // a.stride, 1), max(w['ray_number'][1] // a.stride, 1)
     H_img, W_img = w['ray_img_size']
     M = head.img2lidar.matrices(metas, dev)[0].contiguous()
@@ -77,7 +71,6 @@ def main():
     vol32 = orender.tpv_decode_ref(*[p.float() for p in pl], (H, W, Z), *[t.float() for t in wb])
     vol_tc = vols['tc'][0][..., :Z].cpu().double()[None]          # [1,H,W,Z]
     dec = {'tc_vs_64_max_abs': (vol_tc[0] - vol64[0]).abs().max().item(),
-           'simt_vs_64_max_abs': (vols['simt'][0][..., :Z].cpu().double() - vol64[0]).abs().max().item(),
            'o32_vs_64_max_abs': (vol32[0].double() - vol64[0]).abs().max().item(),
            'sdf_abs_max': vol64[0].abs().max().item(), 'sdf_mean': vol64[0].mean().item(), 'sdf_std': vol64[0].std().item()}
     pix = orays.fixed_ray_grid([ny, nx], [H_img, W_img])
@@ -90,7 +83,7 @@ def main():
     flat = lambda d, k: d[k].reshape(-1).double()
     d64, a64 = flat(O64, 'depth'), flat(O64, 'acc')
     res = {'workload': a.workload, 'stride': a.stride, 'rays': int(d64.numel()), 'inv_s': inv_s, 'decode': dec}
-    pairs = {'K(tc) vs O64': (K['tc']['depth'].double(), d64), 'K(simt) vs O64': (K['simt']['depth'].double(), d64),
+    pairs = {'K(tc) vs O64': (K['tc']['depth'].double(), d64),
              'K(tc) vs O64(tc)': (K['tc']['depth'].double(), flat(O64tc, 'depth')), 'O32 vs O64': (flat(O32, 'depth'), d64),
              'O64(tc) vs O64': (flat(O64tc, 'depth'), d64)}
     bins = [0, 1e-6, 1e-4, 1e-2, 0.5, 0.99, 2.0]

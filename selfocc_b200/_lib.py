@@ -8,7 +8,7 @@ import os
 
 _PKG = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.environ.get('SELFOCC_B200_LIB') or os.path.join(_PKG, 'lib', 'libselfocc_b200.so')   # env: experimental variant
-ABI_VERSION = 9
+ABI_VERSION = 10
 
 
 class AxisMap(C.Structure):
@@ -52,7 +52,6 @@ SIGNATURES = {
     'so_tpv_decode_bwd_features': (C.c_int, [_P, _P, _P, _I, C.POINTER(VolumeDesc), _I, _I, _P, _P]),
     'so_tpv_decode_bwd_hidden': (C.c_int, [_P, _P, _P, _P, _I, C.POINTER(VolumeDesc), _I, _I, _P, _P, _P]),
     'so_tpv_decode_bwd_input': (C.c_int, [_P, _P, _L, _P]),
-    'so_tpv_decode_force_simt': (C.c_int, [C.c_int]),
     'so_bev_decode': (C.c_int, [_P, _I, _P, _P, _P, _P, C.POINTER(VolumeDesc), _P, _P, _P]),
     'so_bev_decode_bwd_gather': (C.c_int, [_P, _P, C.POINTER(VolumeDesc), _L, _L, _P, _P]),
     'so_bev_decode_bwd_features': (C.c_int, [_P, _L, _P, _P]),
@@ -80,7 +79,6 @@ SIGNATURES = {
     'so_field_query': (C.c_int, [_P, _P, C.POINTER(VolumeDesc), _P, _L, _P, _P, _P, _P]),
     'so_msda_forward': (C.c_int, [_P, _P, _P, _P, _P, _P, _I, _I, _I, _I, _I, _I, _I, _P]),
     'so_msda_backward': (C.c_int, [_P, _P, _P, _P, _P, _P, _P, _P, _P, _I, _I, _I, _I, _I, _I, _I, _P]),
-    'so_linear_force_ss': (C.c_int, [C.c_int]),
     'so_split_tf32': (C.c_int, [_P, _P, _P, _L, _P]),
     'so_linear_3xtf32': (C.c_int, [_P, _P, _P, _P, _P, _P, _L, _I, _I, _I, _P]),
     'so_linear_3xtf32_ln': (C.c_int, [_P, _P, _P, _P, _P, _P, _P, _F, _P, _L, _I, _I, _I, _P]),

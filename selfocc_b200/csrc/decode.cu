@@ -1,20 +1,19 @@
 // B5: TPV planes -> decoded volume (SURVEY.md section 8a row B5; semantics bev_nerf.py:62-95).
 //
-// One CTA decodes 128 consecutive (w, z) voxels of one h row:
-//   A[r][:]  = softplus(hw[h,w] + zh[z,h] + wz[w,z])           built in shared memory, never in HBM
-//   H1       = softplus(A * W1^T + b1)                           fp32 register-tiled 128x96x96 GEMM
-//   out[r,:] = H1 * W2^T + b2                                    (1 + n_feat outputs)
+// Per voxel (h, w, z), C channels:
+//   a0  = softplus(hw[h,w] + zh[z,h] + wz[w,z])       built tile by tile in shared memory, never in HBM
+//   a1  = softplus(a0 W1^T + b1)                       3xTF32 wgmma, W1 resident in shared memory
+//   out = a1 W2^T + b2                                 (1 + n_feat outputs) in registers -> volume
 // The reference materialises the [H,W,Z,C] broadcast sum (750 MB at cfg 2); here the only HBM traffic
 // is the 30 MB of planes (L2-resident across CTAs) and the decoded volume itself.
-// fp32 SIMT on purpose: the decoded sdf feeds a 1e-4-relative depth parity bar (fp32 reference,
-// autocast disabled at bev_nerf.py:73).
+// 3xTF32 (gemm.cu's operand split), not plain TF32: the decoded sdf feeds a 1e-4-relative depth parity bar (fp32
+// reference, autocast disabled at bev_nerf.py:73).
+// Also here: the BEV decode of tpv=False heads and the element-wise kernels of both decodes' slab backward.
 #include "tc_common.cuh"
 
 namespace so {
 
-constexpr int kRows = 128;      // voxels per CTA
-constexpr int kThreads = 256;
-constexpr int kMaxOut = 32;
+constexpr int kMaxOut = 32;     // widest second layer (1 + n_feat) so_tpv_decode accepts
 
 __device__ __forceinline__ float softplus_fast(float x) {
   // F.softplus(beta=1, threshold=20): max(x,0) + log1p(exp(-|x|)); identical to x beyond the threshold in fp32.
@@ -82,108 +81,8 @@ __device__ __forceinline__ void build_a_chunk(uint8_t* hi, uint8_t* lo, int row,
   store_split_tf32(hi, lo, swz_off(row, c4), f);
 }
 
-// C = channels (multiple of 32), LD = padded leading dimension (C + 4) in floats
-template <int C>
-__global__ void __launch_bounds__(kThreads) tpv_decode_kernel(
-    const float* __restrict__ hw, const float* __restrict__ zh, const float* __restrict__ wz,
-    const float* __restrict__ w1, const float* __restrict__ b1, const float* __restrict__ w2,
-    const float* __restrict__ b2, int H, int W, int Z, int zpitch, int n_out, int feat_pitch,
-    float* __restrict__ vol_sdf, float* __restrict__ vol_feat, int h_begin) {
-  constexpr int LD = C + 4;
-  constexpr int TN = C / 16;  // output columns per thread (strided by 16)
-  extern __shared__ __align__(16) float smem[];
-  float* As = smem;                 // [kRows][LD]
-  float* Ws = As + kRows * LD;      // [C][LD]   (W1 as given: [out][in])
-  float* W2s = Ws + C * LD;         // [n_out][C]
-  float* b1s = W2s + kMaxOut * C;   // [C]
-  float* b2s = b1s + C;             // [kMaxOut]
-
-  const int tid = threadIdx.x;
-  const int h = h_begin + blockIdx.y;     // row range [h_begin, h_begin + gridDim.y): so_tpv_decode_rows
-  const int v0 = blockIdx.x * kRows;
-  const int WZ = W * Z;
-
-  // stage weights
-  for (int i = tid; i < C * C / 4; i += kThreads) {
-    int j = (i * 4) / C, k = (i * 4) % C;
-    *reinterpret_cast<float4*>(Ws + j * LD + k) = __ldg(reinterpret_cast<const float4*>(w1) + i);
-  }
-  for (int i = tid; i < n_out * C; i += kThreads) W2s[i] = __ldg(w2 + i);
-  for (int i = tid; i < C; i += kThreads) b1s[i] = __ldg(b1 + i);
-  for (int i = tid; i < n_out; i += kThreads) b2s[i] = __ldg(b2 + i);
-
-  // build A = softplus(broadcast sum); a warp walks one voxel row's C channels with float4 (coalesced)
-  constexpr int kVecPerRow = C / 4;
-  for (int i = tid; i < kRows * kVecPerRow; i += kThreads) {
-    int r = i / kVecPerRow, c4 = i % kVecPerRow;
-    int v = v0 + r;
-    float4 f = make_float4(0.f, 0.f, 0.f, 0.f);
-    if (v < WZ) {
-      int w = v / Z, z = v - w * Z;
-      float4 a = __ldg(reinterpret_cast<const float4*>(hw + ((size_t)h * W + w) * C) + c4);
-      float4 b = __ldg(reinterpret_cast<const float4*>(zh + ((size_t)z * H + h) * C) + c4);
-      float4 c = __ldg(reinterpret_cast<const float4*>(wz + (size_t)v * C) + c4);
-      f.x = softplus_fast(a.x + b.x + c.x);
-      f.y = softplus_fast(a.y + b.y + c.y);
-      f.z = softplus_fast(a.z + b.z + c.z);
-      f.w = softplus_fast(a.w + b.w + c.w);
-    }
-    *reinterpret_cast<float4*>(As + r * LD + c4 * 4) = f;
-  }
-  __syncthreads();
-
-  // GEMM1: thread (ty, tx) owns rows ty*8..+7 and columns tx + 16*j
-  const int tx = tid & 15, ty = tid >> 4;
-  float acc[8][TN];
-#pragma unroll
-  for (int i = 0; i < 8; ++i)
-#pragma unroll
-    for (int j = 0; j < TN; ++j) acc[i][j] = 0.f;
-#pragma unroll 2
-  for (int k = 0; k < C; k += 4) {
-    float4 a[8], b[TN];
-#pragma unroll
-    for (int i = 0; i < 8; ++i) a[i] = *reinterpret_cast<const float4*>(As + (ty * 8 + i) * LD + k);
-#pragma unroll
-    for (int j = 0; j < TN; ++j) b[j] = *reinterpret_cast<const float4*>(Ws + (tx + 16 * j) * LD + k);
-#pragma unroll
-    for (int i = 0; i < 8; ++i)
-#pragma unroll
-      for (int j = 0; j < TN; ++j) {
-        acc[i][j] = fmaf(a[i].x, b[j].x, acc[i][j]);
-        acc[i][j] = fmaf(a[i].y, b[j].y, acc[i][j]);
-        acc[i][j] = fmaf(a[i].z, b[j].z, acc[i][j]);
-        acc[i][j] = fmaf(a[i].w, b[j].w, acc[i][j]);
-      }
-  }
-  __syncthreads();  // everyone done reading As
-#pragma unroll
-  for (int i = 0; i < 8; ++i)
-#pragma unroll
-    for (int j = 0; j < TN; ++j) As[(ty * 8 + i) * LD + tx + 16 * j] = softplus_fast(acc[i][j] + b1s[tx + 16 * j]);
-  __syncthreads();
-
-  // GEMM2: (row, out-channel) pairs, K = C
-  for (int idx = tid; idx < kRows * n_out; idx += kThreads) {
-    int r = idx % kRows, c = idx / kRows;
-    int v = v0 + r;
-    if (v >= WZ) continue;
-    float s = b2s[c];
-    const float4* hp = reinterpret_cast<const float4*>(As + r * LD);
-    const float4* wp = reinterpret_cast<const float4*>(W2s + c * C);
-#pragma unroll 4
-    for (int k = 0; k < C / 4; ++k) {
-      float4 x = hp[k], y = wp[k];
-      s = fmaf(x.x, y.x, s); s = fmaf(x.y, y.y, s); s = fmaf(x.z, y.z, s); s = fmaf(x.w, y.w, s);
-    }
-    int w = v / Z, z = v - w * Z;
-    if (c == 0) vol_sdf[((size_t)h * W + w) * zpitch + z] = s;
-    else vol_feat[(((size_t)h * W + w) * Z + z) * feat_pitch + (c - 1)] = s;
-  }
-}
-
 // ---------------------------------------------------------------------------------------------------------------------
-// Tensor-core variant (wgmma, same 3xTF32 operand splitting as gemm.cu so the decoded sdf keeps fp32-level accuracy).
+// TPV decode (wgmma, same 3xTF32 operand splitting as gemm.cu so the decoded sdf keeps fp32-level accuracy).
 // Persistent CTA per SM, 16 warps:
 //   warps 0-7   builders   A tile = softplus(hw + zh + wz) for 128 voxels x 32 channels at a time, split into TF32 hi / lo and
 //                          written straight into the 128B-swizzled K-major operand layout (no TMA: the operand is computed)
@@ -198,8 +97,8 @@ constexpr int kDecStagesMax = 4;
 struct DecSmem {
   int atoms, stages, w_bytes, ring, w2, b1, b2, bars, total;
 };
-__host__ __device__ inline DecSmem dec_smem(int C, int n_out) {
-  DecSmem m;
+__host__ __device__ constexpr DecSmem dec_smem(int C, int n_out) {
+  DecSmem m{};
   m.atoms = C / kAtomK;
   m.w_bytes = 2 * m.atoms * C * 128;                          // W1 hi + lo: atoms x [C rows x 128 B]
   const int fixed = m.w_bytes + n_out * C * 4 + C * 4 + 128 + 256;
@@ -213,6 +112,8 @@ __host__ __device__ inline DecSmem dec_smem(int C, int n_out) {
   m.total = m.bars + 256 + 1024;
   return m;
 }
+// the largest accepted C and n_out leave the fewest ring stages; the pipeline needs two
+static_assert(dec_smem(128, kMaxOut).stages >= 2, "the wgmma decode needs 2 ring stages for every accepted (C, n_out)");
 
 // C = channels (wgmma N); NOUT = compile-time upper bound of the second layer's width (1 + n_feat): the per-row outputs
 // stay in registers
@@ -678,31 +579,9 @@ __global__ void zero_pad_kernel(float* vol_sdf, long long columns, int Z, int zp
   vol_sdf[col * zpitch + z] = 0.f;
 }
 
-template <int C>
-int launch_decode(const float* hw, const float* zh, const float* wz, const float* w1, const float* b1, const float* w2,
-                  const float* b2, const so_volume_desc* d, float* vol_sdf, float* vol_feat, int h_begin, int h_count, cudaStream_t st) {
-  constexpr int LD = C + 4;
-  size_t smem = sizeof(float) * ((size_t)kRows * LD + (size_t)C * LD + (size_t)kMaxOut * C + C + kMaxOut);
-  static PerDeviceOnce attr_simt;
-  int rc_attr = attr_simt.run([smem] {
-    return check_cuda(cudaFuncSetAttribute(tpv_decode_kernel<C>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  });
-  if (rc_attr) return rc_attr;
-  dim3 grid((unsigned)ceil_div64((int64_t)d->W * d->Z, kRows), (unsigned)h_count);
-  ProfScope prof(1, st);
-  tpv_decode_kernel<C><<<grid, kThreads, smem, st>>>(hw, zh, wz, w1, b1, w2, b2, d->H, d->W, d->Z, d->zpitch,
-                                                       1 + d->n_feat, d->feat_pitch, vol_sdf, vol_feat, h_begin);
-  note_launch(1);
-  return check_launch();
-}
-
 }  // namespace so
 
 using namespace so;
-
-static bool g_decode_force_simt = false;
-// Test hook: 1 = use the fp32 SIMT decode kernel even where the tensor-core kernel applies (both are parity-tested).
-extern "C" int so_tpv_decode_force_simt(int on) { g_decode_force_simt = on != 0; return SO_OK; }
 
 extern "C" int so_tpv_decode(const float* tpv_hw, const float* tpv_zh, const float* tpv_wz, int32_t C, const float* w1,
                              const float* b1, const float* w2, const float* b2, const so_volume_desc* d,
@@ -731,47 +610,36 @@ extern "C" int so_tpv_decode_rows(const float* tpv_hw, const float* tpv_zh, cons
     zero_pad_kernel<<<(unsigned)ceil_div64(n, 256), 256, 0, st>>>(vol_sdf + (long long)h_begin * d->W * d->zpitch, cols, d->Z, d->zpitch);
     note_launch(1);
   }
-  if (C % 32 == 0 && C >= 32 && C <= 128 && !g_decode_force_simt) {
-    const int n_out = 1 + d->n_feat;
-    DecSmem Ls = dec_smem(C, n_out);
-    if (Ls.stages >= 2) {
-      static PerDeviceOnce attr_tc;
-      if ((rc = attr_tc.run([] {
-             int r = SO_OK;
+  const int n_out = 1 + d->n_feat;
+  const DecSmem Ls = dec_smem(C, n_out);
+  static PerDeviceOnce attr_tc;
+  if ((rc = attr_tc.run([] {
+         int r = SO_OK;
 #define SO_DEC_ATTR(C_, NO) if (!r) r = check_cuda(cudaFuncSetAttribute(tpv_decode_tc_kernel<C_, NO>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024))
 #define SO_DEC_ATTR_C(C_) SO_DEC_ATTR(C_, 1); SO_DEC_ATTR(C_, 4); SO_DEC_ATTR(C_, 32)
-             SO_DEC_ATTR_C(32); SO_DEC_ATTR_C(64); SO_DEC_ATTR_C(96); SO_DEC_ATTR_C(128);
+         SO_DEC_ATTR_C(32); SO_DEC_ATTR_C(64); SO_DEC_ATTR_C(96); SO_DEC_ATTR_C(128);
 #undef SO_DEC_ATTR_C
 #undef SO_DEC_ATTR
-             return r;
-           })))
-        return rc;
-      const int tiles_per_row = (int)ceil_div64((int64_t)d->W * d->Z, kBM);
-      const int n_tiles = tiles_per_row * h_count;
-      const int sms = num_sms(), grid = n_tiles < sms ? n_tiles : sms;
-      ProfScope prof(1, st);
+         return r;
+       })))
+    return rc;
+  const int tiles_per_row = (int)ceil_div64((int64_t)d->W * d->Z, kBM);
+  const int n_tiles = tiles_per_row * h_count;
+  const int sms = num_sms(), grid = n_tiles < sms ? n_tiles : sms;
+  ProfScope prof(1, st);
 #define SO_DEC_TC(C_, NO) tpv_decode_tc_kernel<C_, NO><<<grid, kDecThreads, Ls.total, st>>>(tpv_hw, tpv_zh, tpv_wz, w1, b1, w2, b2, d->H, d->W, \
-                                                                                  d->Z, d->zpitch, n_out, d->feat_pitch, vol_sdf, vol_feat, tiles_per_row, n_tiles, h_begin)
+                                                                              d->Z, d->zpitch, n_out, d->feat_pitch, vol_sdf, vol_feat, tiles_per_row, n_tiles, h_begin)
 #define SO_DEC_TC_C(C_) if (n_out == 1) SO_DEC_TC(C_, 1); else if (n_out <= 4) SO_DEC_TC(C_, 4); else SO_DEC_TC(C_, 32)
-      switch (C) {
-        case 32: SO_DEC_TC_C(32); break;
-        case 64: SO_DEC_TC_C(64); break;
-        case 96: SO_DEC_TC_C(96); break;
-        default: SO_DEC_TC_C(128); break;
-      }
+  switch (C) {
+    case 32: SO_DEC_TC_C(32); break;
+    case 64: SO_DEC_TC_C(64); break;
+    case 96: SO_DEC_TC_C(96); break;
+    default: SO_DEC_TC_C(128); break;
+  }
 #undef SO_DEC_TC_C
 #undef SO_DEC_TC
-      note_launch(1);
-      return check_launch();
-    }
-  }
-  switch (C) {
-    case 32: return launch_decode<32>(tpv_hw, tpv_zh, tpv_wz, w1, b1, w2, b2, d, vol_sdf, vol_feat, h_begin, h_count, st);
-    case 64: return launch_decode<64>(tpv_hw, tpv_zh, tpv_wz, w1, b1, w2, b2, d, vol_sdf, vol_feat, h_begin, h_count, st);
-    case 96: return launch_decode<96>(tpv_hw, tpv_zh, tpv_wz, w1, b1, w2, b2, d, vol_sdf, vol_feat, h_begin, h_count, st);
-    case 128: return launch_decode<128>(tpv_hw, tpv_zh, tpv_wz, w1, b1, w2, b2, d, vol_sdf, vol_feat, h_begin, h_count, st);
-    default: return SO_ERR_UNSUPPORTED;
-  }
+  note_launch(1);
+  return check_launch();
 }
 
 // ---------------------------------------------------------------------------------------------------------------------

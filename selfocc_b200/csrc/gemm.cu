@@ -23,11 +23,9 @@
 // fills of its own stages (with one shared ring, a warpgroup waiting K/32 atoms ahead of the producer could take an
 // older phase of the same parity for its own).
 //
-// The A operand (X hi / lo) comes from REGISTERS by default: each thread loads its wgmma fragment from the swizzled
-// stage and splits it in registers, so the tensor core reads only W from shared memory and the stage is released as
-// soon as it has been loaded.  Two fragment sets: atom a + 1 is loaded and split while the MMAs of atom a run
-// (wgmma.wait_group 1).  so_linear_force_ss(1) selects the variant with both operands in shared memory (the X atom is
-// split in place into hi plus a second lo buffer); both issue the same products in the same order.
+// The A operand (X hi / lo) comes from REGISTERS: each thread loads its wgmma fragment from the swizzled stage and
+// splits it in registers, so the tensor core reads only W from shared memory and a stage holds the raw X atom only.
+// Two fragment sets: atom a + 1 is loaded and split while the MMAs of atom a run (wgmma.wait_group 1).
 //
 // Tuning, one H100 80GB HBM3 at a 400 W power limit, the 12 launches of one encoder layer (scripts/bench_gemm.py, sum):
 //   both warpgroups on one 128-row tile, wait_group 0 per atom, BN = fewest padded columns   1.244 ms
@@ -76,8 +74,7 @@ static int make_tmap(CUtensorMap* m, const float* base, int64_t rows, int64_t co
 }
 
 struct PipeCfg {
-  int BN, KA, stages;       // n-tile width, atoms along K (K / 32), ring depth
-  int stage_bytes;          // raw X atom (A from registers) or raw/hi + lo atoms (A from shared memory)
+  int BN, KA, stages;       // n-tile width, atoms along K (K / 32), ring depth (one raw X atom per stage)
   int w_bytes;              // resident W bytes = 2 * KA * BN * 128
   int smem;                 // dynamic shared memory request (incl. 1 KB alignment slack)
   int n_tiles, m_tiles, groups;  // grid = n_tiles x groups CTAs; group g walks m-tiles g, g + groups, ...
@@ -109,18 +106,17 @@ static int pick_bn(int N, int m_tiles, int sms, bool whole_row) {
   return best;
 }
 
-static PipeCfg make_pipe_cfg(int64_t M, int N, int K, bool reg_a, bool whole_row, int sms) {
+static PipeCfg make_pipe_cfg(int64_t M, int N, int K, bool whole_row, int sms) {
   PipeCfg c;
   c.m_tiles = (int)ceil_div64(M, kGemmTileM);
   c.BN = pick_bn(N, c.m_tiles, sms, whole_row);
   bn_cost(c.BN, N, c.m_tiles, sms, &c.n_tiles, &c.groups);
   c.KA = K / kAtomK;
   c.w_bytes = 2 * c.KA * c.BN * 128;
-  c.stage_bytes = reg_a ? kGemmTileBytes : 2 * kGemmTileBytes;
   const int fixed = c.w_bytes + 256;                          // + mbarriers
-  c.stages = (227 * 1024 - 1024 - fixed) / c.stage_bytes & ~1;  // even: half of the ring per warpgroup
+  c.stages = (227 * 1024 - 1024 - fixed) / kGemmTileBytes & ~1;  // even: half of the ring per warpgroup
   if (c.stages > kMaxStages) c.stages = kMaxStages;
-  c.smem = fixed + c.stages * c.stage_bytes + 1024;
+  c.smem = fixed + c.stages * kGemmTileBytes + 1024;
   return c;
 }
 
@@ -180,21 +176,20 @@ __device__ __forceinline__ void mma_atom_rs(float* acc, uint32_t* ah, uint32_t* 
   wg_commit();
 }
 
-template <int BN, bool kRegA>
+template <int BN>
 __global__ void __launch_bounds__(kGemmThreads, 1)
 linear_3xtf32_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_constant__ CUtensorMap map_whi,
                      const __grid_constant__ CUtensorMap map_wlo, const float* __restrict__ bias,
                      const float* __restrict__ residual, float* __restrict__ y, long long M, int N, int KA, int stages,
                      int n_tiles, int m_tiles, int relu, const float* __restrict__ ln_gamma, const float* __restrict__ ln_beta,
                      float ln_eps) {
-  constexpr int kStageBytes = kRegA ? kGemmTileBytes : 2 * kGemmTileBytes;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* sm = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
   const int w_bytes = 2 * KA * BN * 128;
   uint8_t* w_hi = sm;
   uint8_t* w_lo = sm + KA * BN * 128;
-  uint8_t* ring = sm + w_bytes;                                   // stages x kStageBytes, 1 KB aligned
-  uint64_t* bars = reinterpret_cast<uint64_t*>(ring + stages * kStageBytes);
+  uint8_t* ring = sm + w_bytes;                                   // stages x kGemmTileBytes, 1 KB aligned
+  uint64_t* bars = reinterpret_cast<uint64_t*>(ring + stages * kGemmTileBytes);
   uint64_t* w_full = bars;
   uint64_t* full = bars + 1;
   uint64_t* empty = full + kMaxStages;
@@ -236,7 +231,7 @@ linear_3xtf32_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_con
           const int slot = w ? half + s1 : s0;
           mbar_wait(empty + slot, (w ? ph1 : ph0) ^ 1);
           mbar_expect_tx(full + slot, (uint32_t)kGemmTileBytes);
-          tma_load_2d(ring + slot * kStageBytes, &map_x, a * kAtomK, mt * kGemmTileM, full + slot);
+          tma_load_2d(ring + slot * kGemmTileBytes, &map_x, a * kAtomK, mt * kGemmTileM, full + slot);
           if (w) ring_advance(s1, ph1, half); else ring_advance(s0, ph0, half);
         }
       }
@@ -252,102 +247,58 @@ linear_3xtf32_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_con
   for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
   const uint32_t whi = smem_u32(w_hi), wlo = smem_u32(w_lo);
   mbar_wait(w_full, 0);
-  uint8_t* my_ring = ring + wg * half * kStageBytes;              // this warpgroup's half of the ring
+  uint8_t* my_ring = ring + wg * half * kGemmTileBytes;           // this warpgroup's half of the ring
   uint64_t* my_full = full + wg * half;
   uint64_t* my_empty = empty + wg * half;
   int s = 0; uint32_t ph = 0;
   for (int mt = group + wg * n_groups; mt < m_tiles; mt += 2 * n_groups) {
     uint32_t accum = 0;
-    if constexpr (kRegA) {
-      // two fragment sets: atom a + 1 is loaded and split while the MMAs of atom a run.  At BN >= 96 the second set
-      // does not fit in the 168 registers a thread gets: one set, and each atom's MMAs complete before the next load.
-      constexpr bool kTwoSets = BN <= 80;
-      uint32_t ah0[16], al0[16], ah1_[kTwoSets ? 16 : 1], al1_[kTwoSets ? 16 : 1];
-      uint32_t* ah1 = kTwoSets ? ah1_ : ah0;
-      uint32_t* al1 = kTwoSets ? al1_ : al0;
-      // A stage goes back to the producer only once the MMAs that took their A fragments from it have completed.  The
-      // fragments are read with generic loads and the next TMA write into the stage is an async-proxy write: releasing
-      // the stage right after the loads were issued let that write overtake loads still in flight (wrong rows in a few
-      // m-tiles of long runs).  An MMA cannot complete before its register operands have arrived.
-      int pending = -1;                                    // two sets: the stage of the MMA group still in flight
-      auto release = [&](int slot) {
-        if (slot < 0) return;
-        __syncwarp();
-        if (lane == 0) mbar_arrive(my_empty + slot);
-      };
-      auto fetch = [&](uint32_t* ah, uint32_t* al) {
-        mbar_wait(my_full + s, ph);
-        load_split_frag(my_ring + s * kStageBytes, frag_row, g, t, ah, al);
-        const int slot = s;
-        ring_advance(s, ph, half);
-        return slot;
-      };
-      auto issue = [&](uint32_t* ah, uint32_t* al, int a, int slot) {
-        mma_atom_rs<BN>(acc, ah, al, whi + a * BN * 128, wlo + a * BN * 128, accum);
-        if constexpr (kTwoSets) {
-          wg_wait1();                                      // atom a - 1 is done: its set and its stage are free
-          release(pending);
-          pending = slot;
-        } else {
-          wg_wait0();                                      // atom a is done: the one set and its stage are free
-          release(slot);
-        }
-      };
-      int cur = fetch(ah0, al0);
-      for (int a = 0; a < KA; a += 2) {
-        issue(ah0, al0, a, cur);
-        if (a + 1 < KA) {
-          cur = fetch(ah1, al1);
-          issue(ah1, al1, a + 1, cur);
-          if (a + 2 < KA) cur = fetch(ah0, al0);
-        }
+    // two fragment sets: atom a + 1 is loaded and split while the MMAs of atom a run.  At BN >= 96 the second set
+    // does not fit in the 168 registers a thread gets: one set, and each atom's MMAs complete before the next load.
+    constexpr bool kTwoSets = BN <= 80;
+    uint32_t ah0[16], al0[16], ah1_[kTwoSets ? 16 : 1], al1_[kTwoSets ? 16 : 1];
+    uint32_t* ah1 = kTwoSets ? ah1_ : ah0;
+    uint32_t* al1 = kTwoSets ? al1_ : al0;
+    // A stage goes back to the producer only once the MMAs that took their A fragments from it have completed.  The
+    // fragments are read with generic loads and the next TMA write into the stage is an async-proxy write: releasing
+    // the stage right after the loads were issued let that write overtake loads still in flight (wrong rows in a few
+    // m-tiles of long runs).  An MMA cannot complete before its register operands have arrived.
+    int pending = -1;                                    // two sets: the stage of the MMA group still in flight
+    auto release = [&](int slot) {
+      if (slot < 0) return;
+      __syncwarp();
+      if (lane == 0) mbar_arrive(my_empty + slot);
+    };
+    auto fetch = [&](uint32_t* ah, uint32_t* al) {
+      mbar_wait(my_full + s, ph);
+      load_split_frag(my_ring + s * kGemmTileBytes, frag_row, g, t, ah, al);
+      const int slot = s;
+      ring_advance(s, ph, half);
+      return slot;
+    };
+    auto issue = [&](uint32_t* ah, uint32_t* al, int a, int slot) {
+      mma_atom_rs<BN>(acc, ah, al, whi + a * BN * 128, wlo + a * BN * 128, accum);
+      if constexpr (kTwoSets) {
+        wg_wait1();                                      // atom a - 1 is done: its set and its stage are free
+        release(pending);
+        pending = slot;
+      } else {
+        wg_wait0();                                      // atom a is done: the one set and its stage are free
+        release(slot);
       }
-      wg_wait0();
-      release(pending);
-      fence_regs<BN / 2>(acc);
-    } else {
-      for (int a = 0; a < KA; ++a) {
-        mbar_wait(my_full + s, ph);
-        uint8_t* stage = my_ring + s * kStageBytes;
-        const uint32_t bhi = whi + a * BN * 128, blo = wlo + a * BN * 128;
-        // split the 64-row atom in place: raw -> hi, lo into the second half of the stage.  Element-wise, so the
-        // swizzle is irrelevant.
-        float4* hi = reinterpret_cast<float4*>(stage);
-        float4* lo = reinterpret_cast<float4*>(stage + kGemmTileBytes);
-        const int wt = tid & 127;
-#pragma unroll
-        for (int i = 0; i < kGemmTileBytes / 16 / 128; ++i) {
-          float4 v = hi[wt + i * 128], h, l;
-          h.x = tf32_rn(v.x); l.x = v.x - h.x;
-          h.y = tf32_rn(v.y); l.y = v.y - h.y;
-          h.z = tf32_rn(v.z); l.z = v.z - h.z;
-          h.w = tf32_rn(v.w); l.w = v.w - h.w;
-          hi[wt + i * 128] = h;
-          lo[wt + i * 128] = l;
-        }
-        asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // generic-proxy smem writes -> visible to wgmma
-        wg_sync(1 + wg);
-        const uint32_t ahi = smem_u32(stage), alo = ahi + kGemmTileBytes;
-        fence_regs<BN / 2>(acc);
-        wg_fence();
-#pragma unroll
-        for (int prod = 0; prod < 3; ++prod) {
-          const uint32_t ab = prod == 1 ? alo : ahi;
-          const uint32_t bb = prod == 2 ? blo : bhi;
-#pragma unroll
-          for (int kk = 0; kk < kAtomK / 8; ++kk) {
-            Wgmma<BN>::ss(acc, make_desc(ab + kk * 32), make_desc(bb + kk * 32), accum);
-            accum = 1u;
-          }
-        }
-        wg_commit();
-        wg_wait0();
-        fence_regs<BN / 2>(acc);
-        __syncwarp();
-        if (lane == 0) mbar_arrive(my_empty + s);          // this warpgroup's MMAs have finished reading the stage
-        ring_advance(s, ph, half);
+    };
+    int cur = fetch(ah0, al0);
+    for (int a = 0; a < KA; a += 2) {
+      issue(ah0, al0, a, cur);
+      if (a + 1 < KA) {
+        cur = fetch(ah1, al1);
+        issue(ah1, al1, a + 1, cur);
+        if (a + 2 < KA) cur = fetch(ah0, al0);
       }
     }
+    wg_wait0();
+    release(pending);
+    fence_regs<BN / 2>(acc);
 
     // ===== epilogue: accumulator registers -> (+bias, ReLU, +residual [, LayerNorm]) -> global =====
     const long long row[2] = {(long long)mt * kGemmTileM + frag_row, (long long)mt * kGemmTileM + frag_row + 8};
@@ -420,18 +371,14 @@ __global__ void split_tf32_kernel(const float* __restrict__ w, float* __restrict
   lo[i] = v - h;
 }
 
-template <int BN, bool kRegA>
+template <int BN>
 static int set_smem_attr() {
-  return check_cuda(cudaFuncSetAttribute(linear_3xtf32_kernel<BN, kRegA>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
+  return check_cuda(cudaFuncSetAttribute(linear_3xtf32_kernel<BN>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
 }
 
 }  // namespace so
 
 using namespace so;
-
-static bool g_linear_force_ss = false;
-// Test hook: 1 = both MMA operands from shared memory; 0 (default) = A operand from registers.
-extern "C" int so_linear_force_ss(int on) { g_linear_force_ss = on != 0; return SO_OK; }
 
 extern "C" int so_split_tf32(const float* w, float* hi, float* lo, int64_t n, void* stream) {
   if (!w || !hi || !lo || n < 0) return SO_ERR_INVALID_ARG;
@@ -451,12 +398,12 @@ extern "C" int so_linear_3xtf32(const float* x, const float* w_hi, const float* 
 }
 
 // y = LayerNorm(act(x w^T + bias) + residual) * gamma + beta over the N output columns, in the GEMM epilogue.
-// N must be a multiple of 32 and <= 128 (one n-tile holds the whole row); register-A pipeline only.
+// N must be a multiple of 32 and <= 128 (one n-tile holds the whole row).
 extern "C" int so_linear_3xtf32_ln(const float* x, const float* w_hi, const float* w_lo, const float* bias, const float* residual,
                                    const float* gamma, const float* beta, float eps, float* y, int64_t M, int32_t N, int32_t K,
                                    int32_t relu, void* stream) {
   if (!gamma || !beta) return SO_ERR_INVALID_ARG;
-  if (N % 32 != 0 || N > 128 || g_linear_force_ss) return SO_ERR_UNSUPPORTED;
+  if (N % 32 != 0 || N > 128) return SO_ERR_UNSUPPORTED;
   return linear_impl(x, w_hi, w_lo, bias, residual, y, M, N, K, relu, gamma, beta, eps, stream);
 }
 
@@ -471,8 +418,7 @@ static int linear_impl(const float* x, const float* w_hi, const float* w_lo, con
   if (M > 0x7fffffffLL) return SO_ERR_UNSUPPORTED;
   // the epilogue stores Y and reads the residual as column pairs (float2)
   if ((reinterpret_cast<uintptr_t>(y) & 7) || (reinterpret_cast<uintptr_t>(residual) & 7) || (N % 2)) return SO_ERR_UNSUPPORTED;
-  const bool reg_a = !g_linear_force_ss;
-  PipeCfg cfg = make_pipe_cfg(M, N, K, reg_a, ln_gamma != nullptr, num_sms());
+  PipeCfg cfg = make_pipe_cfg(M, N, K, ln_gamma != nullptr, num_sms());
   if (cfg.stages < 2) return SO_ERR_UNSUPPORTED;
   CUtensorMap mx, mhi, mlo;
   int rc;
@@ -482,31 +428,24 @@ static int linear_impl(const float* x, const float* w_hi, const float* w_lo, con
   static PerDeviceOnce smem_attr;
   if ((rc = smem_attr.run([] {
          int r;
-         if ((r = set_smem_attr<32, true>()) || (r = set_smem_attr<64, true>()) || (r = set_smem_attr<80, true>()) ||
-             (r = set_smem_attr<96, true>()) || (r = set_smem_attr<128, true>()) || (r = set_smem_attr<32, false>()) ||
-             (r = set_smem_attr<64, false>()) || (r = set_smem_attr<80, false>()) || (r = set_smem_attr<96, false>()) ||
-             (r = set_smem_attr<128, false>()))
+         if ((r = set_smem_attr<32>()) || (r = set_smem_attr<64>()) || (r = set_smem_attr<80>()) || (r = set_smem_attr<96>()) ||
+             (r = set_smem_attr<128>()))
            return r;
          return SO_OK;
        })))
     return rc;
   cudaStream_t st = (cudaStream_t)stream;
   ProfScope prof(8, st);
-#define SO_GEMM(BN_, REGA)                                                                                                   \
-  linear_3xtf32_kernel<BN_, REGA><<<cfg.n_tiles * cfg.groups, kGemmThreads, cfg.smem, st>>>(                                \
+#define SO_GEMM(BN_)                                                                                                           \
+  linear_3xtf32_kernel<BN_><<<cfg.n_tiles * cfg.groups, kGemmThreads, cfg.smem, st>>>(                                         \
       mx, mhi, mlo, bias, residual, y, (long long)M, N, cfg.KA, cfg.stages, cfg.n_tiles, cfg.m_tiles, relu, ln_gamma, ln_beta, \
       ln_eps)
-  switch (cfg.BN * 2 + (reg_a ? 1 : 0)) {
-    case 32 * 2 + 1: SO_GEMM(32, true); break;
-    case 64 * 2 + 1: SO_GEMM(64, true); break;
-    case 80 * 2 + 1: SO_GEMM(80, true); break;
-    case 96 * 2 + 1: SO_GEMM(96, true); break;
-    case 128 * 2 + 1: SO_GEMM(128, true); break;
-    case 32 * 2: SO_GEMM(32, false); break;
-    case 64 * 2: SO_GEMM(64, false); break;
-    case 80 * 2: SO_GEMM(80, false); break;
-    case 96 * 2: SO_GEMM(96, false); break;
-    default: SO_GEMM(128, false); break;
+  switch (cfg.BN) {
+    case 32: SO_GEMM(32); break;
+    case 64: SO_GEMM(64); break;
+    case 80: SO_GEMM(80); break;
+    case 96: SO_GEMM(96); break;
+    default: SO_GEMM(128); break;
   }
 #undef SO_GEMM
   note_launch(1);

@@ -56,8 +56,6 @@ __device__ __forceinline__ void wg_commit() { asm volatile("wgmma.commit_group.s
 __device__ __forceinline__ void wg_wait0() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
 // all but the most recently committed wgmma group have completed
 __device__ __forceinline__ void wg_wait1() { asm volatile("wgmma.wait_group.sync.aligned 1;" ::: "memory"); }
-// named barrier of the 128 threads of one warpgroup (ids 1.. are free: __syncthreads uses 0)
-__device__ __forceinline__ void wg_sync(int id) { asm volatile("bar.sync %0, 128;" ::"r"(id) : "memory"); }
 
 // Shared-memory matrix descriptor: K-major operand, 128-byte swizzle, 8-row groups 1024 B apart.  The atom base must be
 // 1024-byte aligned; a K step inside the atom advances the start address by 32 bytes (8 tf32).

@@ -491,10 +491,9 @@ class FieldSecondGradFunction(torch.autograd.Function):
 
 class TPVDecodeFunction(torch.autograd.Function):
     """Decode with the fused sm_90a forward.  Backward (training only) recomputes the MLP slab by slab -- bounded memory,
-    never the reference's 750 MB intermediate.  Default: the native slab backward (_backward_native: wgmma 3xTF32 GEMMs
-    + the fused element-wise kernels so_tpv_decode_bwd_*); SELFOCC_B200_DECODE_BWD=torch or an unsupported channel count
-    takes the torch/cuBLAS autograd restatement of the same slab (_backward_torch), which is also what the tests compare
-    the native path with."""
+    never the reference's 750 MB intermediate.  The native slab backward (_backward_native: wgmma 3xTF32 GEMMs + the fused
+    element-wise kernels so_tpv_decode_bwd_*) wherever the 3xTF32 GEMM takes the channel count and the second layer has
+    at most 32 outputs; otherwise the torch/cuBLAS autograd restatement of the same slab (_backward_torch)."""
 
     SLAB_ROWS = 32
 
@@ -509,11 +508,9 @@ class TPVDecodeFunction(torch.autograd.Function):
     @staticmethod
     @torch.autograd.function.once_differentiable
     def backward(ctx, g_vs, g_vf):
-        import os
         saved, d = ctx.saved_tensors, ctx.desc
         Cc = saved[0].shape[-1]
-        native = os.environ.get('SELFOCC_B200_DECODE_BWD', 'native') != 'torch' and linear_supported(Cc, Cc) \
-            and tuple(saved[3].shape) == (Cc, Cc) and 1 + d.n_feat <= 32
+        native = linear_supported(Cc, Cc) and tuple(saved[3].shape) == (Cc, Cc) and 1 + d.n_feat <= 32
         fn = TPVDecodeFunction._backward_native if native else TPVDecodeFunction._backward_torch
         return (*fn(saved, d, g_vs, g_vf), None)
 

@@ -140,7 +140,7 @@ def test_entry_points_reject_bad_arguments_without_a_gpu():
     assert lib.so_render_train_probe(C.byref(ok), one, N, C.byref(rd), C.byref(pr), N, one, N) == -1
     pr.num_samples = 257                                                                               # S <= 256
     assert lib.so_render_train_probe(C.byref(ok), one, N, C.byref(rd), C.byref(pr), N, one, N) == -2
-    for hook in (lib.so_attn_force_v1, lib.so_linear_force_ss, lib.so_render_train_force_sem_generic):
+    for hook in (lib.so_attn_force_v1, lib.so_render_train_force_sem_generic):
         assert hook(1) == 0 and hook(0) == 0
 
 

@@ -1,7 +1,7 @@
 """GPU parity of the TPV decode (B5: so_tpv_decode / so_tpv_decode_rows and the slab backward behind
 ops.TPVDecodeFunction) against the fp64 oracle evaluated slab by slab on the device (oracle/decode_parity.py):
 
-  * forward on EVERY voxel and channel at the shipped configs' volume geometry, both kernels, into NaN-filled buffers;
+  * forward on EVERY voxel and channel at the shipped configs' volume geometry, into NaN-filled buffers;
   * the persistent wgmma kernel's tile loop, masks and instantiations at volumes chosen from its tile arithmetic;
   * row slabs (so_tpv_decode_rows) into NaN-filled buffers;
   * inputs that cover the whole softplus domain, with the activation and sigmoid errors reported per pre-activation bucket;
@@ -78,7 +78,7 @@ def _oracle(planes, mlp, d):
     return dp.decode_slabwise(*[p.double() for p in planes], (d.H, d.W, d.Z), *[t.double() for t in mlp])
 
 
-def _launch(planes, mlp, d, simt=False, rows=None, out=None):
+def _launch(planes, mlp, d, rows=None, out=None):
     """so_tpv_decode_rows through the C ABI into NaN-filled (or the given) full-size buffers."""
     from selfocc_b200 import _lib, ops
     lib = _lib.load()
@@ -87,12 +87,8 @@ def _launch(planes, mlp, d, simt=False, rows=None, out=None):
         out = (torch.full((d.H, d.W, d.zpitch), NAN, device=dev),
                torch.full((d.H, d.W, d.Z, d.feat_pitch), NAN, device=dev) if d.n_feat else None)
     h0, hc = (0, d.H) if rows is None else rows
-    lib.so_tpv_decode_force_simt(int(simt))
-    try:
-        _lib.check(lib.so_tpv_decode_rows(*map(ops._p, planes), planes[0].shape[-1], *map(ops._p, mlp),
-                                          C.byref(d), h0, hc, ops._p(out[0]), ops._p(out[1]), ops._stream()), 'so_tpv_decode_rows')
-    finally:
-        lib.so_tpv_decode_force_simt(0)
+    _lib.check(lib.so_tpv_decode_rows(*map(ops._p, planes), planes[0].shape[-1], *map(ops._p, mlp),
+                                      C.byref(d), h0, hc, ops._p(out[0]), ops._p(out[1]), ops._stream()), 'so_tpv_decode_rows')
     return out
 
 
@@ -130,15 +126,6 @@ def _check_volume(out, ref, d, rows=None, scale=1.0):
     return e_sdf, e_feat
 
 
-def _check_pair(tc, simt, ref, d):
-    """wgmma against SIMT on the same inputs: each is within one bar of the oracle, so they are within two of each other."""
-    a, b = tc[0][..., :d.Z].double(), simt[0][..., :d.Z].double()
-    assert float((a - b).abs().max()) <= 2 * SDF_BAR * max(1.0, float(ref[..., 0].abs().max()))
-    if d.n_feat:
-        a, b = tc[1][..., :d.n_feat].double(), simt[1][..., :d.n_feat].double()
-        assert float(((a - b).abs() / (FEAT_ATOL + FEAT_RTOL * ref[..., 1:].abs())).max()) <= 2.0
-
-
 # ---- 1. forward, every voxel, shipped geometry -----------------------------------------------------------------------------
 @gpu
 @pytest.mark.parametrize('name', list(SHIPPED))
@@ -148,21 +135,17 @@ def test_forward_every_voxel_at_shipped_geometry(name):
     d = _shipped_desc(name)
     planes, mlp = _inputs(d, 96, seed=11)
     ref = _oracle(planes, mlp, d)
-    out = {}
-    for simt in (False, True):
-        out[simt] = _launch(planes, mlp, d, simt)
-        e = _check_volume(out[simt], ref, d)
-        print('%s forward (%s): sdf max abs err %.3e (|sdf| max %.2f), features max abs err %.3e'
-              % (name, 'simt' if simt else 'wgmma', e[0], float(ref[..., 0].abs().max()), e[1]))
-    _check_pair(out[False], out[True], ref, d)
-    for simt in (False, True):
-        again = _launch(planes, mlp, d, simt)
-        assert _same_bits(again[0], out[simt][0]) and (not d.n_feat or _same_bits(again[1], out[simt][1])), 'two launches differ'
+    out = _launch(planes, mlp, d)
+    e = _check_volume(out, ref, d)
+    print('%s forward: sdf max abs err %.3e (|sdf| max %.2f), features max abs err %.3e'
+          % (name, e[0], float(ref[..., 0].abs().max()), e[1]))
+    again = _launch(planes, mlp, d)
+    assert _same_bits(again[0], out[0]) and (not d.n_feat or _same_bits(again[1], out[1])), 'two launches differ'
     # the torch front end allocates the buffers and zeroes the feature pad channels; same kernel, same bits elsewhere
     vs, vf = ops.tpv_decode(*planes, *mlp, d)
-    assert torch.equal(vs, out[False][0])
+    assert torch.equal(vs, out[0])
     if d.n_feat:
-        assert torch.equal(vf[..., :d.n_feat], out[False][1][..., :d.n_feat]) and (vf[..., d.n_feat:] == 0).all()
+        assert torch.equal(vf[..., :d.n_feat], out[1][..., :d.n_feat]) and (vf[..., d.n_feat:] == 0).all()
 
 
 # ---- 2. the persistent loop and the instantiations ---------------------------------------------------------------------------
@@ -188,7 +171,7 @@ N_OUT = (1, 2, 4, 5, 25, 32)       # instantiations NOUT = 1 | 4 | 32 cover n_ou
 
 
 def _dec_stages(Cc, n_out):
-    """dec_smem of decode.cu: ring stages left beside the resident W1 hi / lo (below 2 the SIMT kernel takes over)."""
+    """dec_smem of decode.cu: ring stages left beside the resident W1 hi / lo (the pipeline needs at least 2)."""
     fixed = 2 * (Cc // 32) * Cc * 128 + n_out * Cc * 4 + Cc * 4 + 128 + 256
     return min(4, (227 * 1024 - 1024 - fixed) // (2 * 128 * 128))
 
@@ -209,17 +192,12 @@ def test_forward_tile_loop_masks_and_instantiations(geom):
             d = _desc(H, W, Z, n_out - 1)
             planes, mlp = _inputs(d, Cc, seed=Cc + n_out)
             ref = _oracle(planes, mlp, d)
-            tc, simt = _launch(planes, mlp, d, False), _launch(planes, mlp, d, True)
-            for out in (tc, simt):
-                e = _check_volume(out, ref, d)
-                worst = [max(a, b) for a, b in zip(worst, e)]
-            _check_pair(tc, simt, ref, d)
-            # the two kernels round differently (3xTF32 products, another summation order): equal bits would mean the
-            # launch fell back to the SIMT kernel.  Every listed size leaves the ring at least 2 stages (C = 128 with
-            # n_out = 32 exactly 2), so the wgmma kernel is what ran.
-            assert _dec_stages(Cc, n_out) >= 2 and not _same_bits(tc[0], simt[0])
+            e = _check_volume(_launch(planes, mlp, d), ref, d)
+            worst = [max(a, b) for a, b in zip(worst, e)]
+            # every listed size leaves the ring at least 2 stages (C = 128 with n_out = 32 exactly 2)
+            assert _dec_stages(Cc, n_out) >= 2
     assert _dec_stages(128, 32) == 2 and _dec_stages(96, 4) == 4
-    print('%s: H %d W %d Z %d, %d tiles on %d SMs, %d (C, n_out) pairs x 2 kernels: sdf max abs err %.3e, features %.3e'
+    print('%s: H %d W %d Z %d, %d tiles on %d SMs, %d (C, n_out) pairs: sdf max abs err %.3e, features %.3e'
           % (geom, H, W, Z, tiles, sms, len(CHANNELS) * len(N_OUT), *worst))
 
 
@@ -245,19 +223,18 @@ def test_unsupported_widths_are_refused_before_any_launch():
 
 
 @gpu
-@pytest.mark.parametrize('simt', [False, True])
-def test_row_slabs_write_their_rows_only_and_tile_the_whole_launch(simt):
+def test_row_slabs_write_their_rows_only_and_tile_the_whole_launch():
     """so_tpv_decode_rows at the nuScenes novel-depth volume: ragged slabs, a one-row first and last slab, an empty one."""
     _dev()
     d = _shipped_desc('nuScenes_novel_depth')
     planes, mlp = _inputs(d, 96, seed=12)
     ref = _oracle(planes, mlp, d)
-    whole = _launch(planes, mlp, d, simt)
+    whole = _launch(planes, mlp, d)
     _check_volume(whole, ref, d)
     union = None
     for rows in ((100, 0), (0, 1), (1, 32), (33, 223), (256, 1)):
-        _check_volume(_launch(planes, mlp, d, simt, rows=rows), ref, d, rows=rows)
-        union = _launch(planes, mlp, d, simt, rows=rows, out=union)
+        _check_volume(_launch(planes, mlp, d, rows=rows), ref, d, rows=rows)
+        union = _launch(planes, mlp, d, rows=rows, out=union)
     assert _same_bits(union[0], whole[0]) and _same_bits(union[1], whole[1])
 
 
@@ -313,12 +290,9 @@ def test_forward_over_the_whole_activation_domain():
     assert f.min() < -40 and f.max() > 40 and (f[0, ..., 16] == 0).all() and (f[1, ..., 17] == 20).all() and (f[1, ..., 18] == -20).all()
     assert 0 < f[..., 19].max() < 1e-38
     ref = _oracle(planes, mlp, d)
-    tc, simt = _launch(planes, mlp, d, False), _launch(planes, mlp, d, True)
-    for name, out in (('wgmma', tc), ('simt', simt)):
-        e = _check_volume(out, ref, d)
-        print('wide inputs (%s): sdf max abs err %.3e (|sdf| max %.2f), features max abs err %.3e (|f| max %.2f)'
-              % (name, e[0], float(ref[..., 0].abs().max()), e[1], float(ref[..., 1:].abs().max())))
-    _check_pair(tc, simt, ref, d)
+    e = _check_volume(_launch(planes, mlp, d), ref, d)
+    print('wide inputs: sdf max abs err %.3e (|sdf| max %.2f), features max abs err %.3e (|f| max %.2f)'
+          % (e[0], float(ref[..., 0].abs().max()), e[1], float(ref[..., 1:].abs().max())))
 
 
 @gpu
@@ -394,12 +368,14 @@ def _cotangent(d, kind, seed):
 def _backward(planes, mlp, d, g_vs, g_vf, mode, monkeypatch):
     from selfocc_b200 import ops
     assert ops.TPVDecodeFunction.SLAB_ROWS == 32
-    monkeypatch.setenv('SELFOCC_B200_DECODE_BWD', mode)
-    ins = [t.clone().requires_grad_(True) for t in (*planes, *mlp)]
-    vs, vf = ops.TPVDecodeFunction.apply(*ins, d)
-    if d.n_feat:
-        return torch.autograd.grad([vs, vf], ins, [g_vs, g_vf])
-    return torch.autograd.grad([vs], ins, [g_vs])
+    with monkeypatch.context() as m:               # the next case's 'native' run must take the native path again
+        if mode == 'torch':
+            m.setattr(ops.TPVDecodeFunction, '_backward_native', ops.TPVDecodeFunction._backward_torch)
+        ins = [t.clone().requires_grad_(True) for t in (*planes, *mlp)]
+        vs, vf = ops.TPVDecodeFunction.apply(*ins, d)
+        if d.n_feat:
+            return torch.autograd.grad([vs, vf], ins, [g_vs, g_vf])
+        return torch.autograd.grad([vs], ins, [g_vs])
 
 
 def _grad_report(tag, got, ref, b1_mass):

@@ -146,14 +146,11 @@ def test_pixel_table_equals_in_kernel_grid():
     assert torch.allclose(a['depth'], b['depth'], rtol=1e-5)
 
 
-@pytest.mark.parametrize('simt', [False, True])
 @pytest.mark.parametrize('C,n_feat,hw,d', [(96, 0, 12, 6), (96, 24, 8, 5), (32, 3, 6, 4), (128, 0, 5, 9)])
-def test_tpv_decode_matches_oracle(C, n_feat, hw, d, simt):
-    """Both decode kernels: wgmma 3xTF32 (default) and the fp32 SIMT one (forced through the test hook)."""
+def test_tpv_decode_matches_oracle(C, n_feat, hw, d):
     dev = _dev()
     from oracle import render as orender
-    from selfocc_b200 import ops, _lib
-    _lib.load().so_tpv_decode_force_simt(int(simt))
+    from selfocc_b200 import ops
     margs, _ = synth.small_mapping(hw, d)
     m = GridMeterMapping(**margs)
     planes = synth.random_planes(m, C, scale=1.0, seed=3)
@@ -161,14 +158,11 @@ def test_tpv_decode_matches_oracle(C, n_feat, hw, d, simt):
     ref = orender.tpv_decode_ref(*[p.double() for p in planes], (m.size_h, m.size_w, m.size_d), w1.double(), b1.double(),
                                  w2.double(), b2.double()).float()
     desc = m.volume_desc(n_feat)
-    try:
-        vs, vf = ops.tpv_decode(*[p.to(dev) for p in planes], w1.to(dev), b1.to(dev), w2.to(dev), b2.to(dev), desc)
-        vs, vf = vs.cpu(), (vf.cpu() if vf is not None else None)
-    finally:
-        _lib.load().so_tpv_decode_force_simt(0)
+    vs, vf = ops.tpv_decode(*[p.to(dev) for p in planes], w1.to(dev), b1.to(dev), w2.to(dev), b2.to(dev), desc)
+    vs, vf = vs.cpu(), (vf.cpu() if vf is not None else None)
     assert torch.all(vs[..., m.size_d:] == 0)
     err = (vs[..., :m.size_d] - ref[0]).abs().max().item()
-    print('decode (%s) sdf max abs err %.3e (|sdf| max %.2f)' % ('simt' if simt else 'wgmma', err, ref[0].abs().max().item()))
+    print('decode sdf max abs err %.3e (|sdf| max %.2f)' % (err, ref[0].abs().max().item()))
     assert err < 2e-5 * max(1.0, ref[0].abs().max().item())
     if n_feat:
         assert torch.allclose(vf[..., :n_feat], ref[1:].permute(1, 2, 3, 0), atol=5e-5, rtol=1e-5)

@@ -273,7 +273,7 @@ def test_head_forward_with_the_shipped_occ_config_options():
 def test_decode_backward_native_matches_oracle_autograd(n_feat, hw, d, slab, monkeypatch):
     """TPVDecodeFunction.backward, native slab path (wgmma GEMMs + so_tpv_decode_bwd_*): gradients of every plane and
     MLP parameter vs fp64 autograd through the oracle's decode (oracle/render.py:tpv_decode_ref), with several ragged slabs;
-    the torch/cuBLAS restatement of the same slab (SELFOCC_B200_DECODE_BWD=torch) must agree as well."""
+    the torch/cuBLAS restatement of the same slab (_backward_torch) must agree as well."""
     dev = _dev()
     from oracle import render as orender
     from selfocc_b200 import ops
@@ -295,7 +295,8 @@ def test_decode_backward_native_matches_oracle_autograd(n_feat, hw, d, slab, mon
     gref = torch.autograd.grad(loss, ins64)
 
     def run(mode):
-        monkeypatch.setenv('SELFOCC_B200_DECODE_BWD', mode)
+        if mode == 'torch':
+            monkeypatch.setattr(ops.TPVDecodeFunction, '_backward_native', ops.TPVDecodeFunction._backward_torch)
         monkeypatch.setattr(ops.TPVDecodeFunction, 'SLAB_ROWS', slab)
         ins = [t.to(dev).requires_grad_(True) for t in (*planes, *mlp)]
         vs, vf = ops.TPVDecodeFunction.apply(*ins, desc)

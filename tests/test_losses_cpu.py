@@ -232,4 +232,4 @@ def test_sample_mean_entry_points_reject_bad_arguments_without_a_gpu():
     assert fwd(C.c_void_p(18), 12, 1, ws, one, N) == -1                                   # x not 4-byte aligned
     assert fwd(one, 12, 1, C.c_void_p(20), one, N) == -1                                  # workspace not 8-byte aligned
     assert bwd(one, 12, 1, one, C.c_void_p(18), N) == -1
-    assert lib.so_abi_version() == 9
+    assert lib.so_abi_version() == 10
