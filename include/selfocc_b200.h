@@ -522,6 +522,59 @@ int so_reproj_stats_backward(const float* ts, const float* deltas, const float* 
 int so_sample_mean_forward(const float* x, int64_t n, int32_t op, void* workspace, float* out, void* stream);
 int so_sample_mean_backward(const float* x, int64_t n, int32_t op, const float* grad_out, float* grad_x, void* stream);
 
+/* ---------------------------------------------------------------------------------------
+ * 8f-2  training render with the objective's per-sample terms fused in.  Renders exactly as so_render_train_forward
+ * (same sampling, field, alpha, compositing and kernel choice: the per-ray outputs are bit-identical) and, instead of
+ * storing the per-sample tensors the losses read, reduces them per ray while it renders:
+ *   reprojection (reproj_mode SO_REPROJ_COMBINE / SO_REPROJ_MULTI_NEW): reproj_stats [rays, 6 * sets] and reproj_colours
+ *     [rays, 9] (NULL ok) with the contract and the arithmetic of so_reproj_stats_forward with deltas == NULL, from the
+ *     weights and ts of the render.  Row i is flat ray ray_begin + i, of camera (ray_begin + i) / rays_per_cam and loss pixel
+ *     pix[(ray_begin + i) % rays_per_cam]; images and matrices are indexed by that camera.
+ *   eikonal (eikonal = 1): eikonal_mean [1] = mean over the call's rays x S samples of (|eik_grad| - 1)^2, as
+ *     so_sample_mean_forward(EIKONAL): per-ray fp64 sums in `workspace` (8-byte aligned, >= 8 * ray_count bytes), then one
+ *     index-ordered pass.  Deterministic, no float atomics, the same value on every device.
+ * The per-sample outputs of so_render_train_forward stay available and NULL = not written (a head that also needs the
+ * sample positions asks for ts / deltas).
+ * so_render_train_objective_backward recomputes the forward as so_render_train_backward does and forms every sample's
+ * d loss / d w (the adjoint of so_reproj_stats_backward: reproj_stats = the forward's, grad_reproj_stats [rays, 6 * sets])
+ * and d loss / d eik_grad (the adjoint of so_sample_mean_backward: grad_eikonal_mean [1] on the device, NULL = 0, never
+ * read on the host) in registers; with the per-ray g_depth / g_acc / g_rgb / g_sem it ACCUMULATES into g_vol_sdf,
+ * g_vol_feat and g_inv_s as so_render_train_backward does (the caller zero-fills them).  g_inv_s is formed from per-ray
+ * fp64 values in `workspace` (as the forward's eikonal sums: >= 8 * ray_count bytes when g_inv_s != NULL) summed in ray
+ * order, so it is the same on every run; g_vol_sdf / g_vol_feat are accumulated with atomics.
+ * Argument errors return SO_ERR_INVALID_ARG / SO_ERR_UNSUPPORTED before any launch: the checks of so_render_train_forward /
+ * _backward (S <= 256) and, for the objective, those of so_reproj_stats_forward (operands, image sizes) plus 4-byte
+ * alignment of every float operand. */
+#define SO_OBJECTIVE_NO_REPROJ (-1)
+typedef struct so_objective_desc {
+  int32_t reproj_mode;       /* SO_REPROJ_COMBINE, SO_REPROJ_MULTI_NEW or SO_OBJECTIVE_NO_REPROJ */
+  int32_t eikonal;           /* 1: the eikonal mean is computed, 0: not */
+  const float* pix;          /* [rays_per_cam, 2] (x, y) loss pixel of each ray */
+  const float* img2prev;     /* [n_cam, 4, 4] img2prevImg */
+  const float* img2next;     /* [n_cam, 4, 4] img2nextImg */
+  const float* curr_imgs;    /* [n_cam, 3, img_h, img_w] fp32 */
+  const float* prev_imgs;
+  const float* next_imgs;
+  int32_t img_h, img_w;
+  float size_h, size_w;      /* the loss's img_size */
+  void* workspace;           /* forward with eikonal, backward with g_inv_s: >= 8 * ray_count bytes, 8-byte aligned */
+  int64_t workspace_bytes;
+} so_objective_desc;
+int so_render_train_objective_forward(const float* vol_sdf, const float* vol_feat, const so_volume_desc* vol_host,
+                                      const float* cam_mats, const float* pix, const so_ray_desc* rays_host,
+                                      const so_render_params* params_host, const float* jitter, const float* bkgd_rand,
+                                      const so_objective_desc* objective, float* depth, float* acc, float* fars, float* rgb,
+                                      float* sem, float* max_depth, float* weights, float* ts, float* deltas, float* eik_grad,
+                                      float* sample_sdf, float* reproj_stats, float* reproj_colours, float* eikonal_mean,
+                                      float* workspace, float* pair_workspace, void* stream);
+int so_render_train_objective_backward(const float* vol_sdf, const float* vol_feat, const so_volume_desc* vol_host,
+                                       const float* cam_mats, const float* pix, const so_ray_desc* rays_host,
+                                       const so_render_params* params_host, const float* jitter, const float* bkgd_rand,
+                                       const so_objective_desc* objective, const float* g_depth, const float* g_acc,
+                                       const float* g_rgb, const float* g_sem, const float* reproj_stats,
+                                       const float* grad_reproj_stats, const float* grad_eikonal_mean, float* g_vol_sdf,
+                                       float* g_vol_feat, float* g_inv_s, float* workspace, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -33,6 +33,13 @@ class RenderParams(C.Structure):
                 ('anchor_mid', C.c_int32), ('sh_act', C.c_int32), ('bkgd_mode', C.c_int32)]
 
 
+class ObjectiveDesc(C.Structure):
+    _fields_ = [('reproj_mode', C.c_int32), ('eikonal', C.c_int32), ('pix', C.c_void_p), ('img2prev', C.c_void_p),
+                ('img2next', C.c_void_p), ('curr_imgs', C.c_void_p), ('prev_imgs', C.c_void_p), ('next_imgs', C.c_void_p),
+                ('img_h', C.c_int32), ('img_w', C.c_int32), ('size_h', C.c_float), ('size_w', C.c_float),
+                ('workspace', C.c_void_p), ('workspace_bytes', C.c_int64)]
+
+
 _P = C.c_void_p
 _I = C.c_int32
 _L = C.c_int64
@@ -101,6 +108,10 @@ SIGNATURES = {
     'so_occ_confusion': (C.c_int, [_P, _P, _P, _L, _I, _I, _P, _P]),
     'so_sample_mean_forward': (C.c_int, [_P, _L, _I, _P, _P, _P]),
     'so_sample_mean_backward': (C.c_int, [_P, _L, _I, _P, _P, _P]),
+    'so_render_train_objective_forward': (C.c_int, [_P, _P, C.POINTER(VolumeDesc), _P, _P, C.POINTER(RayDesc),
+                                                    C.POINTER(RenderParams), _P, _P, C.POINTER(ObjectiveDesc)] + [_P] * 17),
+    'so_render_train_objective_backward': (C.c_int, [_P, _P, C.POINTER(VolumeDesc), _P, _P, C.POINTER(RayDesc),
+                                                     C.POINTER(RenderParams), _P, _P, C.POINTER(ObjectiveDesc)] + [_P] * 12),
 }
 
 _lib = None

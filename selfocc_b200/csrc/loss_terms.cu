@@ -7,7 +7,7 @@
 // mean.  No float atomics: the result is bitwise repeatable on any device.
 // Backward: one read of x and one write of grad_x, the scale grad_out[0] / count read on the device.
 #include <algorithm>
-#include "common.cuh"
+#include "eikonal_terms.cuh"
 
 namespace so {
 namespace {
@@ -16,30 +16,17 @@ constexpr int kThreads = 256;
 constexpr int kMaxPartials = SO_SAMPLE_MEAN_WORKSPACE_BYTES / 8;
 static_assert(kMaxPartials == 1024, "the finalising CTA reduces one partial per thread");
 
-// ---- the three elementwise functions and their torch subgradients
-__device__ __forceinline__ float eik_norm(float x, float y, float z) { return sqrtf(fmaf(x, x, fmaf(y, y, z * z))); }
-
+// ---- the elementwise functions of ABS and NEG_RELU and their torch subgradients (EIKONAL: eikonal_terms.cuh)
 template <int OP>
 __device__ __forceinline__ double f_scalar(float x) {
   if (OP == SO_SAMPLE_MEAN_ABS) return (double)fabsf(x);
   return x < 0.f ? -(double)x : 0.0;                               // relu(-x)
 }
 
-__device__ __forceinline__ double f_row(float x, float y, float z) {
-  const double d = (double)eik_norm(x, y, z) - 1.0;
-  return d * d;
-}
-
 template <int OP>
 __device__ __forceinline__ float df_scalar(float x, float s) {
   if (OP == SO_SAMPLE_MEAN_ABS) return x > 0.f ? s : (x < 0.f ? -s : 0.f);   // sign(x) * s, 0 at 0
   return x < 0.f ? -s : 0.f;                                                 // 0 at x = 0
-}
-
-// 2 (|g| - 1) g / |g| * s, 0 where |g| = 0 (vector_norm's backward masks zero norms)
-__device__ __forceinline__ float eik_coef(float x, float y, float z, float s) {
-  const float n = eik_norm(x, y, z);
-  return n > 0.f ? 2.f * (n - 1.f) * s / n : 0.f;
 }
 
 // Work split: `head` scalar units before the first aligned word, `nvec` vector items, then the tail.  A unit is one
@@ -92,7 +79,7 @@ __global__ void __launch_bounds__(kThreads) sample_mean_partial_kernel(const flo
     const float4* v = reinterpret_cast<const float4*>(x + 3 * sp.head);
     for (int64_t i = tid; i < sp.nvec; i += stride) {
       const float4 a = __ldcs(v + 3 * i), b = __ldcs(v + 3 * i + 1), c = __ldcs(v + 3 * i + 2);
-      acc += f_row(a.x, a.y, a.z) + f_row(a.w, b.x, b.y) + f_row(b.z, b.w, c.x) + f_row(c.y, c.z, c.w);
+      acc += eik_row(a.x, a.y, a.z) + eik_row(a.w, b.x, b.y) + eik_row(b.z, b.w, c.x) + eik_row(c.y, c.z, c.w);
     }
   } else {
     const float4* v = reinterpret_cast<const float4*>(x + sp.head);
@@ -112,7 +99,7 @@ __global__ void __launch_bounds__(kThreads) sample_mean_partial_kernel(const flo
   for (int64_t j = tid; j < sp.head + n_tail; j += stride) {
     const int64_t u = j < sp.head ? j : sp.tail_begin + (j - sp.head);
     if (OP == SO_SAMPLE_MEAN_EIKONAL)
-      acc += f_row(x[3 * u], x[3 * u + 1], x[3 * u + 2]);
+      acc += eik_row(x[3 * u], x[3 * u + 1], x[3 * u + 2]);
     else
       acc += f_scalar<OP>(x[u]);
   }

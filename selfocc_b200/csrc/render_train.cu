@@ -7,6 +7,8 @@
 // transmittance is an exclusive product scan along the sample dimension done with warp shuffles (5 steps per
 // 32-sample chunk + a carried prefix); the backward needs the matching suffix sums and runs the chunks in reverse.
 #include "render_common.cuh"
+#include "render_objective.cuh"
+#include <type_traits>
 #ifndef SO_TRAIN_FWD_MIN_CTAS
 #define SO_TRAIN_FWD_MIN_CTAS 8   // H100 SXM (700 W), cfg-5 sizes, Cf = 25: 0.664-0.668 ms, 4 CTAs/SM the same; latency-bound
 #endif
@@ -231,9 +233,10 @@ __device__ __forceinline__ void colour_act(const RenderDev& P, const float f[3],
 
 // FAST = affine metre->grid map, S a power of two (multiple of 32), cos-anneal finished, mid-point anchor: lean per-sample
 // path (closed-form jittered edges, interior gather chosen by a warp vote, base-2 alpha), ~2.4x fewer instructions.
-template <bool HAS_RGB, int SEM, bool FAST>
+// OBJ: kObjOff, or the objective folded in (render_objective.cuh)
+template <bool HAS_RGB, int SEM, bool FAST, int OBJ>
 __global__ void __launch_bounds__(128, SEM == 24 ? SO_TRAIN_FWD24_MIN_CTAS : SO_TRAIN_FWD_MIN_CTAS) render_train_fwd_kernel(VolumeDev V, RayDev R, RenderDev P, const float* __restrict__ ws,
-                                                               const float* __restrict__ bkgd_rand, TrainOut O) {
+                                                               const float* __restrict__ bkgd_rand, TrainOut O, ObjectiveDev D) {
   constexpr bool HAS_SEM = SEM != 0;
   const int lane = threadIdx.x & 31;
   const long long warps = (long long)gridDim.x * (blockDim.x >> 5);
@@ -245,6 +248,8 @@ __global__ void __launch_bounds__(128, SEM == 24 ? SO_TRAIN_FWD24_MIN_CTAS : SO_
     long long gid = R.ray_begin + ray;
     RayCtx c;
     make_ctx(V, R, P, gid, c);
+    ObjFwd<OBJ> ob;
+    if (OBJ) { const int cam = (int)(gid / R.rays_per_cam); ob.begin(D, cam, (int)(gid - (long long)cam * R.rays_per_cam), ray, lane); }
     const float nrm = c.nrm, tf = c.tf;
     float carry = 1.0f, acc = 0.f, dsum = 0.f, cr = 0.f, cg = 0.f, cb = 0.f;
     float best = -INFINITY, best_ts = 0.f;
@@ -304,6 +309,7 @@ __global__ void __launch_bounds__(128, SEM == 24 ? SO_TRAIN_FWD24_MIN_CTAS : SO_
         if (O.deltas) O.deltas[oidx] = dl;
         if (O.sdf) O.sdf[oidx] = q.sdf;
         if (O.eik) { O.eik[3 * oidx] = q.gx; O.eik[3 * oidx + 1] = q.gy; O.eik[3 * oidx + 2] = q.gz; }
+        if (OBJ) ob.sample(D, w, ts, q.gx, q.gy, q.gz);
         acc += w;
         dsum = fmaf(w, q.mid, dsum);
         float cand = (dl < eps ? 0.f : w) * __fdividef(1.0f, fmaxf(dl, eps));  // neus_head.py:579-587
@@ -349,6 +355,7 @@ __global__ void __launch_bounds__(128, SEM == 24 ? SO_TRAIN_FWD24_MIN_CTAS : SO_
       if (ob > best || (ob == best && oi < best_i)) { best = ob; best_i = oi; best_ts = ot; }
     }
     if (HAS_RGB) { cr = warp_sum(cr); cg = warp_sum(cg); cb = warp_sum(cb); }
+    if (OBJ) ob.end(D, ray, lane);
     if (SEM == 24) {
 #pragma unroll
       for (int c = 0; c < kSem24; ++c) sem_acc[c] = warp_sum(sem_acc[c]);
@@ -427,10 +434,11 @@ __device__ __forceinline__ void prefetch_global(const void* p) {
 }
 
 // ZP / WZP: compile-time zpitch and W * zpitch (0 = take them from the descriptor)
-template <bool HAS_RGB, bool PAIR, int ZP, int WZP>
+// OBJ: kObjOff, or the objective folded in (render_objective.cuh)
+template <bool HAS_RGB, bool PAIR, int ZP, int WZP, int OBJ>
 __global__ void __launch_bounds__(32 * SO_TRAIN_FWD5_WARPS, SO_TRAIN_FWD5_MIN_CTAS)
 render_train_fwd5_kernel(VolumeDev V, RayDev R, RenderDev P, const float* __restrict__ ws, const float2* __restrict__ vpair,
-                         const float* __restrict__ bkgd_rand, TrainOut O) {
+                         const float* __restrict__ bkgd_rand, TrainOut O, ObjectiveDev D) {
   constexpr int B = SO_TRAIN_FWD5_BATCH, U = SO_TRAIN_FWD5_U;
   constexpr unsigned kFull = 0xffffffffu;
   const int lane = threadIdx.x & 31;
@@ -471,6 +479,12 @@ render_train_fwd5_kernel(VolumeDev V, RayDev R, RenderDev P, const float* __rest
       float carry = 1.0f, acc = 0.f, dsum = 0.f, cr = 0.f, cg = 0.f, cb = 0.f;
       float best = -INFINITY, best_ts = 0.f;
       int best_i = 0x7fffffff;
+      ObjFwd<OBJ> ob;
+      if (OBJ) {
+        const long long gid = R.ray_begin + ray;
+        const int cam = (int)(gid / R.rays_per_cam);
+        ob.begin(D, cam, (int)(gid - (long long)cam * R.rays_per_cam), ray, lane);
+      }
 #if SO_TRAIN_FWD5_AHEAD
       float ucur[U], unx = 0.f;           // jitter of the current group's samples / of the first edge of the next group
 #pragma unroll
@@ -597,6 +611,7 @@ render_train_fwd5_kernel(VolumeDev V, RayDev R, RenderDev P, const float* __rest
           if (O.deltas) __stcs(O.deltas + oidx, dl);
           if (O.sdf) __stcs(O.sdf + oidx, sdf[j]);
           if (O.eik) { __stcs(O.eik + 3 * oidx, gx[j]); __stcs(O.eik + 3 * oidx + 1, gy[j]); __stcs(O.eik + 3 * oidx + 2, gz[j]); }
+          if (OBJ) ob.sample(D, w, ts, gx[j], gy[j], gz[j]);
           acc += w;
           dsum = fmaf(w, mid[j], dsum);
           if (want_max) {
@@ -623,6 +638,7 @@ render_train_fwd5_kernel(VolumeDev V, RayDev R, RenderDev P, const float* __rest
         }
       }
       if (HAS_RGB) { cr = warp_sum(cr); cg = warp_sum(cg); cb = warp_sum(cb); }
+      if (OBJ) ob.end(D, ray, lane);
       if (lane == b) { r_acc = acc; r_dsum = dsum; r_best = best_ts; if (HAS_RGB) { r_cr = cr; r_cg = cg; r_cb = cb; } }
     }
     // ---- per-ray tail of ray (ray0 + lane)
@@ -679,10 +695,12 @@ __device__ __forceinline__ void scatter_feat(const VolumeDev& V, float* __restri
   }
 }
 
-// FAST: recompute the samples with the arithmetic of the FAST forwards (sample_geom<true>, neus_alpha_log2)
-template <bool HAS_RGB, int SEM, bool FAST>
+// FAST: recompute the samples with the arithmetic of the FAST forwards (sample_geom<true>, neus_alpha_log2).
+// OBJ: kObjOff, or the objective folded in (render_objective.cuh): the sample's d loss / d w and the eikonal gradient
+// come from the objective instead of G.g_weights / G.g_eik.
+template <bool HAS_RGB, int SEM, bool FAST, int OBJ>
 __global__ void __launch_bounds__(128, SEM == 24 ? SO_TRAIN_BWD24_MIN_CTAS : 1) render_train_bwd_kernel(VolumeDev V, RayDev R, RenderDev P, const float* __restrict__ ws,
-                                                               const float* __restrict__ bkgd_rand, TrainGrad G) {
+                                                               const float* __restrict__ bkgd_rand, TrainGrad G, ObjectiveDev D) {
   constexpr bool HAS_SEM = SEM != 0;
   const int lane = threadIdx.x & 31;
   const long long warps = (long long)gridDim.x * (blockDim.x >> 5);
@@ -694,6 +712,9 @@ __global__ void __launch_bounds__(128, SEM == 24 ? SO_TRAIN_BWD24_MIN_CTAS : 1) 
     long long gid = R.ray_begin + ray;
     RayCtx c;
     make_ctx(V, R, P, gid, c);
+    ObjBwd<OBJ> ob;
+    float g_invs_ray = 0.f;      // OBJ: this ray's d loss / d inv_s (summed in ray order after the launch)
+    if (OBJ) { const int cam = (int)(gid / R.rays_per_cam); ob.begin(D, cam, (int)(gid - (long long)cam * R.rays_per_cam), ray); }
     const float nrm = c.nrm;
     const float* d = c.d;
     // ---- pass 1: transmittance per sample, ray sums
@@ -740,7 +761,8 @@ __global__ void __launch_bounds__(128, SEM == 24 ? SO_TRAIN_BWD24_MIN_CTAS : 1) 
       float w = alpha * T;
       long long oidx = ray * S + (live ? s : S - 1);
       // dL/dw_s
-      float Gw = (G.g_weights ? G.g_weights[oidx] : 0.f) + ga + gd * (q.mid - draw) / (acc + 1e-10f);
+      const float g_w = OBJ ? ob.g_w(D, q.mid * c.inv_nrm) : (G.g_weights ? G.g_weights[oidx] : 0.f);
+      float Gw = g_w + ga + gd * (q.mid - draw) / (acc + 1e-10f);
       float col[3] = {0.f, 0.f, 0.f}, raw[3] = {0.f, 0.f, 0.f};
       float lg[SEM == 24 ? 24 : (HAS_SEM ? kMaxSem : 1)];      // SEM == 24: the 24 gathered channels, then [3..23] = softmax
       float gdot = 0.f;
@@ -785,7 +807,7 @@ __global__ void __launch_bounds__(128, SEM == 24 ? SO_TRAIN_BWD24_MIN_CTAS : 1) 
       float db = -q.pb * (1.0f - q.pb) / den;
       float g_sdf = dalpha * (da + db) * P.inv_s;
       float g_half = dalpha * (db - da) * P.inv_s;
-      g_invs_local += dalpha * (da * (q.sdf - q.half) + db * (q.sdf + q.half));
+      (OBJ ? g_invs_ray : g_invs_local) += dalpha * (da * (q.sdf - q.half) + db * (q.sdf + q.half));
       // half = ic * delta / 2,  ic = -(relu(-tc/2 + 1/2)(1-r) + relu(-tc) r)
       float dic = 0.f;
       if (fmaf(-q.tc, 0.5f, 0.5f) > 0.f) dic += 0.5f * (1.0f - P.cos_anneal);
@@ -795,6 +817,7 @@ __global__ void __launch_bounds__(128, SEM == 24 ? SO_TRAIN_BWD24_MIN_CTAS : 1) 
       if (live) {
         if (G.g_sdf) g_sdf += G.g_sdf[oidx];
         if (G.g_eik) { ggx += G.g_eik[3 * oidx]; ggy += G.g_eik[3 * oidx + 1]; ggz += G.g_eik[3 * oidx + 2]; }
+        if (OBJ) ob.add_g_eik(D, q.gx, q.gy, q.gz, ggx, ggy, ggz);
         // metre gradient (gx, gy, gz) = (dgw kw, dgh kh, dgd kd)
         scatter_sdf(V, G.g_vol_sdf, q.t, g_sdf, ggy * q.kh, ggx * q.kw, ggz * q.kd);
         if (SEM == 24 && G.g_vol_feat && (G.g_rgb || G.g_sem)) {
@@ -825,8 +848,12 @@ __global__ void __launch_bounds__(128, SEM == 24 ? SO_TRAIN_BWD24_MIN_CTAS : 1) 
         }
       }
     }
+    if (OBJ && D.inv_part) {
+      g_invs_ray = warp_sum(g_invs_ray);
+      if (lane == 0) D.inv_part[ray] = g_invs_ray;
+    }
   }
-  if (G.g_inv_s) {
+  if (!OBJ && G.g_inv_s) {
     g_invs_local = warp_sum(g_invs_local);
     if (lane == 0 && g_invs_local != 0.f) atomicAdd(G.g_inv_s, g_invs_local);
   }
@@ -912,12 +939,22 @@ extern "C" int64_t so_render_train_pair_floats(const so_volume_desc* vol_host) {
   return zpair_floats(*vol_host);
 }
 
-extern "C" int so_render_train_forward(const float* vol_sdf, const float* vol_feat, const so_volume_desc* vol_host,
-                                       const float* cam_mats, const float* pix, const so_ray_desc* rd,
-                                       const so_render_params* pr, const float* jitter, const float* bkgd_rand,
-                                       float* depth, float* acc, float* fars, float* rgb, float* sem, float* max_depth,
-                                       float* weights, float* ts, float* deltas, float* eik_grad, float* sample_sdf,
-                                       float* workspace, float* pair_workspace, void* stream) {
+// calls f(std::integral_constant<int, OBJ>) for the runtime objective `obj` (kObj*)
+template <typename F>
+static void with_obj(int obj, F&& f) {
+  switch (obj) {
+    case kObjNoReproj: f(std::integral_constant<int, kObjNoReproj>{}); break;
+    case kObjCombine: f(std::integral_constant<int, kObjCombine>{}); break;
+    case kObjMultiNew: f(std::integral_constant<int, kObjMultiNew>{}); break;
+    default: f(std::integral_constant<int, kObjOff>{}); break;
+  }
+}
+
+int so::render_train_forward_obj(const float* vol_sdf, const float* vol_feat, const so_volume_desc* vol_host, const float* cam_mats,
+                                 const float* pix, const so_ray_desc* rd, const so_render_params* pr, const float* jitter,
+                                 const float* bkgd_rand, float* depth, float* acc, float* fars, float* rgb, float* sem,
+                                 float* max_depth, float* weights, float* ts, float* deltas, float* eik_grad, float* sample_sdf,
+                                 float* workspace, float* pair_workspace, int obj, const ObjectiveDev& D, void* stream) {
   bool want_rgb = rgb != nullptr, want_sem = sem != nullptr;
   if (pair_workspace && (reinterpret_cast<uintptr_t>(pair_workspace) & 7)) return SO_ERR_INVALID_ARG;
   int rc = train_common_checks(vol_sdf, vol_feat, vol_host, cam_mats, rd, pr, workspace, want_rgb, want_sem, bkgd_rand);
@@ -937,39 +974,41 @@ extern "C" int so_render_train_forward(const float* vol_sdf, const float* vol_fe
   // non-affine mappings, S not a multiple of 32 U and the cos-anneal phase
   const bool sem24 = want_sem && V.n_feat == 24 && V.feat_pitch == 24 && (reinterpret_cast<uintptr_t>(vol_feat) & 15) == 0 && !g_force_sem_generic;
   const bool v5 = fast && !want_sem && ((P.S >> 5) % SO_TRAIN_FWD5_U) == 0 && !g_force_fwd32;
-#define SO_TRAIN_FWD(RGB, SEM, F) render_train_fwd_kernel<RGB, SEM, F><<<grid, 128, 0, st>>>(V, R, P, workspace, bkgd_rand, O)
-  if (v5) {
-    const float2* vp = nullptr;
-    if (pair_workspace) {
-      launch_zpair_pack(vol_sdf, *vol_host, pair_workspace, st);
-      note_launch(1);
-      vp = reinterpret_cast<const float2*>(pair_workspace);
-    }
-    const long long n_batches = ceil_div64(R.ray_count, SO_TRAIN_FWD5_BATCH);
-    const unsigned grid5 = (unsigned)ceil_div64(n_batches, SO_TRAIN_FWD5_WARPS);   // one batch per warp
-    const bool cp = SO_TRAIN_FWD5_CONST_PITCH && V.zpitch == 32 && V.W == 257;
+  const float2* vp = nullptr;
+  if (v5 && pair_workspace) {
+    launch_zpair_pack(vol_sdf, *vol_host, pair_workspace, st);
+    note_launch(1);
+    vp = reinterpret_cast<const float2*>(pair_workspace);
+  }
+  with_obj(obj, [&](auto o) {
+    constexpr int OBJ = decltype(o)::value;
+#define SO_TRAIN_FWD(RGB, SEM, F) render_train_fwd_kernel<RGB, SEM, F, OBJ><<<grid, 128, 0, st>>>(V, R, P, workspace, bkgd_rand, O, D)
+    if (v5) {
+      const long long n_batches = ceil_div64(R.ray_count, SO_TRAIN_FWD5_BATCH);
+      const unsigned grid5 = (unsigned)ceil_div64(n_batches, SO_TRAIN_FWD5_WARPS);   // one batch per warp
+      const bool cp = SO_TRAIN_FWD5_CONST_PITCH && V.zpitch == 32 && V.W == 257;
 #define SO_TRAIN_FWD5(RGB, PAIR, ZP, WZP) \
-  render_train_fwd5_kernel<RGB, PAIR, ZP, WZP><<<grid5, 32 * SO_TRAIN_FWD5_WARPS, 0, st>>>(V, R, P, workspace, vp, bkgd_rand, O)
+  render_train_fwd5_kernel<RGB, PAIR, ZP, WZP, OBJ><<<grid5, 32 * SO_TRAIN_FWD5_WARPS, 0, st>>>(V, R, P, workspace, vp, bkgd_rand, O, D)
 #define SO_TRAIN_FWD5_P(RGB, PAIR) do { if (cp) SO_TRAIN_FWD5(RGB, PAIR, 32, 257 * 32); else SO_TRAIN_FWD5(RGB, PAIR, 0, 0); } while (0)
-    if (want_rgb) { if (vp) SO_TRAIN_FWD5_P(true, true); else SO_TRAIN_FWD5_P(true, false); }
-    else { if (vp) SO_TRAIN_FWD5_P(false, true); else SO_TRAIN_FWD5_P(false, false); }
+      if (want_rgb) { if (vp) SO_TRAIN_FWD5_P(true, true); else SO_TRAIN_FWD5_P(true, false); }
+      else { if (vp) SO_TRAIN_FWD5_P(false, true); else SO_TRAIN_FWD5_P(false, false); }
 #undef SO_TRAIN_FWD5_P
 #undef SO_TRAIN_FWD5
-  } else if (want_sem && sem24) { if (fast) SO_TRAIN_FWD(true, 24, true); else SO_TRAIN_FWD(true, 24, false); }
-  else if (want_sem) { if (fast) SO_TRAIN_FWD(true, 1, true); else SO_TRAIN_FWD(true, 1, false); }
-  else if (want_rgb) { if (fast) SO_TRAIN_FWD(true, 0, true); else SO_TRAIN_FWD(true, 0, false); }
-  else { if (fast) SO_TRAIN_FWD(false, 0, true); else SO_TRAIN_FWD(false, 0, false); }
+    } else if (want_sem && sem24) { if (fast) SO_TRAIN_FWD(true, 24, true); else SO_TRAIN_FWD(true, 24, false); }
+    else if (want_sem) { if (fast) SO_TRAIN_FWD(true, 1, true); else SO_TRAIN_FWD(true, 1, false); }
+    else if (want_rgb) { if (fast) SO_TRAIN_FWD(true, 0, true); else SO_TRAIN_FWD(true, 0, false); }
+    else { if (fast) SO_TRAIN_FWD(false, 0, true); else SO_TRAIN_FWD(false, 0, false); }
 #undef SO_TRAIN_FWD
+  });
   note_launch(1);
   return check_launch();
 }
 
-extern "C" int so_render_train_backward(const float* vol_sdf, const float* vol_feat, const so_volume_desc* vol_host,
-                                        const float* cam_mats, const float* pix, const so_ray_desc* rd,
-                                        const so_render_params* pr, const float* jitter, const float* bkgd_rand,
-                                        const float* g_depth, const float* g_acc, const float* g_rgb, const float* g_sem,
-                                        const float* g_weights, const float* g_eik, const float* g_sdf, float* g_vol_sdf,
-                                        float* g_vol_feat, float* g_inv_s, float* workspace, void* stream) {
+int so::render_train_backward_obj(const float* vol_sdf, const float* vol_feat, const so_volume_desc* vol_host, const float* cam_mats,
+                                  const float* pix, const so_ray_desc* rd, const so_render_params* pr, const float* jitter,
+                                  const float* bkgd_rand, const float* g_depth, const float* g_acc, const float* g_rgb,
+                                  const float* g_sem, const float* g_weights, const float* g_eik, const float* g_sdf, float* g_vol_sdf,
+                                  float* g_vol_feat, float* g_inv_s, float* workspace, int obj, const ObjectiveDev& D, void* stream) {
   bool want_rgb = g_rgb != nullptr, want_sem = g_sem != nullptr;
   if (!g_vol_sdf) return SO_ERR_INVALID_ARG;
   int rc = train_common_checks(vol_sdf, vol_feat, vol_host, cam_mats, rd, pr, workspace, want_rgb, want_sem, bkgd_rand);
@@ -988,16 +1027,41 @@ extern "C" int so_render_train_backward(const float* vol_sdf, const float* vol_f
   const bool sem24 = V.n_feat == 24 && V.feat_pitch == 24 && (want_rgb || want_sem) && !g_force_sem_generic &&
                      ((reinterpret_cast<uintptr_t>(vol_feat) | reinterpret_cast<uintptr_t>(g_vol_feat)) & 15) == 0;
   const bool fast = train_fast(V, P);      // recompute the samples with the arithmetic of the paired forward
+  with_obj(obj, [&](auto o) {
+    constexpr int OBJ = decltype(o)::value;
 #define SO_TRAIN_BWD(RGB, SEM) do { \
-    if (fast) render_train_bwd_kernel<RGB, SEM, true><<<grid, 128, 0, st>>>(V, R, P, workspace, bkgd_rand, G); \
-    else render_train_bwd_kernel<RGB, SEM, false><<<grid, 128, 0, st>>>(V, R, P, workspace, bkgd_rand, G); } while (0)
-  if (sem24) SO_TRAIN_BWD(true, 24);
-  else if (want_sem) SO_TRAIN_BWD(true, 1);
-  else if (want_rgb) SO_TRAIN_BWD(true, 0);
-  else SO_TRAIN_BWD(false, 0);
+    if (fast) render_train_bwd_kernel<RGB, SEM, true, OBJ><<<grid, 128, 0, st>>>(V, R, P, workspace, bkgd_rand, G, D); \
+    else render_train_bwd_kernel<RGB, SEM, false, OBJ><<<grid, 128, 0, st>>>(V, R, P, workspace, bkgd_rand, G, D); } while (0)
+    if (sem24) SO_TRAIN_BWD(true, 24);
+    else if (want_sem) SO_TRAIN_BWD(true, 1);
+    else if (want_rgb) SO_TRAIN_BWD(true, 0);
+    else SO_TRAIN_BWD(false, 0);
 #undef SO_TRAIN_BWD
+  });
   note_launch(1);
   return check_launch();
+}
+
+extern "C" int so_render_train_forward(const float* vol_sdf, const float* vol_feat, const so_volume_desc* vol_host,
+                                       const float* cam_mats, const float* pix, const so_ray_desc* rd,
+                                       const so_render_params* pr, const float* jitter, const float* bkgd_rand,
+                                       float* depth, float* acc, float* fars, float* rgb, float* sem, float* max_depth,
+                                       float* weights, float* ts, float* deltas, float* eik_grad, float* sample_sdf,
+                                       float* workspace, float* pair_workspace, void* stream) {
+  return render_train_forward_obj(vol_sdf, vol_feat, vol_host, cam_mats, pix, rd, pr, jitter, bkgd_rand, depth, acc, fars, rgb,
+                                  sem, max_depth, weights, ts, deltas, eik_grad, sample_sdf, workspace, pair_workspace, kObjOff,
+                                  ObjectiveDev{}, stream);
+}
+
+extern "C" int so_render_train_backward(const float* vol_sdf, const float* vol_feat, const so_volume_desc* vol_host,
+                                        const float* cam_mats, const float* pix, const so_ray_desc* rd,
+                                        const so_render_params* pr, const float* jitter, const float* bkgd_rand,
+                                        const float* g_depth, const float* g_acc, const float* g_rgb, const float* g_sem,
+                                        const float* g_weights, const float* g_eik, const float* g_sdf, float* g_vol_sdf,
+                                        float* g_vol_feat, float* g_inv_s, float* workspace, void* stream) {
+  return render_train_backward_obj(vol_sdf, vol_feat, vol_host, cam_mats, pix, rd, pr, jitter, bkgd_rand, g_depth, g_acc, g_rgb,
+                                   g_sem, g_weights, g_eik, g_sdf, g_vol_sdf, g_vol_feat, g_inv_s, workspace, kObjOff,
+                                   ObjectiveDev{}, stream);
 }
 
 extern "C" int so_render_train_probe(const so_volume_desc* vol_host, const float* cam_mats, const float* pix, const so_ray_desc* rd,

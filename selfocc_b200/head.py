@@ -254,6 +254,7 @@ class NeuSHead(nn.Module):
         self.bev_size = [self.model.field.mapping.size_h, self.model.field.mapping.size_w]
         self.two_split = two_split
         self.cos_anneal_ratio = 1.0
+        self.fused_objective = None       # loss.fuse_objective: the training render computes the objective's per-sample terms
 
     # ------------------------------------------------------------------ checkpoints
     # The field's parameters follow the in-repo analogue's names (bev_nerf.py:62-71: ``density_net.{1,3}``) under

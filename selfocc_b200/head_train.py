@@ -21,7 +21,14 @@ def forward_train(head, representation, metas=None, jitter=None, bkgd_rand=None,
     torch AND numpy identically on all ranks (the reference's train.py seeds them; INTEGRATION.md lists what else it needs
     for a sharded run).  The cellular ray grid comes from numpy (RaySampler.draw); the stratified
     jitter and the random background are drawn for all rays and sliced; the uniform_sdf lattice shift and the encoder's
-    dropout masks are then drawn identically.  An explicit ``jitter`` / ``bkgd_rand`` is this rank's slice."""
+    dropout masks are then drawn identically.  An explicit ``jitter`` / ``bkgd_rand`` is this rank's slice.
+
+    Fused objective (``head.fused_objective``, set by loss.fuse_objective; training mode only): the render computes the
+    reprojection statistics and the eikonal mean itself (RenderTrainObjectiveFunction) and the outputs carry
+    ``reproj_stats`` [num_cams, R, 6 * sets], ``reproj_colours`` [num_cams, R, 9] and ``eikonal_mean`` (0-d) in place of
+    ``weights``, ``ts``, ``deltas`` and ``eik_grad``.  The reprojection term's images arrive as the model kwargs
+    ``curr_imgs`` / ``prev_imgs`` / ``next_imgs`` ([1, num_cams, 3, H, W]) and its matrices as metas' img2prevImg /
+    img2nextImg."""
     f = head.model.field
     vol_sdf, vol_feat = f.decode(representation, train=True)
     vol_feat = vol_feat if f.desc.n_feat else None
@@ -66,21 +73,29 @@ def forward_train(head, representation, metas=None, jitter=None, bkgd_rand=None,
                                     cos_anneal=head.cos_anneal_ratio, anchor_mid=head.sample_anchor == 'mid', sh_act=f.sh_act,
                                     bkgd=head.render_bkgd)
     rd = ops.make_ray_desc(num_cams, grid=grid, n_pix=num_rays)
-    want = ['depth', 'acc', 'fars', 'weights', 'ts', 'deltas', 'eik_grad']
+    fused = getattr(head, 'fused_objective', None) if training else None
+    if fused is None:
+        want = ['depth', 'acc', 'fars', 'weights', 'ts', 'deltas', 'eik_grad']
+    else:                                                  # sample positions only for the second-grad query
+        want = ['depth', 'acc', 'fars'] + (['ts', 'deltas'] if head.return_second_grad else [])
     want += ['rgb'] if has_rgb else []
     want += ['sem'] if head.return_sem else []
     want += ['max_depth'] if head.return_max_depth else []
     want += ['sample_sdf'] if head.return_sample_sdf else []
     cfg = dict(desc=f.desc, cam_mats=M[0].contiguous(), rays=rd, params=params, pix=None if grid is not None else rays.contiguous(),
                jitter=jitter, bkgd_rand=bkgd_rand, want=want)
-    res = dict(zip(ops.RenderTrainFunction.ORDER, ops.RenderTrainFunction.apply(vol_sdf, vol_feat, inv_s, cfg)))
+    if fused is None:
+        res = dict(zip(ops.RenderTrainFunction.ORDER, ops.RenderTrainFunction.apply(vol_sdf, vol_feat, inv_s, cfg)))
+    else:
+        cfg['objective'] = _objective(fused, kwargs, metas, rays, num_cams, dev)
+        res = dict(zip(ops.RenderTrainObjectiveFunction.ORDER, ops.RenderTrainObjectiveFunction.apply(vol_sdf, vol_feat, inv_s, cfg)))
 
     shp = (bs, num_cams, num_rays)
     depth, acc, fars = res['depth'].reshape(shp), res['acc'].reshape(shp), res['fars'].reshape(shp)
     rgb = res['rgb'].reshape(*shp, 3) if has_rgb else depth.new_empty(*shp, 0)
-    weights = res['weights'].reshape(*shp, S, 1)
-    ts = res['ts'].reshape(total, S, 1)
-    deltas = res['deltas'].reshape(total, S, 1)
+    if 'ts' in want:
+        ts = res['ts'].reshape(total, S, 1)
+        deltas = res['deltas'].reshape(total, S, 1)
     # img2lidar outputs kept for API parity (neus_head.py:674-676)
     origin, direction = head.img2lidar(metas, rays)
     origin = origin.unsqueeze(2).repeat(1, 1, num_rays, 1).flatten(0, 2)
@@ -91,9 +106,10 @@ def forward_train(head, representation, metas=None, jitter=None, bkgd_rand=None,
     uniform_sdf = None
     if head.return_uniform_sdf:
         uniform_sdf = _uniform_sdf_train(head, dev, uniform_shift)
-    weights_for_cams = chunk_cams(weights, num_cams)
-    ts_for_cams = chunk_cams(ts, num_cams)
-    deltas_for_cams = chunk_cams(deltas, num_cams)
+    if fused is None:
+        weights_for_cams = chunk_cams(res['weights'].reshape(*shp, S, 1), num_cams)
+        ts_for_cams = chunk_cams(ts, num_cams)
+        deltas_for_cams = chunk_cams(deltas, num_cams)
     ray_idx = [torch.arange(num_rays, device=dev).unsqueeze(-1).repeat(1, S).flatten()] * num_cams
     sem = res['sem'].reshape(*shp, -1) if head.return_sem else None
     max_depth = res['max_depth'].reshape(shp) if head.return_max_depth else None
@@ -113,9 +129,16 @@ def forward_train(head, representation, metas=None, jitter=None, bkgd_rand=None,
             sem = sem[:, half:]
 
     outputs = {'ms_depths': [depth], 'ms_colors': [rgb], 'ms_accs': [acc], 'ms_fars': [fars], 'ms_rays': rays,
-               'origin': origin, 'direction': direction, 'direction_norm': direction_norm, 'ray_indices': ray_idx,
-               'weights': weights_for_cams, 'ts': ts_for_cams, 'deltas': deltas_for_cams,
-               'eik_grad': res['eik_grad'].reshape(total, S, 3), 'uniform_sdf': uniform_sdf, 'inv_s': inv_s}
+               'origin': origin, 'direction': direction, 'direction_norm': direction_norm, 'ray_indices': ray_idx}
+    if fused is None:
+        outputs.update(weights=weights_for_cams, ts=ts_for_cams, deltas=deltas_for_cams, eik_grad=res['eik_grad'].reshape(total, S, 3))
+    else:
+        if fused['mode'] is not None:
+            outputs.update(reproj_stats=res['reproj_stats'].reshape(num_cams, num_rays, -1),
+                           reproj_colours=res['reproj_colours'].reshape(num_cams, num_rays, 9))
+        if fused['eikonal']:
+            outputs['eikonal_mean'] = res['eikonal_mean']
+    outputs.update(uniform_sdf=uniform_sdf, inv_s=inv_s)
     if head.return_max_depth:
         outputs['ms_max_depths'] = [max_depth]
     if head.return_second_grad:
@@ -132,6 +155,24 @@ def forward_train(head, representation, metas=None, jitter=None, bkgd_rand=None,
     if sharded:
         outputs['ray_shard'] = (shard[0], shard[1], r_full)
     return outputs
+
+
+def _objective(fused, kwargs, metas, rays, num_cams, dev):
+    """RenderTrainObjectiveFunction's cfg['objective'] from head.fused_objective: the reprojection term's loss pixels (the
+    rays), matrices (metas, as the loss reads them) and images (the model kwargs), and whether the eikonal mean is on."""
+    ob = dict(mode=fused['mode'], eikonal=fused['eikonal'])
+    if fused['mode'] is None:
+        return ob
+    from .loss import _mats
+    keys = ('curr_imgs', 'prev_imgs', 'next_imgs')
+    missing = [k for k in keys if kwargs.get(k) is None]
+    if missing:
+        raise ValueError('the fused objective renders the reprojection statistics from the images: call the model with '
+                         'curr_imgs=, prev_imgs=, next_imgs= (missing %s)' % missing)
+    ob.update(pix=rays.detach().float().contiguous(), img2prev=_mats(metas, 'img2prevImg', num_cams, dev),
+              img2next=_mats(metas, 'img2nextImg', num_cams, dev),
+              images=tuple(kwargs[k][0, :num_cams].float().contiguous() for k in keys), img_size=fused['img_size'])
+    return ob
 
 
 def uniform_lattice_train(head, dev):

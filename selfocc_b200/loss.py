@@ -74,7 +74,10 @@ class _ReprojLoss(nn.Module):
         self.iter_counter = 0
 
     def forward(self, inputs):
-        """BaseLoss.forward: weight * loss over the inputs named by input_dict."""
+        """BaseLoss.forward: weight * loss over the inputs named by input_dict.  With the fused objective
+        (fuse_objective) the head has already computed the per-ray statistics (inputs['reproj_stats'])."""
+        if 'reproj_stats' in inputs:
+            return self.weight * self.tail(*self._fused(inputs))
         return self.weight * self.reproj_loss(**{k: inputs[v] for k, v in self.input_dict.items()})
 
     def reproj_loss(self, curr_imgs, prev_imgs, next_imgs, ray_indices, weights, ts, metas, ms_rays, deltas=None,
@@ -83,9 +86,24 @@ class _ReprojLoss(nn.Module):
 
     # ray-sharded evaluation (MultiLoss): the per-ray statistics of this rank's rays, the tail on the gathered grid
     def local_payload(self, inputs, shard):
+        if 'reproj_stats' in inputs:
+            stats, colours, _ = self._fused(inputs, full_grid=False)
+            return [(stats, shard[2]), (colours, shard[2])]
         kw = {k: inputs[v] for k, v in self.input_dict.items() if k != 'sample_sdfs'}
         stats, colours, _ = self._stats(**kw, full_grid=False)
         return [(stats, shard[2]), (colours, shard[2])]
+
+    def _fused(self, inputs, full_grid=True):
+        """(stats, colours, num_cams) from the statistics the fused training render emitted, as _stats returns them."""
+        stats, colours = inputs['reproj_stats'], inputs['reproj_colours']
+        if stats.shape[-1] != 6 * ops.REPROJ_SETS[self.MODE]:
+            raise ValueError('reproj_stats hold %d values per ray, %s needs %d: fuse the head with this objective '
+                             '(fuse_objective)' % (stats.shape[-1], type(self).__name__, 6 * ops.REPROJ_SETS[self.MODE]))
+        R = stats.shape[1]
+        if full_grid and not self.no_ssim and R != self.ray_resize[0] * self.ray_resize[1]:
+            raise ValueError('SSIM needs the rays to fill ray_resize %s, got %d rays (ray sharding or a partial ray set: '
+                             'set no_ssim=True)' % (self.ray_resize, R))
+        return stats.double(), colours.double(), inputs[self.input_dict['curr_imgs']].shape[1]
 
     def from_gathered(self, full, inputs):
         return self.weight * self.tail(full[0], full[1], inputs[self.input_dict['curr_imgs']].shape[1])
@@ -247,6 +265,19 @@ class EikonalLoss(_SampleMeanTerm):
 
     def loss_func(self, eik_grad):
         return ops.SampleMeanFunction.apply(eik_grad, 'eikonal')
+
+    # the fused objective (fuse_objective): the head's render has already taken the mean (inputs['eikonal_mean'])
+    def forward(self, inputs):
+        if 'eikonal_mean' in inputs:
+            return self.weight * inputs['eikonal_mean']
+        return super().forward(inputs)
+
+    def local_payload(self, inputs, shard):
+        if 'eikonal_mean' not in inputs:
+            return super().local_payload(inputs, shard)
+        n = sum(t.numel() for t in inputs['ray_indices'])        # this rank's samples: the mean's count
+        part = inputs['eikonal_mean'].double() * n
+        return [(torch.stack([part, part.new_full((), float(n))]).reshape(1, 1, 2), shard[1])]
 
 
 @LOSSES.register_module()
@@ -481,6 +512,48 @@ class EdgeLoss3DMS(_Term):
 
     def from_gathered(self, full, inputs):
         return self.weight * self._tail([(d, rgb.transpose(1, 2).contiguous()) for d, rgb in zip(full[0::2], full[1::2])])
+
+
+_PER_SAMPLE_KEYS = ('weights', 'ts', 'deltas', 'eik_grad', 'sample_sdf')
+
+
+def fuse_objective(head, multi_loss):
+    """Let ``head``'s training render compute ``multi_loss``'s per-sample terms itself (so_render_train_objective_forward):
+    the reprojection term's per-ray statistics and the eikonal mean come out of the render, and the per-sample tensors
+    weights / ts / deltas / eik_grad are never written.  The losses' values and gradients are those of the unfused step.
+    The model is then called with the reprojection images as kwargs: model(..., curr_imgs=, prev_imgs=, next_imgs=).
+
+    Supported: at most one reprojection term (ReprojLossMonoMultiNewCombine or ReprojLossMonoMultiNew on the head's
+    outputs, without ``deltas`` / ``sample_sdfs`` inputs or sdf_loss), at most one EikonalLoss on ``eik_grad``, any number of
+    terms that read no per-sample output, and a head without two_split or return_sample_sdf; anything else raises
+    NotImplementedError and leaves the head unfused.  Returns what it recorded on the head (``head.fused_objective``);
+    ``head.fused_objective = None`` undoes it.  Evaluation (head.eval()) is unaffected."""
+    if head.two_split and head.img2lidar.two_split:
+        raise NotImplementedError('fuse_objective: two_split=True renders half the cameras for the reprojection term')
+    if head.return_sample_sdf:
+        raise NotImplementedError('fuse_objective: return_sample_sdf needs the per-sample sdf tensor')
+    reproj, eik = [], []
+    for term in multi_loss.losses:
+        keys = getattr(term, 'input_dict', {})
+        if isinstance(term, _ReprojLoss):
+            if 'deltas' in keys or 'sample_sdfs' in keys or getattr(term, 'sdf_loss', False):
+                raise NotImplementedError('fuse_objective: %s with deltas / sample_sdfs / sdf_loss' % type(term).__name__)
+            if any(keys.get(k, k) != k for k in _DEFAULT_KEYS):
+                raise NotImplementedError('fuse_objective: %s must read the head\'s outputs and the model\'s image kwargs '
+                                          'under their own names, got input_dict %r' % (type(term).__name__, keys))
+            reproj.append(term)
+        elif isinstance(term, EikonalLoss):
+            if keys != {'eik_grad': 'eik_grad'}:
+                raise NotImplementedError('fuse_objective: EikonalLoss must read eik_grad, got input_dict %r' % (keys,))
+            eik.append(term)
+        elif any(v in _PER_SAMPLE_KEYS for v in keys.values()):
+            raise NotImplementedError('fuse_objective: %s reads per-sample outputs %r' % (type(term).__name__, keys))
+    if len(reproj) > 1 or len(eik) > 1:
+        raise NotImplementedError('fuse_objective: at most one reprojection term and one EikonalLoss, got %d and %d'
+                                  % (len(reproj), len(eik)))
+    head.fused_objective = dict(mode=reproj[0].MODE if reproj else None,
+                                img_size=tuple(reproj[0].img_size) if reproj else None, eikonal=bool(eik))
+    return head.fused_objective
 
 
 @LOSSES.register_module()

@@ -424,6 +424,103 @@ class RenderTrainFunction(torch.autograd.Function):
         return gvs, gvf, ginv, None
 
 
+class RenderTrainObjectiveFunction(torch.autograd.Function):
+    """The training-form render with the objective's per-sample terms fused in (so_render_train_objective_forward /
+    _backward): the per-ray outputs of RenderTrainFunction, bit-identical, and instead of the per-sample tensors the
+    reprojection statistics and the eikonal mean, differentiable w.r.t. the decoded volume and inv_s.
+    forward(vol_sdf, vol_feat_or_None, inv_s[1], cfg) -> ORDER; cfg = RenderTrainFunction's cfg ('want' may name the per-ray
+    outputs and 'ts' / 'deltas') plus cfg['objective'] = dict(mode='combine' | 'multi_new' | None, eikonal=bool, and with a mode:
+    pix=[rays_per_cam, 2] loss pixels, img2prev / img2next=[n_cam, 4, 4], images=(curr, prev, next) each [n_cam, 3, H, W],
+    img_size=(h, w) of the loss).  reproj_stats [n, 6 * sets] / reproj_colours [n, 9] are ReprojStatsFunction's (row = ray),
+    eikonal_mean a 0-d tensor = SampleMeanFunction(eik_grad, 'eikonal'); entries not computed are empty tensors."""
+
+    ORDER = ('depth', 'acc', 'fars', 'max_depth', 'rgb', 'sem', 'ts', 'deltas', 'reproj_stats', 'reproj_colours', 'eikonal_mean')
+
+    @staticmethod
+    def _desc(ob, workspace=None):
+        d = _lib.ObjectiveDesc()
+        mode = ob.get('mode')
+        d.reproj_mode = -1 if mode is None else REPROJ_MODES[mode]       # SO_OBJECTIVE_NO_REPROJ
+        d.eikonal = int(bool(ob.get('eikonal')))
+        if mode is not None:
+            for k in ('pix', 'img2prev', 'img2next'):
+                _chk(ob[k], name=k)
+            curr, prev, nxt = (_chk(t, name='images') for t in ob['images'])
+            d.pix, d.img2prev, d.img2next = ob['pix'].data_ptr(), ob['img2prev'].data_ptr(), ob['img2next'].data_ptr()
+            d.curr_imgs, d.prev_imgs, d.next_imgs = curr.data_ptr(), prev.data_ptr(), nxt.data_ptr()
+            d.img_h, d.img_w = curr.shape[-2], curr.shape[-1]
+            d.size_h, d.size_w = float(ob['img_size'][0]), float(ob['img_size'][1])
+        if workspace is not None:
+            d.workspace, d.workspace_bytes = workspace.data_ptr(), workspace.numel() * workspace.element_size()
+        return d
+
+    @staticmethod
+    def forward(ctx, vol_sdf, vol_feat, inv_s, cfg):
+        lib = _lib.load()
+        desc, cam_mats, rays, params, ob = cfg['desc'], cfg['cam_mats'], cfg['rays'], cfg['params'], cfg['objective']
+        pix, jitter, bkgd = cfg.get('pix'), cfg.get('jitter'), cfg.get('bkgd_rand')
+        _chk(vol_sdf, name='vol_sdf'); _chk(vol_feat, name='vol_feat'); _chk(cam_mats, name='cam_mats')
+        _chk(pix, name='pix'); _chk(jitter, name='jitter'); _chk(bkgd, name='bkgd_rand')
+        n, S, dev = rays.ray_count, params.num_samples, vol_sdf.device
+        if jitter is not None:
+            assert jitter.shape == (rays.n_cam * rays.rays_per_cam, S + 1)
+        mode = ob.get('mode')
+        want = set(cfg['want']) | ({'reproj_stats', 'reproj_colours'} if mode is not None else set()) | \
+            ({'eikonal_mean'} if ob.get('eikonal') else set())
+        shapes = dict(depth=(n,), acc=(n,), fars=(n,), max_depth=(n,), rgb=(n, 3), sem=(n, max(desc.n_feat - 3, 0)), ts=(n, S),
+                      deltas=(n, S), reproj_stats=(n, 6 * REPROJ_SETS[mode] if mode is not None else 0), reproj_colours=(n, 9),
+                      eikonal_mean=())
+        out = {k: (torch.empty(shapes[k], device=dev) if k in want else None) for k in RenderTrainObjectiveFunction.ORDER}
+        ws = _render_ws(lib, rays, dev)
+        pair = torch.empty(lib.so_render_train_pair_floats(C.byref(desc)), device=dev) if cfg.get('zpair', True) else None
+        eik_ws = torch.empty(max(n, 1), dtype=torch.float64, device=dev) if ob.get('eikonal') else None
+        d = RenderTrainObjectiveFunction._desc(ob, eik_ws)
+        g = lambda k: _p(out[k])
+        none = _p(None)
+        _lib.check(lib.so_render_train_objective_forward(
+            _p(vol_sdf), _p(vol_feat), C.byref(desc), _p(cam_mats), _p(pix), C.byref(rays), C.byref(params), _p(jitter), _p(bkgd),
+            C.byref(d), g('depth'), g('acc'), g('fars'), g('rgb'), g('sem'), g('max_depth'), none, g('ts'), g('deltas'), none, none,
+            g('reproj_stats'), g('reproj_colours'), g('eikonal_mean'), _p(ws), _p(pair), _stream()), 'so_render_train_objective_forward')
+        ctx.cfg = cfg
+        ctx.save_for_backward(vol_sdf, vol_feat if vol_feat is not None else vol_sdf.new_empty(0),
+                              out['reproj_stats'] if out['reproj_stats'] is not None else vol_sdf.new_empty(0))
+        ctx.has_feat = vol_feat is not None
+        res = tuple(out[k] if out[k] is not None else vol_sdf.new_empty(0) for k in RenderTrainObjectiveFunction.ORDER)
+        ctx.mark_non_differentiable(res[2], res[3], res[6], res[7], res[9])   # fars, max_depth, ts, deltas, colours
+        return res
+
+    @staticmethod
+    @torch.autograd.function.once_differentiable
+    def backward(ctx, g_depth, g_acc, g_fars, g_maxd, g_rgb, g_sem, g_ts, g_deltas, g_stats, g_colours, g_eik):
+        lib = _lib.load()
+        cfg = ctx.cfg
+        vol_sdf, vol_feat, stats = ctx.saved_tensors
+        vol_feat = vol_feat if ctx.has_feat else None
+        desc, rays, params, ob = cfg['desc'], cfg['rays'], cfg['params'], cfg['objective']
+        want = set(cfg['want'])
+
+        def gr(name, t):
+            return t.contiguous() if (name in want and t is not None and t.numel()) else None
+        gd, ga, grgb, gsem = gr('depth', g_depth), gr('acc', g_acc), gr('rgb', g_rgb), gr('sem', g_sem)
+        mode = ob.get('mode')
+        gst = None
+        if mode is not None:
+            gst = _chk(g_stats.contiguous() if g_stats is not None else torch.zeros_like(stats), name='grad_stats')
+        geik = _chk(g_eik.reshape(1).contiguous(), name='grad_eikonal_mean') if (ob.get('eikonal') and g_eik is not None) else None
+        gvs = torch.zeros_like(vol_sdf)
+        gvf = torch.zeros_like(vol_feat) if vol_feat is not None else None
+        ginv = torch.zeros(1, device=vol_sdf.device)
+        ws = _render_ws(lib, rays, vol_sdf.device)
+        inv_ws = torch.empty(max(rays.ray_count, 1), dtype=torch.float64, device=vol_sdf.device)    # per-ray d / d inv_s
+        d = RenderTrainObjectiveFunction._desc(ob, inv_ws)
+        _lib.check(lib.so_render_train_objective_backward(
+            _p(vol_sdf), _p(vol_feat), C.byref(desc), _p(cfg['cam_mats']), _p(cfg.get('pix')), C.byref(rays), C.byref(params),
+            _p(cfg.get('jitter')), _p(cfg.get('bkgd_rand')), C.byref(d), _p(gd), _p(ga), _p(grgb), _p(gsem),
+            _p(stats if mode is not None else None), _p(gst), _p(geik), _p(gvs), _p(gvf), _p(ginv), _p(ws), _stream()),
+            'so_render_train_objective_backward')
+        return gvs, gvf, ginv, None
+
+
 def render_train_probe(desc, cam_mats, rays, params, pix=None, jitter=None):
     """Test probe (so_render_train_probe): [n, S, 3], the fp32 (h, w, d) grid coordinates of every sample as the training
     forward and its backward compute them for these operands."""
