@@ -277,6 +277,19 @@ int so_depth_metric_sample(const float* depth_pred, const float* loc, int32_t N,
                            float* sampled, void* stream);
 int so_depth_metric_sums(const float* sampled, const float* depth_gt, const uint8_t* mask, const float* scale, int32_t N,
                          int32_t n, float* sums, void* stream);
+/* 8f-3  novel-view depth evaluation (eval_novel_depth.py:159-208, eval_novel_depth_kitti.py): the depth maps of K poses x
+ * N cameras, depth_maps [n_seg = K*N, h, w], against a ragged LiDAR set in CSR form with one segment per (pose, camera):
+ * segment s is points [offsets[s], offsets[s+1]) of loc [T,2] in [0,1] (x,y), depth_gt [T], mask [T] (uint8).  Each point
+ * with mask != 0 samples map s with the arithmetic of so_depth_metric_sample; errors [n_seg, 7] = the segment's
+ * compute_depth_errors_torch (utils/metric_util.py:424-445) metrics (abs_rel, sq_rel, rmse, rmse_log, a1, a2, a3) at
+ * pred' = clamp(sampled, 1e-3, 80): means over the masked points, rmse / rmse_log the square roots of means.  A segment
+ * without a masked point gives NaN in all seven.  One CTA per segment, fp64 sums in a fixed order: bit-identical run to
+ * run.  offsets lives on the device; offsets_host is the same array in host memory, checked before the launch: refused
+ * (SO_ERR_INVALID_ARG) are null pointers, n_seg < 1, h or w < 1, offsets_host[0] != 0, offsets_host[n_seg] != T and
+ * decreasing offsets; h * w >= 2^31 is SO_ERR_UNSUPPORTED. */
+int so_novel_depth_errors(const float* depth_maps, int32_t n_seg, int32_t h, int32_t w, const int64_t* offsets,
+                          const int64_t* offsets_host, int64_t T, const float* loc, const float* depth_gt, const uint8_t* mask,
+                          float* errors, void* stream);
 
 /* B12  field query at arbitrary points.  Replaces field.forward_sdfnetwork / forward_geonetwork
  * as used by NeuSHead.get_uniform_sdf (neus_head.py:265-293).  points [n,3] metres ->

@@ -4,6 +4,7 @@
 (``so_depth_metric_sample`` + ``so_depth_metric_sums``) and a sort-based masked median, so a frame's metric step
 enqueues without synchronising."""
 import ctypes as C
+import math
 import numpy as np
 import torch
 import torch.nn as nn
@@ -102,6 +103,165 @@ class DepthMetric(nn.Module):
                     logger.info('%12s | ' % name + ' '.join('%s %.3f' % (k, res[k][ti, cam]) for k in KEYS + ('scaling',)))
                 logger.info('%12s | ' % 'All' + ' '.join('%s %.3f' % (k, res[k][ti].mean()) for k in KEYS + ('scaling',)))
         return res
+
+
+# ------------------------------------------------------------------------------------------------------------------------
+# Novel-view depth on the device (eval_novel_depth.py:159-208, eval_novel_depth_kitti.py).  The reference renders, samples
+# and reduces each of a frame's S source poses separately, with a boolean-mask gather (a host sync) per camera; here the S
+# poses are one render_poses launch, the frame's LiDAR points one host-to-device copy and the per-(pose, camera) errors one
+# so_novel_depth_errors launch, accumulated into fixed-size per-distance bins on the device.
+
+def novel_depth_errors(depth_maps, offsets, loc, depth_gt, mask_u8, offsets_host=None):
+    """depth_maps [S, h, w] (one map per (pose, camera) segment), offsets int64 [S + 1], loc [T, 2] in [0, 1] (x, y),
+    depth_gt [T], mask_u8 uint8 [T] -> [S, 7] compute_depth_errors_torch metrics (KEYS order) per segment, NaN where a
+    segment has no masked-in point.  ``offsets_host``: the same offsets as a CPU tensor, checked before the launch; when
+    omitted they are read back from the device, which synchronises."""
+    lib = _lib.load()
+    _chk(depth_maps, name='depth_maps'); _chk(offsets, torch.int64, 'offsets'); _chk(loc, name='depth_loc')
+    _chk(depth_gt, name='depth_gt'); _chk(mask_u8, torch.uint8, 'depth_mask')
+    S, h, w = depth_maps.shape
+    T = depth_gt.shape[0]
+    if offsets.shape != (S + 1,) or loc.shape != (T, 2) or depth_gt.shape != (T,) or mask_u8.shape != (T,):
+        raise ValueError('novel_depth_errors: expected offsets [%d], loc [T, 2], depth_gt [T], mask [T]; got %s, %s, %s, %s'
+                         % (S + 1, tuple(offsets.shape), tuple(loc.shape), tuple(depth_gt.shape), tuple(mask_u8.shape)))
+    if offsets_host is None:
+        offsets_host = offsets.cpu()
+    elif offsets_host.is_cuda or offsets_host.dtype != torch.int64 or offsets_host.shape != (S + 1,) or not offsets_host.is_contiguous():
+        raise ValueError('offsets_host must be a contiguous int64 CPU tensor of shape [%d]' % (S + 1))
+    out = torch.empty(S, 7, device=depth_maps.device)
+    _lib.check(lib.so_novel_depth_errors(_p(depth_maps), S, h, w, _p(offsets), _p(offsets_host), T, _p(loc), _p(depth_gt),
+                                         _p(mask_u8), _p(out), _stream()), 'so_novel_depth_errors')
+    return out
+
+
+def _align(n, a=16):
+    return (n + a - 1) // a * a
+
+
+def pack_novel_depth(meta, num_cams, max_distance, pin=True):
+    """One frame's loader metas (``depth_loc`` [N, n_s, 2], ``depth_gt`` [N, n_s], ``depth_mask`` [N, n_s] per source s,
+    numpy, and ``frame_dists`` [S]) -> (buf, layout): every array in one uint8 CPU tensor (pinned unless ``pin`` is False),
+    so that a frame is one host-to-device copy.  Sections, each 16-byte aligned, as layout[name] = (byte offset, bytes):
+    offsets int64 [S*N + 1] (segment s*N + c = source s, camera c: render_poses' [S, N] order), perm / bins int64 [S] (the
+    sources ordered in rounds, each round holding every distance bin at most once, and their bins), loc float32 [T, 2],
+    gt float32 [T], mask uint8 [T].  layout['rounds'] holds the [begin, end) of each round in perm / bins."""
+    locs, gts, masks, dists = meta['depth_loc'], meta['depth_gt'], meta['depth_mask'], meta['frame_dists']
+    S, N = len(dists), num_cams
+    if not (len(locs) == len(gts) == len(masks) == S) or S == 0:
+        raise ValueError('depth_loc / depth_gt / depth_mask / frame_dists must hold one entry per source pose (got %d, %d, %d, %d)'
+                         % (len(locs), len(gts), len(masks), S))
+    bins = []
+    for d in dists:
+        k = math.ceil(float(d))
+        if not 0 <= k <= max_distance:
+            raise ValueError('source distance %r falls in bin %d, outside the metric\'s bins [0, %d]: construct '
+                             'NovelDepthMetric with a larger max_distance' % (d, k, max_distance))
+        bins.append(k)
+    counts = []
+    for s in range(S):
+        n = np.shape(gts[s])[-1] if np.ndim(gts[s]) == 2 else -1
+        if np.shape(gts[s]) != (N, n) or np.shape(locs[s]) != (N, n, 2) or np.shape(masks[s]) != (N, n):
+            raise ValueError('source %d: expected depth_loc [%d, n, 2], depth_gt / depth_mask [%d, n]; got %s, %s, %s'
+                             % (s, N, N, np.shape(locs[s]), np.shape(gts[s]), np.shape(masks[s])))
+        counts.append(n)
+    seg = np.repeat(np.asarray(counts, dtype=np.int64), N)
+    T = int(seg.sum())
+    seen, rank = {}, []
+    for k in bins:
+        rank.append(seen.get(k, 0))
+        seen[k] = rank[-1] + 1
+    perm = sorted(range(S), key=lambda s: (rank[s], s))
+    rounds, b = [], 0
+    for r in range(max(rank) + 1):
+        e = b + rank.count(r)
+        rounds.append((b, e))
+        b = e
+    layout, off = {'S': S, 'N': N, 'T': T, 'rounds': rounds}, 0
+    for name, nbytes in (('offsets', 8 * (S * N + 1)), ('perm', 8 * S), ('bins', 8 * S), ('loc', 8 * T), ('gt', 4 * T),
+                         ('mask', T)):
+        layout[name] = (off, nbytes)
+        off += _align(nbytes)
+    buf = torch.empty(max(off, 16), dtype=torch.uint8, pin_memory=pin)
+    raw = buf.numpy()
+    view = lambda name, dt: raw[layout[name][0]:layout[name][0] + layout[name][1]].view(dt)
+    offsets = view('offsets', np.int64)
+    offsets[0] = 0
+    np.cumsum(seg, out=offsets[1:])
+    view('perm', np.int64)[:] = perm
+    view('bins', np.int64)[:] = [bins[s] for s in perm]
+    loc, gt, mask = view('loc', np.float32).reshape(T, 2), view('gt', np.float32), view('mask', np.uint8)
+    b = 0
+    for s in range(S):
+        e = b + N * counts[s]
+        loc[b:e] = np.asarray(locs[s]).reshape(-1, 2)
+        gt[b:e] = np.asarray(gts[s]).reshape(-1)
+        mask[b:e] = np.asarray(masks[s]).reshape(-1)
+        b = e
+    return buf, layout
+
+
+class NovelDepthMetric(nn.Module):
+    """Per-distance novel-view depth errors of eval_novel_depth.py / eval_novel_depth_kitti.py on the device.
+
+    ``errors`` [B, N, 7] (fp64) and ``n_frames`` [B] (int64) hold one bin per integer distance k = ceil(source distance) in
+    [0, max_distance]; a source farther away is refused, not clipped.  ``_after_step(metas, depth_maps)`` takes one frame:
+    the loader's metas (``depth_loc`` / ``depth_gt`` / ``depth_mask`` / ``frame_dists``) and the depth maps of its S source
+    poses, render_poses' ``ms_depths[0]`` or ``ms_max_depths[0]`` reshaped to [S, N, h, w] (or [S*N, h, w]) with h, w the
+    eval ray grid, as the reference reshapes to ``cfg.num_rays``.  Each (source, camera) adds its seven errors to the
+    source's bin and each source one frame to the bin's count, as ``agg_depth_errors[k] += cams_depth_errors;
+    n_frames[k] += 1`` does; a step enqueues one host-to-device copy and a few launches and reads nothing back.
+    ``_after_epoch()`` all-reduces the two buffers when torch.distributed is initialised and returns ``as_dicts()``."""
+
+    def __init__(self, num_cams, max_distance, device='cuda'):
+        super().__init__()
+        if num_cams < 1 or max_distance < 0:
+            raise ValueError('num_cams must be >= 1 and max_distance >= 0')
+        self.num_cams, self.max_distance = int(num_cams), int(max_distance)
+        self.register_buffer('errors', torch.zeros(self.max_distance + 1, self.num_cams, 7, dtype=torch.float64, device=device))
+        self.register_buffer('n_frames', torch.zeros(self.max_distance + 1, dtype=torch.int64, device=device))
+
+    def _reset(self):
+        self.errors.zero_()
+        self.n_frames.zero_()
+
+    @torch.no_grad()
+    def _after_step(self, metas, depth_maps):
+        meta = metas[0] if isinstance(metas, (list, tuple)) else metas
+        buf, lay = pack_novel_depth(meta, self.num_cams, self.max_distance)
+        S, N, T = lay['S'], lay['N'], lay['T']
+        h, w = depth_maps.shape[-2:]
+        if depth_maps.numel() != S * N * h * w:
+            raise ValueError('depth_maps %s: expected the maps of %d source poses x %d cameras, [S, N, h, w] or [S*N, h, w]'
+                             % (tuple(depth_maps.shape), S, N))
+        dev = self.errors.device
+        d = buf.to(dev, non_blocking=True)
+        part = lambda name, dt: d[lay[name][0]:lay[name][0] + lay[name][1]].view(dt)
+        o0, ob = lay['offsets']
+        err = novel_depth_errors(depth_maps.reshape(S * N, h, w).float().contiguous(), part('offsets', torch.int64),
+                                 part('loc', torch.float32).view(T, 2), part('gt', torch.float32), part('mask', torch.uint8),
+                                 offsets_host=buf[o0:o0 + ob].view(torch.int64))
+        err = err.view(S, N, 7).double()
+        perm, bins = part('perm', torch.int64), part('bins', torch.int64)
+        for b, e in lay['rounds']:                 # every bin once per round: a fixed order of additions
+            self.errors.index_add_(0, bins[b:e], err.index_select(0, perm[b:e]))
+        self.n_frames.index_add_(0, bins, torch.ones(S, dtype=torch.int64, device=dev))
+
+    def _after_epoch(self):
+        d = _dist()
+        if d is not None:
+            d.all_reduce(self.errors)
+            d.all_reduce(self.n_frames)
+        return self.as_dicts()
+
+    def as_dicts(self):
+        """(agg_depth_errors, n_frames) keyed by distance, bins without a frame left out, as the scripts' print_metrics
+        takes them: eval_novel_depth.py's ({k: [N, 7] tensor}, {k: [1] int tensor}); for N = 1 eval_novel_depth_kitti.py's
+        ({k: [7] ndarray}, {k: int})."""
+        nf = self.n_frames.cpu()
+        keep = [k for k in range(self.max_distance + 1) if nf[k] > 0]
+        if self.num_cams == 1:
+            return {k: self.errors[k, 0].cpu().numpy() for k in keep}, {k: int(nf[k]) for k in keep}
+        return {k: self.errors[k] for k in keep}, {k: self.n_frames[k:k + 1] for k in keep}
 
 
 # ------------------------------------------------------------------------------------------------------------------------
