@@ -123,6 +123,13 @@ int so_tpv_decode_bwd_input(float* g0, const float* a0, int64_t n, void* stream)
  * launch; bev, w1 and w2 16-byte aligned. */
 int so_bev_decode(const float* bev, int32_t C, const float* w1, const float* b1, const float* w2, const float* b2,
                   const so_volume_desc* vol_host, float* vol_sdf, float* vol_feat, void* stream);
+/* Same, for the row range [h_begin, h_begin + h_count) of the volume only (the decode-sharded training step: every rank
+ * decodes its slab of h rows, BEV rows h_begin * W .. (h_begin + h_count) * W - 1, into the full-size buffers).  Other rows
+ * untouched, including their sdf pads.  A negative or overflowing range is SO_ERR_INVALID_ARG; h_count == 0 does nothing.
+ * so_bev_decode is the range [0, H). */
+int so_bev_decode_rows(const float* bev, int32_t C, const float* w1, const float* b1, const float* w2, const float* b2,
+                       const so_volume_desc* vol_host, int32_t h_begin, int32_t h_count, float* vol_sdf, float* vol_feat,
+                       void* stream);
 /* Element-wise pieces of its backward (training), around the products on so_linear_3xtf32 / cuBLAS:
  *   gather:   g_out[row_count][Z * Cf] of rows [row_begin, row_begin + row_count) from g_vol_sdf / g_vol_feat (NULL = zero;
  *             sdf pads and feature pad channels never read)

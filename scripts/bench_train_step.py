@@ -24,7 +24,11 @@ between ranks and from the 1-GPU run; with --loss shipped the total is the Multi
     --emulate-world W (one process): ONE rank's share of a W-rank step with both shardings on one GPU -- rank 0's rows
     through every layer, a local stand-in for the exchange (it fills the other ranks' rows with this rank's buffer and returns
     this rank's own gradient rows, talking to no one), the head on rank 0's ray slice.  Compute per rank, communication
-    excluded; the loss value is not the W-rank step's."""
+    excluded; the loss value is not the W-rank step's.
+    --shard-decode (under torchrun, or with --emulate-world): the head's decode is sharded too (head.decode_shard, its
+    exchange on its own NCCL process group; emulated by the same local stand-ins): each rank decodes and backpropagates
+    its slab of the volume's h rows, one all_gather of the volume forward and one reduce-scatter of its gradient backward.
+    The JSON line then carries the bytes that exchange moves per rank and step (decode_exchange_bytes_per_rank)."""
 import json, os, sys, time
 import numpy as np
 import torch
@@ -45,6 +49,7 @@ rng = [-40.0, -40.0, -1.0, 40.0, 40.0, 5.4]
 loss_mode = sys.argv[sys.argv.index('--loss') + 1] if '--loss' in sys.argv else None
 emulate = int(sys.argv[sys.argv.index('--emulate-world') + 1]) if '--emulate-world' in sys.argv else 0
 shard_encoder = '--shard-encoder' in sys.argv
+shard_decode = '--shard-decode' in sys.argv
 if emulate and world > 1:
     raise SystemExit('--emulate-world runs in one process (it emulates one rank of the W-rank step)')
 shipped = loss_mode == 'shipped'
@@ -89,6 +94,9 @@ if world > 1:
     if shard_encoder:
         model.encoder.query_shard = (rank, world)
         model.encoder.query_shard_group = dist.new_group(backend='nccl')
+    if shard_decode:
+        model.head.decode_shard = (rank, world)
+        model.head.decode_shard_group = dist.new_group(backend='nccl')
     net = torch.nn.parallel.DistributedDataParallel(model, device_ids=[local], broadcast_buffers=False)
 
 
@@ -104,6 +112,9 @@ def local_reduce_scatter(out, buf):
 
 if emulate:
     model.head.ray_shard = (0, emulate)
+    if shard_decode:
+        model.head.decode_shard = (0, emulate)
+        model.head.decode_shard_collectives = (local_gather, local_reduce_scatter)
     for ml_ in (objective, reproj):
         if ml_ is not None:
             ml_.collective = local_gather
@@ -176,14 +187,19 @@ if world > 1 and terms:            # the last step's loss terms on every rank: r
     print(json.dumps({'rank': rank, 'terms': {k: float(v) for k, v in terms.items()}}), flush=True)
     dist.barrier()
 if emulate:
-    mode = ', ONE rank of %d emulated (query- and ray-sharded): compute per rank, communication excluded' % emulate
+    mode = ', ONE rank of %d emulated (query-%s and ray-sharded): compute per rank, communication excluded' % (
+        emulate, ', decode-' if shard_decode else '')
 elif world > 1:
-    mode = ' ray-sharded%s + DDP' % (' + query-sharded encoder' if shard_encoder else '')
+    mode = ' ray-sharded%s%s + DDP' % (' + query-sharded encoder' if shard_encoder else '', ' + decode-sharded' if shard_decode else '')
 else:
     mode = ''
+exchange = {}
+if shard_decode and (emulate or world > 1):
+    from selfocc_b200.dist import volume_exchange_bytes
+    exchange = {'decode_exchange_bytes_per_rank': volume_exchange_bytes(model.head.model.field.desc, emulate or world)}
 if rank == 0:
   print(json.dumps({'workload': 'nuscenes_occ-like training step, %d GPU(s)%s, fp32, 6x48x100 rays x 256, TPV 257x257x25, colour%s' % (world, mode, ', reprojection loss' if reproj is not None else ', nuscenes_occ MultiLoss (24 colour dims, semantics, second grad)' if shipped else ''), 'ms_per_step': ms,
                   'rays_per_s': 28800 / (ms * 1e-3), 'library_launches_per_step': (_lib.launch_count() - l0) / K, 'peak_mem_gb': peak_gb,
-                  'loss': float(last), 'finite': bool(torch.isfinite(last))}))
+                  'loss': float(last), 'finite': bool(torch.isfinite(last)), **exchange}))
 if world > 1:
     dist.destroy_process_group()

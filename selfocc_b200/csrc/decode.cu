@@ -773,15 +773,31 @@ extern "C" int so_tpv_decode_bwd_input(float* g0, const float* a0, int64_t n, vo
 
 extern "C" int so_bev_decode(const float* bev, int32_t C, const float* w1, const float* b1, const float* w2, const float* b2,
                              const so_volume_desc* d, float* vol_sdf, float* vol_feat, void* stream) {
+  if (!d) return SO_ERR_INVALID_ARG;
+  return so_bev_decode_rows(bev, C, w1, b1, w2, b2, d, 0, d->H, vol_sdf, vol_feat, stream);
+}
+
+// Rows [h_begin, h_begin + h_count) of the volume only (the decode-sharded training step: every rank decodes its slab of h
+// rows into the full-size volume buffers).  A BEV row r = h * W + w is one pillar, so the slab is the contiguous run of
+// h_count * W rows starting at h_begin * W, in the BEV plane and in both volume buffers alike: the kernel runs on that run
+// as on a smaller volume.  Rows outside the range are untouched.
+extern "C" int so_bev_decode_rows(const float* bev, int32_t C, const float* w1, const float* b1, const float* w2, const float* b2,
+                                  const so_volume_desc* d, int32_t h_begin, int32_t h_count, float* vol_sdf, float* vol_feat,
+                                  void* stream) {
   if (!bev || !w1 || !b1 || !w2 || !b2 || !vol_sdf) return SO_ERR_INVALID_ARG;
   int rc = validate_volume(d);
   if (rc) return rc;
+  if (h_begin < 0 || h_count < 0 || h_begin > d->H - h_count) return SO_ERR_INVALID_ARG;
+  if (h_count == 0) return SO_OK;
   if (d->n_feat > 0 && !vol_feat) return SO_ERR_INVALID_ARG;
   if (C != 96) return SO_ERR_UNSUPPORTED;
   if ((int64_t)d->Z * (1 + d->n_feat) > kBevMaxCols) return SO_ERR_UNSUPPORTED;
   if (misaligned16(bev) || misaligned16(w1) || misaligned16(w2)) return SO_ERR_INVALID_ARG;
   cudaStream_t st = (cudaStream_t)stream;
-  const long long cols = (long long)d->H * d->W;
+  const long long row0 = (long long)h_begin * d->W, cols = (long long)h_count * d->W;
+  bev += row0 * C;
+  vol_sdf += row0 * d->zpitch;
+  if (vol_feat) vol_feat += row0 * d->Z * d->feat_pitch;
   if (d->zpitch > d->Z) {
     long long n = cols * (d->zpitch - d->Z);
     zero_pad_kernel<<<(unsigned)ceil_div64(n, 256), 256, 0, st>>>(vol_sdf, cols, d->Z, d->zpitch);

@@ -247,6 +247,56 @@ def all_gather_rows(local, sizes, rank, world, collective=None, reduce_scatter=N
     return _RowGather.apply((sizes, rank, world, collective, reduce_scatter), local.contiguous())
 
 
+# ---------------------------------------------------------------------------------------- h-row slabs of the decoded volume
+# The decode-sharded training step (head.decode_shard): the volume is H-major (vol_sdf [H, W, zpitch], vol_feat
+# [H, W, Z, feat_pitch]), so rank r's slab is rows ray_slice(H, world, r) of both tensors, and the exchange is
+# all_gather_rows over ONE plane of H rows whose row is an h row of vol_sdf followed by the same h row of vol_feat.
+def volume_slab(H, rank, world):
+    """(h_begin, h_count) of this rank's slab of the volume's H rows."""
+    if H < world:
+        raise ValueError('decode_shard: a volume of %d h rows cannot be split over %d ranks (a rank without rows would leave '
+                         'the decode without a gradient there)' % (H, world))
+    return ray_slice(H, world, rank)
+
+
+def pack_volume_rows(vol_sdf, vol_feat):
+    """A slab of the volume ([c, W, zpitch], [c, W, Z, feat_pitch] or None) -> the [c, row] rows all_gather_volume sends:
+    each row is the slab row of vol_sdf followed by that of vol_feat."""
+    c = vol_sdf.shape[0]
+    if vol_feat is None:
+        return vol_sdf.reshape(c, -1)
+    return torch.cat([vol_sdf.reshape(c, -1), vol_feat.reshape(c, -1)], 1)
+
+
+def volume_exchange_bytes(desc, world):
+    """Bytes one decode-sharded step moves per rank through the exchange: the all_gather receives world - 1 padded slabs
+    and the reduce-scatter sends as many (ring algorithms; fp32)."""
+    row = desc.W * desc.zpitch + (desc.W * desc.Z * desc.feat_pitch if desc.n_feat else 0)
+    per = -(-desc.H // world)
+    return dict(all_gather=4 * (world - 1) * per * row, reduce_scatter=4 * (world - 1) * per * row)
+
+
+def all_gather_volume(vol_sdf, vol_feat, H, rank, world, collective=None, reduce_scatter=None, group=None):
+    """This rank's slab of the decoded volume (rows volume_slab(H, rank, world) of vol_sdf and vol_feat; vol_feat None when
+    no features are decoded) -> the full (vol_sdf, vol_feat) on every rank, contiguous and autograd-connected.
+
+    Forward: ONE all_gather of both tensors' slab rows side by side (pack_volume_rows).  Backward: ONE reduce-scatter (SUM)
+    of the full volume gradient, whose block for this rank is the gradient of its slab.  ``collective`` /
+    ``reduce_scatter`` / ``group``: as all_gather_rows, over a single plane of H rows.  Gradient rule: as all_gather_rows --
+    the sum over the ranks of their volume gradients is world x the full gradient, so this rank's slab receives world x
+    its share."""
+    b, c = volume_slab(H, rank, world)
+    if vol_sdf.shape[0] != c or (vol_feat is not None and vol_feat.shape[0] != c):
+        raise ValueError('all_gather_volume: rank %d of %d holds h rows [%d, %d), got a slab of %s'
+                         % (rank, world, b, b + c, tuple(vol_sdf.shape)))
+    full = all_gather_rows(pack_volume_rows(vol_sdf, vol_feat), [H], rank, world, collective, reduce_scatter, group)
+    n_sdf = math.prod(vol_sdf.shape[1:])
+    vs = full[:, :n_sdf].reshape(H, *vol_sdf.shape[1:]).contiguous()
+    if vol_feat is None:
+        return vs, None
+    return vs, full[:, n_sdf:].reshape(H, *vol_feat.shape[1:]).contiguous()
+
+
 def _num_cams(head, metas):
     """Number of cameras the head will render, read from the metas' SHAPES (no copy: usable inside CUDA-graph capture)."""
     import os

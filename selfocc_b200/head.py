@@ -153,22 +153,24 @@ class _SDFField(nn.Module):
         self.vol_sdf = self.vol_feat = None
         self._pack = None
 
-    def decode(self, representation, train=False):
+    def decode(self, representation, train=False, rows=None):
         """The representation -> (vol_sdf, vol_feat): the fused decode for prepare / forward_occ, its autograd form for the
-        training forward (``train``; vol_feat is then an empty tensor when no features are decoded)."""
+        training forward (``train``; vol_feat is then an empty tensor when no features are decoded).  ``rows`` =
+        (h_begin, h_count), training form only: that slab of h rows of the volume (the decode-sharded training step)."""
+        assert rows is None or train, 'a slab of rows is decoded by the training form only'
         l1, l2 = self.density_net[1], self.density_net[3]
         w = (l1.weight, l1.bias, l2.weight, l2.bias)
         if self.tpv:
             hw, zh, wz = representation
             assert hw.shape[0] == 1, 'only support bs = 1 currently'
             if train:
-                return ops.TPVDecodeFunction.apply(hw[0], zh[0], wz[0], *w, self.desc)
+                return ops.TPVDecodeFunction.apply(hw[0], zh[0], wz[0], *w, self.desc, rows)
             return ops.tpv_decode(hw[0].contiguous(), zh[0].contiguous(), wz[0].contiguous(), *w, self.desc)
         bev = representation
         assert torch.is_tensor(bev) and bev.dim() == 3, 'tpv=False: the representation is one BEV plane [bs, H*W, C]'
         assert bev.shape[0] == 1, 'only support bs = 1 currently'
         if train:
-            return ops.BEVDecodeFunction.apply(bev[0], *w, self.desc)
+            return ops.BEVDecodeFunction.apply(bev[0], *w, self.desc, rows)
         return ops.bev_decode(bev[0].contiguous(), *w, self.desc)
 
     def pre_compute_density_color(self, representation):
@@ -255,6 +257,11 @@ class NeuSHead(nn.Module):
         self.two_split = two_split
         self.cos_anneal_ratio = 1.0
         self.fused_objective = None       # loss.fuse_objective: the training render computes the objective's per-sample terms
+        # decode-sharded training (head_train.decode_train): (rank, world) of this process, the process group of the volume
+        # exchange (None: the default group), and optional (collective, reduce_scatter) hooks of dist.all_gather_volume
+        self.decode_shard = None
+        self.decode_shard_group = None
+        self.decode_shard_collectives = None
 
     # ------------------------------------------------------------------ checkpoints
     # The field's parameters follow the in-repo analogue's names (bev_nerf.py:62-71: ``density_net.{1,3}``) under

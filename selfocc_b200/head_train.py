@@ -28,9 +28,12 @@ def forward_train(head, representation, metas=None, jitter=None, bkgd_rand=None,
     ``reproj_stats`` [num_cams, R, 6 * sets], ``reproj_colours`` [num_cams, R, 9] and ``eikonal_mean`` (0-d) in place of
     ``weights``, ``ts``, ``deltas`` and ``eik_grad``.  The reprojection term's images arrive as the model kwargs
     ``curr_imgs`` / ``prev_imgs`` / ``next_imgs`` ([1, num_cams, 3, H, W]) and its matrices as metas' img2prevImg /
-    img2nextImg."""
+    img2nextImg.
+
+    Decode-sharded training (``head.decode_shard = (rank, world)``, world > 1; training mode with grad enabled): see
+    decode_train.  The gathered volume feeds the render, ``uniform_sdf``, ``second_grad`` and the fused objective alike."""
     f = head.model.field
-    vol_sdf, vol_feat = f.decode(representation, train=True)
+    vol_sdf, vol_feat = decode_train(head, representation)
     vol_feat = vol_feat if f.desc.n_feat else None
     f.vol_sdf, f.vol_feat = vol_sdf.detach(), (vol_feat.detach() if vol_feat is not None else None)
     f.vol_sdf_live, f.vol_feat_live = vol_sdf, vol_feat           # autograd-connected views for get_uniform_sdf
@@ -155,6 +158,35 @@ def forward_train(head, representation, metas=None, jitter=None, bkgd_rand=None,
     if sharded:
         outputs['ray_shard'] = (shard[0], shard[1], r_full)
     return outputs
+
+
+def decode_train(head, representation):
+    """The training form of the decode -> (vol_sdf, vol_feat; an empty tensor when no features are decoded).
+
+    With ``head.decode_shard = (rank, world)``, world > 1, in training mode with grad enabled, this rank decodes only its
+    slab of the volume's h rows (dist.volume_slab: H < world is refused) and dist.all_gather_volume assembles the full volume
+    on every rank over ``head.decode_shard_group`` (``head.decode_shard_collectives``: optional (collective,
+    reduce_scatter) hooks in its place): one all_gather forward, one reduce-scatter of the volume gradient backward.  The
+    decode's backward then runs over the slab's rows only.  Both fields (tpv True / False) shard the same way.
+
+    Gradient rule (DESIGN.md section 6): a rank's gradient w.r.t. the full volume is partial and scaled by world under
+    ``head.ray_shard``, full and unscaled for the replicated terms (uniform_sdf, second_grad, any term of a step without ray
+    sharding); either way the sum over the ranks is world x the full gradient.  The reduce-scatter hands rank r world x the
+    full gradient on its slab, so its plane and MLP-weight gradients are world x the slab's share, and their sum over the
+    ranks is world x the full gradient: DistributedDataParallel's mean is exact.  Eval and no_grad ignore the switch
+    (inference shards its decode with dist.decode_sharded)."""
+    f = head.model.field
+    shard = getattr(head, 'decode_shard', None)
+    if shard is None or shard[1] <= 1 or not (head.training and torch.is_grad_enabled()):
+        return f.decode(representation, train=True)
+    from .dist import all_gather_volume, volume_slab
+    rank, world = shard
+    rows = volume_slab(f.desc.H, rank, world)
+    vs, vf = f.decode(representation, train=True, rows=rows)
+    hooks = getattr(head, 'decode_shard_collectives', None) or (None, None)
+    vs, vf = all_gather_volume(vs, vf if f.desc.n_feat else None, f.desc.H, rank, world, *hooks,
+                               group=getattr(head, 'decode_shard_group', None))
+    return vs, (vf if vf is not None else vs.new_empty(0))
 
 
 def _objective(fused, kwargs, metas, rays, num_cams, dev):

@@ -57,9 +57,11 @@ def tpv_decode(tpv_hw, tpv_zh, tpv_wz, w1, b1, w2, b2, desc, rows=None, out=None
     return vol_sdf, vol_feat
 
 
-def bev_decode(bev, w1, b1, w2, b2, desc):
+def bev_decode(bev, w1, b1, w2, b2, desc, rows=None, out=None):
     """tpv=False decode: bev [H*W, C] + MLP (w2 [Z * (1 + n_feat), C]) -> (vol_sdf [H,W,zpitch], vol_feat [H,W,Z,feat_pitch] | None),
-    the layout tpv_decode writes."""
+    the layout tpv_decode writes.  rows=(h_begin, h_count): decode that slab of h rows only (BEV rows h_begin * W ..
+    (h_begin + h_count) * W - 1); out=(vol_sdf, vol_feat): write into existing full-size buffers (rows outside the slab are
+    left untouched), as tpv_decode."""
     lib = _lib.load()
     for n, t in (('bev', bev), ('w1', w1), ('b1', b1), ('w2', w2), ('b2', b2)):
         _chk(t, name=n)
@@ -67,13 +69,18 @@ def bev_decode(bev, w1, b1, w2, b2, desc):
     assert bev.numel() == desc.H * desc.W * Cc, 'bev shape does not match the mapping'
     assert w1.shape == (Cc, Cc) and w2.shape == (desc.Z * (1 + desc.n_feat), Cc)
     dev = bev.device
-    vol_sdf = torch.empty(desc.H, desc.W, desc.zpitch, device=dev, dtype=torch.float32)
-    vol_feat = None
-    if desc.n_feat:
-        vol_feat = (torch.zeros if desc.feat_pitch > desc.n_feat else torch.empty)(
-            desc.H, desc.W, desc.Z, desc.feat_pitch, device=dev, dtype=torch.float32)
-    _lib.check(lib.so_bev_decode(_p(bev), Cc, _p(w1), _p(b1), _p(w2), _p(b2), C.byref(desc), _p(vol_sdf), _p(vol_feat), _stream()),
-               'so_bev_decode')
+    if out is not None:
+        vol_sdf, vol_feat = out
+        _chk(vol_sdf, name='vol_sdf'); _chk(vol_feat, name='vol_feat')
+        assert vol_sdf.shape == (desc.H, desc.W, desc.zpitch)
+    else:
+        vol_sdf = torch.empty(desc.H, desc.W, desc.zpitch, device=dev, dtype=torch.float32)
+        vol_feat = torch.empty(desc.H, desc.W, desc.Z, desc.feat_pitch, device=dev, dtype=torch.float32) if desc.n_feat else None
+    h0, hc = (0, desc.H) if rows is None else rows
+    if vol_feat is not None and desc.feat_pitch > desc.n_feat:
+        vol_feat[h0:h0 + hc].zero_()
+    _lib.check(lib.so_bev_decode_rows(_p(bev), Cc, _p(w1), _p(b1), _p(w2), _p(b2), C.byref(desc), int(h0), int(hc), _p(vol_sdf),
+                                      _p(vol_feat), _stream()), 'so_bev_decode_rows')
     return vol_sdf, vol_feat
 
 
@@ -586,20 +593,40 @@ class FieldSecondGradFunction(torch.autograd.Function):
         return gvs, None, None
 
 
+def _slab(vol, rows):
+    """Rows [h_begin, h_begin + h_count) of a full-size volume tensor (None stays None)."""
+    return None if vol is None else vol[rows[0]:rows[0] + rows[1]]
+
+
+def _slab_desc(d, h_count):
+    """The volume descriptor of an h_count-row slab: the decode backward reads a slab's volume gradient through it."""
+    s = _lib.VolumeDesc()
+    C.pointer(s)[0] = d
+    s.H = h_count
+    return s
+
+
 class TPVDecodeFunction(torch.autograd.Function):
     """Decode with the fused sm_90a forward.  Backward (training only) recomputes the MLP slab by slab -- bounded memory,
     never the reference's 750 MB intermediate.  The native slab backward (_backward_native: wgmma 3xTF32 GEMMs + the fused
     element-wise kernels so_tpv_decode_bwd_*) wherever the 3xTF32 GEMM takes the channel count and the second layer has
-    at most 32 outputs; otherwise the torch/cuBLAS autograd restatement of the same slab (_backward_torch)."""
+    at most 32 outputs; otherwise the torch/cuBLAS autograd restatement of the same slab (_backward_torch).
+
+    rows=(h_begin, h_count) (the decode-sharded training step): the forward decodes that slab of h rows only and returns
+    it, vol_sdf [h_count, W, zpitch] and vol_feat [h_count, W, Z, feat_pitch]; the backward takes the slab's gradient and
+    runs the slab loop over those rows only, so g_hw is filled on the slab's rows, g_zh on its columns, and g_wz and the
+    MLP's gradients are the sums over the slab's voxels."""
 
     SLAB_ROWS = 32
 
     @staticmethod
-    def forward(ctx, hw, zh, wz, w1, b1, w2, b2, desc):
-        ctx.desc = desc
+    def forward(ctx, hw, zh, wz, w1, b1, w2, b2, desc, rows=None):
+        ctx.desc, ctx.rows = desc, rows
         ctx.save_for_backward(hw, zh, wz, w1, b1, w2, b2)
         vs, vf = tpv_decode(hw.contiguous(), zh.contiguous(), wz.contiguous(), w1.contiguous(), b1.contiguous(),
-                            w2.contiguous(), b2.contiguous(), desc)
+                            w2.contiguous(), b2.contiguous(), desc, rows=rows)
+        if rows is not None:
+            vs, vf = _slab(vs, rows), _slab(vf, rows)
         return vs, (vf if vf is not None else vs.new_empty(0))
 
     @staticmethod
@@ -609,34 +636,37 @@ class TPVDecodeFunction(torch.autograd.Function):
         Cc = saved[0].shape[-1]
         native = linear_supported(Cc, Cc) and tuple(saved[3].shape) == (Cc, Cc) and 1 + d.n_feat <= 32
         fn = TPVDecodeFunction._backward_native if native else TPVDecodeFunction._backward_torch
-        return (*fn(saved, d, g_vs, g_vf), None)
+        return (*fn(saved, d, g_vs, g_vf, ctx.rows), None, None)
 
     @staticmethod
-    def _backward_native(saved, d, g_vs, g_vf):
+    def _backward_native(saved, d, g_vs, g_vf, rows=None):
         lib = _lib.load()
         hw, zh, wz, w1, b1, w2, b2 = [t.contiguous() for t in saved]
         H, W, Z, Cc, n_out = d.H, d.W, d.Z, hw.shape[-1], 1 + d.n_feat
+        hb, hc = (0, H) if rows is None else rows
+        gd = d if rows is None else _slab_desc(d, hc)           # the volume gradient is the slab's: rows from hb on
         dev = hw.device
         g_vs = g_vs.contiguous() if g_vs is not None else None
         g_vf = g_vf.contiguous() if (g_vf is not None and d.n_feat) else None
         w1_hi, w1_lo = split_tf32(w1)
         w1t_hi, w1t_lo = split_tf32(w1.t().contiguous())
-        g_hw, g_zh, g_wz = torch.empty_like(hw), torch.empty_like(zh), torch.zeros_like(wz)
+        part = torch.empty_like if rows is None else torch.zeros_like        # a slab fills only its own rows / columns
+        g_hw, g_zh, g_wz = part(hw), part(zh), torch.zeros_like(wz)
         g_w1, g_b1, g_w2, g_b2 = (torch.zeros_like(t) for t in (w1, b1, w2, b2))
-        step = min(H, TPVDecodeFunction.SLAB_ROWS)
+        step = max(1, min(hc, TPVDecodeFunction.SLAB_ROWS))
         rows_max = step * W * Z
         a0b, z1b, g1b = (torch.empty(rows_max, Cc, device=dev) for _ in range(3))
         gob = torch.empty(rows_max, n_out, device=dev)
         st = _stream()
-        for h0 in range(0, H, step):
-            nh = min(H, h0 + step) - h0
-            rows = nh * W * Z
-            a0, z1, g1, go = a0b[:rows], z1b[:rows], g1b[:rows], gob[:rows]
+        for h0 in range(hb, hb + hc, step):
+            nh = min(hb + hc, h0 + step) - h0
+            n_vox = nh * W * Z
+            a0, z1, g1, go = a0b[:n_vox], z1b[:n_vox], g1b[:n_vox], gob[:n_vox]
             _lib.check(lib.so_tpv_decode_bwd_features(_p(hw), _p(zh), _p(wz), Cc, C.byref(d), h0, nh, _p(a0), st),
                        'so_tpv_decode_bwd_features')
             linear_3xtf32(a0, w1_hi, w1_lo, b1, out=z1)
-            _lib.check(lib.so_tpv_decode_bwd_hidden(_p(z1), _p(g_vs), _p(g_vf), _p(w2), Cc, C.byref(d), h0, nh, _p(g1), _p(go), st),
-                       'so_tpv_decode_bwd_hidden')
+            _lib.check(lib.so_tpv_decode_bwd_hidden(_p(z1), _p(g_vs), _p(g_vf), _p(w2), Cc, C.byref(gd), h0 - hb, nh, _p(g1), _p(go),
+                                                    st), 'so_tpv_decode_bwd_hidden')
             # weight gradients: reductions over the slab's rows (cuBLAS; z1 now holds a1)
             g_w2.addmm_(go.t(), z1)
             g_b2.add_(go.sum(0))
@@ -651,18 +681,19 @@ class TPVDecodeFunction(torch.autograd.Function):
         return g_hw, g_zh, g_wz, g_w1, g_b1, g_w2, g_b2
 
     @staticmethod
-    def _backward_torch(saved, d, g_vs, g_vf):
+    def _backward_torch(saved, d, g_vs, g_vf, rows=None):
         import torch.nn.functional as F
         hw, zh, wz, w1, b1, w2, b2 = saved
         H, W, Z, Cc = d.H, d.W, d.Z, hw.shape[-1]
-        g_out = g_vs[..., :Z, None]
+        hb, hc = (0, H) if rows is None else rows
+        g_out = g_vs[..., :Z, None]                                # [hc, W, Z, 1 + n_feat]: row h of the volume is hb + h
         if d.n_feat:
             g_out = torch.cat([g_out, g_vf[..., :d.n_feat]], -1)
         grads = [torch.zeros_like(t) for t in (hw, zh, wz, w1, b1, w2, b2)]
         zh3, wz3 = zh.view(Z, H, Cc), wz.view(W, Z, Cc)
         step = 8
-        for h0 in range(0, H, step):
-            h1 = min(H, h0 + step)
+        for h0 in range(hb, hb + hc, step):
+            h1 = min(hb + hc, h0 + step)
             with torch.enable_grad():
                 a = hw.view(H, W, Cc)[h0:h1].detach().requires_grad_(True)
                 b = zh3[:, h0:h1].detach().requires_grad_(True)
@@ -670,7 +701,7 @@ class TPVDecodeFunction(torch.autograd.Function):
                 ws = [t.detach().requires_grad_(True) for t in (w1, b1, w2, b2)]
                 f = a[:, :, None, :] + b.permute(1, 0, 2)[:, None, :, :] + c[None]
                 out = F.linear(F.softplus(F.linear(F.softplus(f), ws[0], ws[1])), ws[2], ws[3])
-                gs = torch.autograd.grad(out, [a, b, c] + ws, g_out[h0:h1])
+                gs = torch.autograd.grad(out, [a, b, c] + ws, g_out[h0 - hb:h1 - hb])
             grads[0].view(H, W, Cc)[h0:h1] += gs[0]
             grads[1].view(Z, H, Cc)[:, h0:h1] += gs[1]
             grads[2].view(W, Z, Cc).add_(gs[2])
@@ -691,15 +722,21 @@ class BEVDecodeFunction(torch.autograd.Function):
     """bev_decode with autograd (training form of the tpv=False field): (bev [H*W, C], w1, b1, w2, b2, desc) ->
     (vol_sdf, vol_feat or an empty tensor).  Backward recomputes a0 / z1 / a1 in slabs of rows (nothing of the forward's
     MLP is kept) and gathers the slab's [rows, Z * Cf] output gradient from the volume gradients (so_bev_decode_bwd_gather);
-    the products run through _matmul_wt, the weight-gradient reductions over the rows on cuBLAS (as TPVDecodeFunction)."""
+    the products run through _matmul_wt, the weight-gradient reductions over the rows on cuBLAS (as TPVDecodeFunction).
+
+    rows=(h_begin, h_count) (the decode-sharded training step): the forward decodes and returns that slab of h rows only,
+    as TPVDecodeFunction; the backward runs over the slab's BEV rows h_begin * W .. (h_begin + h_count) * W - 1, so g_bev is
+    filled on those rows and the MLP's gradients are the sums over them."""
 
     SLAB_ROWS = 8192
 
     @staticmethod
-    def forward(ctx, bev, w1, b1, w2, b2, desc):
-        ctx.desc = desc
+    def forward(ctx, bev, w1, b1, w2, b2, desc, rows=None):
+        ctx.desc, ctx.rows = desc, rows
         ctx.save_for_backward(bev, w1, b1, w2, b2)
-        vs, vf = bev_decode(bev.contiguous(), w1.contiguous(), b1.contiguous(), w2.contiguous(), b2.contiguous(), desc)
+        vs, vf = bev_decode(bev.contiguous(), w1.contiguous(), b1.contiguous(), w2.contiguous(), b2.contiguous(), desc, rows=rows)
+        if rows is not None:
+            vs, vf = _slab(vs, rows), _slab(vf, rows)
         return vs, (vf if vf is not None else vs.new_empty(0))
 
     @staticmethod
@@ -708,20 +745,24 @@ class BEVDecodeFunction(torch.autograd.Function):
         lib = _lib.load()
         bev, w1, b1, w2, b2 = [t.detach().contiguous() for t in ctx.saved_tensors]
         d = ctx.desc
-        rows_total, Cc = bev.shape
+        Cc = bev.shape[1]
+        hb, hc = (0, d.H) if ctx.rows is None else ctx.rows
+        gd = d if ctx.rows is None else _slab_desc(d, hc)        # the volume gradient is the slab's: rows from hb * W on
+        r_begin, r_end = hb * d.W, (hb + hc) * d.W
         g_vs = _chk(g_vs.contiguous(), name='g_vol_sdf') if g_vs is not None else None
         g_vf = _chk(g_vf.contiguous(), name='g_vol_feat') if (g_vf is not None and d.n_feat) else None
         w1_hi, w1_lo = split_tf32(w1)
-        g_bev = torch.empty_like(bev)
+        g_bev = torch.empty_like(bev) if ctx.rows is None else torch.zeros_like(bev)
         g_w1, g_b1, g_w2, g_b2 = (torch.zeros_like(t) for t in (w1, b1, w2, b2))
         st = _stream()
-        for r0 in range(0, rows_total, BEVDecodeFunction.SLAB_ROWS):
-            n = min(rows_total, r0 + BEVDecodeFunction.SLAB_ROWS) - r0
+        for r0 in range(r_begin, r_end, BEVDecodeFunction.SLAB_ROWS):
+            n = min(r_end, r0 + BEVDecodeFunction.SLAB_ROWS) - r0
             a0 = torch.empty(n, Cc, device=bev.device)
             _lib.check(lib.so_bev_decode_bwd_features(_p(bev[r0:r0 + n]), a0.numel(), _p(a0), st), 'so_bev_decode_bwd_features')
             z1 = linear_3xtf32(a0, w1_hi, w1_lo, b1)
             go = torch.empty(n, w2.shape[0], device=bev.device)
-            _lib.check(lib.so_bev_decode_bwd_gather(_p(g_vs), _p(g_vf), C.byref(d), r0, n, _p(go), st), 'so_bev_decode_bwd_gather')
+            _lib.check(lib.so_bev_decode_bwd_gather(_p(g_vs), _p(g_vf), C.byref(gd), r0 - r_begin, n, _p(go), st),
+                       'so_bev_decode_bwd_gather')
             g1 = _matmul_wt(go, w2.t())
             _lib.check(lib.so_bev_decode_bwd_hidden(_p(z1), _p(g1), z1.numel(), st), 'so_bev_decode_bwd_hidden')
             g_w2.addmm_(go.t(), z1)                                   # z1 now holds a1
@@ -731,7 +772,7 @@ class BEVDecodeFunction(torch.autograd.Function):
             g0 = _matmul_wt(g1, w1.t())
             _lib.check(lib.so_tpv_decode_bwd_input(_p(g0), _p(a0), g0.numel(), st), 'so_tpv_decode_bwd_input')
             g_bev[r0:r0 + n] = g0
-        return g_bev, g_w1, g_b1, g_w2, g_b2, None
+        return g_bev, g_w1, g_b1, g_w2, g_b2, None, None
 
 
 # --------------------------------------------------------------------------------------- A6/A9 tensor-core projections
