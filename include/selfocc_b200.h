@@ -543,6 +543,41 @@ int so_sample_mean_forward(const float* x, int64_t n, int32_t op, void* workspac
 int so_sample_mean_backward(const float* x, int64_t n, int32_t op, const float* grad_out, float* grad_x, void* stream);
 
 /* ---------------------------------------------------------------------------------------
+ * 8f-2  the sparsity terms of loss/sparsity_loss.py, on the launches and conventions of so_sample_mean_* (fixed grid, fp64
+ * partials in SO_SAMPLE_MEAN_WORKSPACE_BYTES of workspace summed in index order, grad_out read on the device).
+ * so_sparsity_forward: SparsityLoss (:24-27), out[0] = mean over x [n] of sech^2(x / (2 scale)), evaluated as
+ *   4e / (1 + e)^2 with e = exp(-|x| / scale): 0, not NaN, where cosh overflows.  scale finite and != 0.
+ * so_sparsity_backward: grad_x = grad_out[0] / n * (-tanh(u) sech^2(u) / scale), u = x / (2 scale); overwritten.
+ * so_hard_sparsity_forward: HardSparsityLoss (:46-63) on the lattice x [H, W, D] (H * W * D < 2^31):
+ *   out[0] = relu(mean sigmoid(-scale x') - thresh), the mean in fp32 as the reference's, where x' is x with the crop
+ *   borders read as 100: crop (host, NULL = none) = {h0, h1, w0, w1, d0, d1}, the first h0 and last h1 cells along h (and
+ *   so on) are cropped, 0 = none, negative values are SO_ERR_INVALID_ARG.  x is never written.
+ * so_hard_sparsity_backward: grad_x = grad_out[0] / n * (-scale) sigmoid (1 - sigmoid), 0 in the cropped cells and
+ *   everywhere unless loss[0] (the forward's out, on the device) is > 0: relu's gradient, read without the host.
+ * AdaptiveSparsityLoss (:102-114) per ray: sdf, ts [n_rays, S] ray-major, depth [n_rays] fp32; a sample counts where
+ *   ts > depth + slack (fp32, as the reference's mask).
+ * so_adaptive_sparsity_rays -> ray_stats [n_rays] of (sum of relu(-sdf) over the counted samples, their count) in fp64
+ *   (16-byte aligned).  One warp per ray, fixed reduction order.  n_rays == 0 does nothing.
+ * so_adaptive_sparsity_reduce: ray_stats [n_rays >= 1] -> out[0] = (float)(sum / count) over all rays, NaN when no sample
+ *   counts (torch's mean of an empty tensor); total (NULL ok) [2] = the fp64 (sum, count).  A fixed grid sums the pairs
+ *   into workspace (SO_SAMPLE_MEAN_WORKSPACE_BYTES, 16-byte aligned) and one CTA sums those in index order: the result
+ *   is a function of ray_stats alone, so per-ray pairs gathered from ray-sharded ranks reduce to the unsharded value.
+ * so_adaptive_sparsity_backward: grad_stats [n_rays] (d loss / d sum, d loss / d count; the count slot is ignored, the
+ *   mask has no gradient) -> grad_sdf [n_rays, S] = -grad_stats[ray].sum where the sample counts and sdf < 0, else 0. */
+int so_sparsity_forward(const float* x, int64_t n, float scale, void* workspace, float* out, void* stream);
+int so_sparsity_backward(const float* x, int64_t n, float scale, const float* grad_out, float* grad_x, void* stream);
+int so_hard_sparsity_forward(const float* x, int32_t H, int32_t W, int32_t D, const int32_t* crop, float scale,
+                             float thresh, void* workspace, float* out, void* stream);
+int so_hard_sparsity_backward(const float* x, int32_t H, int32_t W, int32_t D, const int32_t* crop, float scale,
+                              const float* loss, const float* grad_out, float* grad_x, void* stream);
+int so_adaptive_sparsity_rays(const float* sdf, const float* ts, const float* depth, int64_t n_rays, int32_t S,
+                              float slack, double* ray_stats, void* stream);
+int so_adaptive_sparsity_reduce(const double* ray_stats, int64_t n_rays, void* workspace, float* out, double* total,
+                                void* stream);
+int so_adaptive_sparsity_backward(const float* sdf, const float* ts, const float* depth, int64_t n_rays, int32_t S,
+                                  float slack, const double* grad_stats, float* grad_sdf, void* stream);
+
+/* ---------------------------------------------------------------------------------------
  * 8f-2  training render with the objective's per-sample terms fused in.  Renders exactly as so_render_train_forward
  * (same sampling, field, alpha, compositing and kernel choice: the per-ray outputs are bit-identical) and, instead of
  * storing the per-sample tensors the losses read, reduces them per ray while it renders:

@@ -110,6 +110,13 @@ SIGNATURES = {
     'so_occ_confusion': (C.c_int, [_P, _P, _P, _L, _I, _I, _P, _P]),
     'so_sample_mean_forward': (C.c_int, [_P, _L, _I, _P, _P, _P]),
     'so_sample_mean_backward': (C.c_int, [_P, _L, _I, _P, _P, _P]),
+    'so_sparsity_forward': (C.c_int, [_P, _L, _F, _P, _P, _P]),
+    'so_sparsity_backward': (C.c_int, [_P, _L, _F, _P, _P, _P]),
+    'so_hard_sparsity_forward': (C.c_int, [_P, _I, _I, _I, _P, _F, _F, _P, _P, _P]),
+    'so_hard_sparsity_backward': (C.c_int, [_P, _I, _I, _I, _P, _F, _P, _P, _P, _P]),
+    'so_adaptive_sparsity_rays': (C.c_int, [_P, _P, _P, _L, _I, _F, _P, _P]),
+    'so_adaptive_sparsity_reduce': (C.c_int, [_P, _L, _P, _P, _P, _P]),
+    'so_adaptive_sparsity_backward': (C.c_int, [_P, _P, _P, _L, _I, _F, _P, _P, _P]),
     'so_render_train_objective_forward': (C.c_int, [_P, _P, C.POINTER(VolumeDesc), _P, _P, C.POINTER(RayDesc),
                                                     C.POINTER(RenderParams), _P, _P, C.POINTER(ObjectiveDesc)] + [_P] * 17),
     'so_render_train_objective_backward': (C.c_int, [_P, _P, C.POINTER(VolumeDesc), _P, _P, C.POINTER(RayDesc),

@@ -215,7 +215,8 @@ class ReprojLossMonoMultiNew(_ReprojLoss):
 #
 # EikonalLoss, SecondGradLoss and SoftSparsityLoss read the largest per-sample tensors of the objective (eik_grad,
 # second_grad: [rays, S, 3]; uniform_sdf: the lattice) and run on so_sample_mean_forward / _backward (csrc/loss_terms.cu):
-# one read forward, one read and one write backward, no per-sample temporaries.  RGBLossMS, SemLossMS, SemCELossMS and
+# one read forward, one read and one write backward, no per-sample temporaries.  SparsityLoss and HardSparsityLoss run on
+# the same launches (so_sparsity_*, so_hard_sparsity_*), AdaptiveSparsityLoss per ray (so_adaptive_sparsity_*).  RGBLossMS, SemLossMS, SemCELossMS and
 # EdgeLoss3DMS work per ray ([cameras, rays] grids) and stay in torch, batched over cameras.
 
 class _Term(nn.Module):
@@ -292,10 +293,25 @@ class SecondGradLoss(_SampleMeanTerm):
         return ops.SampleMeanFunction.apply(second_grad, 'abs')
 
 
-@LOSSES.register_module()
-class SoftSparsityLoss(_Term):
-    """mean relu(-density) (loss/sparsity_loss.py SoftSparsityLoss); the shipped configs feed it uniform_sdf."""
+class _LatticeTerm(_Term):
+    """A term on the density lattice; the shipped configs feed it uniform_sdf."""
     DEFAULT_KEYS = ('density',)
+
+    # under ray sharding the uniform_sdf lattice is the same on every rank: each rank computes the whole term, unscaled, and
+    # the average over the ranks of its (equal) gradients is the gradient
+    def local_payload(self, inputs, shard):
+        if self.input_dict['density'] != 'uniform_sdf':
+            raise NotImplementedError('%s under ray sharding takes the replicated uniform_sdf, got %r'
+                                      % (type(self).__name__, self.input_dict['density']))
+        return []
+
+    def from_gathered(self, full, inputs):
+        return self(inputs)
+
+
+@LOSSES.register_module()
+class SoftSparsityLoss(_LatticeTerm):
+    """mean relu(-density) (loss/sparsity_loss.py SoftSparsityLoss); the shipped configs feed it uniform_sdf."""
 
     def __init__(self, weight=1.0, input_dict=None, **kwargs):
         super().__init__(weight, input_dict)
@@ -303,16 +319,78 @@ class SoftSparsityLoss(_Term):
     def loss_func(self, density):
         return ops.SampleMeanFunction.apply(density, 'neg_relu')
 
-    # under ray sharding the uniform_sdf lattice is the same on every rank: each rank computes the whole term, unscaled, and
-    # the average over the ranks of its (equal) gradients is the gradient
+
+@LOSSES.register_module()
+class SparsityLoss(_LatticeTerm):
+    """mean sech^2(density / (2 scale)) (loss/sparsity_loss.py SparsityLoss, StreetSurf style), on so_sparsity_forward /
+    _backward: 0 where the reference's 1 / cosh overflows to 1 / inf."""
+
+    def __init__(self, weight=1.0, scale=1.0, input_dict=None, **kwargs):
+        super().__init__(weight, input_dict)
+        self.scale = scale
+
+    def loss_func(self, density):
+        return ops.SparsityFunction.apply(density, self.scale)
+
+
+@LOSSES.register_module()
+class HardSparsityLoss(_LatticeTerm):
+    """relu(mean sigmoid(-scale density) - thresh) over the [H, W, D] lattice with the crop borders counted as density 100
+    (loss/sparsity_loss.py HardSparsityLoss), on so_hard_sparsity_forward / _backward.  Unlike the reference, which writes
+    100 into the caller's tensor, the crop is applied inside the kernel: the input (and every term after this one that
+    reads it) is left as it was."""
+
+    def __init__(self, weight=1.0, scale=1.0, thresh=0.2, crop=((0, 0), (0, 0), (0, 0)), input_dict=None, **kwargs):
+        super().__init__(weight, input_dict)
+        self.scale = scale
+        self.thresh = thresh
+        self.crop = [[int(v) for v in row] for row in crop]
+
+    def loss_func(self, density):
+        return ops.HardSparsityFunction.apply(density, self.scale, self.thresh, self.crop)
+
+
+@LOSSES.register_module()
+class AdaptiveSparsityLoss(_Term):
+    """mean relu(-sdf) over the samples more than ``slack`` behind the ray's rendered depth, ts > depth + slack
+    (loss/sparsity_loss.py AdaptiveSparsityLoss).  Per ray so_adaptive_sparsity_rays forms (sum, count) in fp64 and
+    so_adaptive_sparsity_reduce takes their ratio in a fixed order: no boolean-mask gather, no host read; NaN when no sample
+    counts, as the reference's mean of an empty selection.  The gradient reaches the sdf only.
+
+    The reference's default keys name an ``sdfs`` input that NeuSHead does not emit: with ``return_sample_sdf=True`` the
+    head's per-sample sdf is ``sample_sdf``, so a config maps input_dict={'sdfs': 'sample_sdf', 'ts': 'ts',
+    'ms_depths': 'ms_depths'}.  Under ray sharding each rank sends its rays' (sum, count) pairs; the gathered pairs reduce to
+    the unsharded value bit for bit."""
+    DEFAULT_KEYS = ('sdfs', 'ts', 'ms_depths')
+
+    def __init__(self, weight=1, input_dict=None, slack=4.0, **kwargs):
+        super().__init__(weight, input_dict)
+        self.slack = slack
+
+    def _args(self, inputs):
+        missing = [(k, v) for k, v in self.input_dict.items() if v not in inputs]
+        if missing:
+            raise KeyError('AdaptiveSparsityLoss reads %s, which the inputs lack (the head emits its per-sample sdf as '
+                           "'sample_sdf' with return_sample_sdf=True: map input_dict {'sdfs': 'sample_sdf', ...})"
+                           % ', '.join('%r (input_dict key %r)' % (v, k) for k, v in missing))
+        return super()._args(inputs)
+
+    def loss_func(self, sdfs, ts, ms_depths):
+        return ops.AdaptiveSparsityReduceFunction.apply(self._rays(sdfs, ts, ms_depths))
+
+    def _rays(self, sdfs, ts, ms_depths):
+        """[N, R, 2] fp64 (sum, count) per ray of camera."""
+        depths = ms_depths[0]
+        bs, num_cams, num_rays = depths.shape
+        if bs != 1:
+            raise NotImplementedError('batch size %d: AdaptiveSparsityLoss supports batch size 1 (as the reference)' % bs)
+        return ops.AdaptiveSparsityRaysFunction.apply(self.slack, [t.detach() for t in ts], depths[0].detach(), *sdfs)
+
     def local_payload(self, inputs, shard):
-        if self.input_dict['density'] != 'uniform_sdf':
-            raise NotImplementedError('SoftSparsityLoss under ray sharding takes the replicated uniform_sdf, got %r'
-                                      % self.input_dict['density'])
-        return []
+        return [(self._rays(**self._args(inputs)), shard[2])]
 
     def from_gathered(self, full, inputs):
-        return self(inputs)
+        return self.weight * ops.AdaptiveSparsityReduceFunction.apply(full[0])
 
 
 def sample_at_rays(imgs, rays, img_size, padding):

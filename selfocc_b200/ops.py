@@ -1030,3 +1030,145 @@ class SampleMeanFunction(torch.autograd.Function):
         _lib.check(_lib.load().so_sample_mean_backward(_p(x), x.numel(), SAMPLE_MEAN_OPS[ctx.op], _p(g), _p(gx), _stream()),
                    'so_sample_mean_backward')
         return gx, None
+
+
+# --------------------------------------------------------------------------------------- 8f-2 sparsity terms
+def _lattice_input(x):
+    if isinstance(x, torch.Tensor) and x.is_cuda and x.dtype == torch.float32:
+        x = x.contiguous()
+    _chk(x, name='density')
+    if x.numel() == 0:
+        raise ValueError('the mean of an empty tensor is undefined')
+    return x
+
+
+class SparsityFunction(torch.autograd.Function):
+    """SparsityLoss's mean of sech^2(x / (2 scale)) over a fp32 CUDA tensor (so_sparsity_forward / _backward).
+    apply(x, scale) -> 0-d fp32 tensor; finite (0) where torch.cosh would overflow.  Non-contiguous input is copied."""
+
+    @staticmethod
+    def forward(ctx, x, scale):
+        x = _lattice_input(x)
+        ws = torch.empty(SAMPLE_MEAN_WORKSPACE_BYTES // 8, dtype=torch.float64, device=x.device)
+        out = torch.empty((), device=x.device)
+        _lib.check(_lib.load().so_sparsity_forward(_p(x), x.numel(), float(scale), _p(ws), _p(out), _stream()),
+                   'so_sparsity_forward')
+        ctx.scale = float(scale)
+        ctx.save_for_backward(x)
+        return out
+
+    @staticmethod
+    @torch.autograd.function.once_differentiable
+    def backward(ctx, g):
+        x, = ctx.saved_tensors
+        g = _chk(g.reshape(1).contiguous(), name='grad_out')
+        gx = torch.empty_like(x)
+        _lib.check(_lib.load().so_sparsity_backward(_p(x), x.numel(), ctx.scale, _p(g), _p(gx), _stream()),
+                   'so_sparsity_backward')
+        return gx, None
+
+
+def _crop6(crop):
+    """[[h0, h1], [w0, w1], [d0, d1]] -> the entry points' int32[6]; the reference crops only where a value is > 0."""
+    flat = [int(v) for row in crop for v in row]
+    if len(flat) != 6:
+        raise ValueError('crop must be [[h0, h1], [w0, w1], [d0, d1]], got %r' % (crop,))
+    return (C.c_int32 * 6)(*[max(v, 0) for v in flat])
+
+
+class HardSparsityFunction(torch.autograd.Function):
+    """HardSparsityLoss's relu(mean sigmoid(-scale x') - thresh) over the lattice x [H, W, D] (so_hard_sparsity_forward /
+    _backward), x' = x with the crop borders ([[h0, h1], [w0, w1], [d0, d1]]) read as 100 inside the kernel: x is not
+    written.  A crop-free term takes any shape.  The backward reads the forward's value on the device for relu's gate."""
+
+    @staticmethod
+    def forward(ctx, x, scale, thresh, crop):
+        x = _lattice_input(x)
+        c = _crop6(crop)
+        if x.dim() == 3:
+            dims = tuple(x.shape)
+        elif not any(c):
+            dims = (1, 1, x.numel())
+        else:
+            raise ValueError('HardSparsityLoss crops a [H, W, D] lattice, got shape %s' % (tuple(x.shape),))
+        ws = torch.empty(SAMPLE_MEAN_WORKSPACE_BYTES // 8, dtype=torch.float64, device=x.device)
+        out = torch.empty((), device=x.device)
+        _lib.check(_lib.load().so_hard_sparsity_forward(_p(x), *dims, c, float(scale), float(thresh), _p(ws), _p(out),
+                                                         _stream()), 'so_hard_sparsity_forward')
+        ctx.args = (dims, c, float(scale))
+        ctx.save_for_backward(x, out)
+        return out
+
+    @staticmethod
+    @torch.autograd.function.once_differentiable
+    def backward(ctx, g):
+        x, out = ctx.saved_tensors
+        dims, c, scale = ctx.args
+        g = _chk(g.reshape(1).contiguous(), name='grad_out')
+        gx = torch.empty_like(x)
+        _lib.check(_lib.load().so_hard_sparsity_backward(_p(x), *dims, c, scale, _p(out), _p(g), _p(gx), _stream()),
+                   'so_hard_sparsity_backward')
+        return gx, None, None, None
+
+
+class AdaptiveSparsityRaysFunction(torch.autograd.Function):
+    """AdaptiveSparsityLoss's per-ray statistics (so_adaptive_sparsity_rays / _backward).
+    apply(slack, ts, depth, *sdfs): ts and sdfs per camera R * S samples ray-major (NeuSHead's ts and sample_sdf), depth
+    [N, R] -> stats [N, R, 2] fp64 = (sum of relu(-sdf), count) over the samples with ts > depth + slack.  The gradient
+    reaches the sdfs only (the mask is not differentiable), as views of one [N, R*S] buffer."""
+
+    @staticmethod
+    def forward(ctx, slack, ts, depth, *sdfs):
+        N, R = depth.shape
+        sdf = _one_buffer(sdfs, 'sdfs')
+        t = _one_buffer(ts, 'ts')
+        depth = _chk(depth.contiguous(), name='depth')
+        n = sdf.shape[1]
+        if N != len(sdfs) or len(ts) != N or t.shape != sdf.shape or (R and n % R) or (not R and n):
+            raise ValueError('AdaptiveSparsityLoss: %d cameras of %d rays in the depths, but %d sdfs of %d and %d ts of %d '
+                             'samples' % (N, R, len(sdfs), n, len(ts), t.shape[1]))
+        S = n // R if R else 1
+        stats = torch.empty(N, R, 2, dtype=torch.float64, device=sdf.device)
+        _lib.check(_lib.load().so_adaptive_sparsity_rays(_p(sdf), _p(t), _p(depth), N * R, S, float(slack), _p(stats),
+                                                          _stream()), 'so_adaptive_sparsity_rays')
+        ctx.args = (float(slack), S, [s.shape for s in sdfs])
+        ctx.save_for_backward(sdf, t, depth)
+        return stats
+
+    @staticmethod
+    @torch.autograd.function.once_differentiable
+    def backward(ctx, g_stats):
+        sdf, t, depth = ctx.saved_tensors
+        slack, S, shapes = ctx.args
+        g = _chk(g_stats.contiguous(), dtype=torch.float64, name='grad_stats')
+        gx = torch.empty_like(sdf)
+        _lib.check(_lib.load().so_adaptive_sparsity_backward(_p(sdf), _p(t), _p(depth), depth.numel(), S, slack, _p(g),
+                                                              _p(gx), _stream()), 'so_adaptive_sparsity_backward')
+        return (None, None, None) + tuple(gx[i].view(shp) for i, shp in enumerate(shapes))
+
+
+class AdaptiveSparsityReduceFunction(torch.autograd.Function):
+    """sum / count over per-ray (sum, count) pairs [..., 2] fp64 in a fixed order (so_adaptive_sparsity_reduce) -> 0-d
+    fp32; NaN when nothing counts.  The gradient is d loss / d sum = grad / count for every ray, 0 for the counts."""
+
+    @staticmethod
+    def forward(ctx, stats):
+        stats = _chk(stats.contiguous(), dtype=torch.float64, name='ray_stats')
+        if stats.shape[-1] != 2 or stats.numel() == 0:
+            raise ValueError('ray_stats must be non-empty (sum, count) pairs, got shape %s' % (tuple(stats.shape),))
+        ws = torch.empty(SAMPLE_MEAN_WORKSPACE_BYTES // 8, dtype=torch.float64, device=stats.device)
+        out = torch.empty((), device=stats.device)
+        total = torch.empty(2, dtype=torch.float64, device=stats.device)
+        _lib.check(_lib.load().so_adaptive_sparsity_reduce(_p(stats), stats.numel() // 2, _p(ws), _p(out), _p(total),
+                                                            _stream()), 'so_adaptive_sparsity_reduce')
+        ctx.shape = stats.shape
+        ctx.save_for_backward(total)
+        return out
+
+    @staticmethod
+    @torch.autograd.function.once_differentiable
+    def backward(ctx, g):
+        total, = ctx.saved_tensors
+        gs = torch.zeros(ctx.shape, dtype=torch.float64, device=g.device)
+        gs[..., 0] = g.double() / total[1]              # a device scalar broadcast: no host read
+        return gs
