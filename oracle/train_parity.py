@@ -49,10 +49,11 @@ def flip_rays(grid, *others):
 
 
 def oracle_train(vol64, mapping, o, d, nrm, aabb, inv_s, S, cot, jitter=None, color_dims=0, bkgd_rand=None, grid_override=None,
-                 depth_clip=None, chunk=512, **kw):
+                 depth_clip=None, chunk=512, extra=None, **kw):
     """Differentiable fp64 oracle over ray chunks: returns (outputs in kernel names, d/d vol [Cf,H,W,Z], d/d inv_s,
     sum over samples of |per-sample term of d/d inv_s|) where the gradients are those of sum_k <output_k, cot[k]>
-    (missing cotangents = zero)."""
+    (missing cotangents = zero).  ``extra(sl, named)`` -> (loss term, {name: per-ray tensor}) adds terms computed from a
+    chunk's outputs (rays ``sl``) to its loss and outputs (train_objective.py)."""
     vol = vol64.detach().clone().requires_grad_(True)
     invs = torch.tensor(float(inv_s), dtype=torch.float64, device=vol.device, requires_grad=True)
     n = o.shape[0]
@@ -71,8 +72,12 @@ def oracle_train(vol64, mapping, o, d, nrm, aabb, inv_s, S, cot, jitter=None, co
         r['deltas'] = (r['ends'] - r['starts']) / nrm[sl]
         named = {k: r[rk] for k, rk in PER_SAMPLE + PER_RAY if rk in r}
         loss = sum((named[k] * cot[k][sl].to(named[k])).sum() for k in DIFF if k in cot and k in named)
+        if extra is not None:
+            term, more = extra(sl, named)
+            loss = loss + term
+            named.update(more)
         loss.backward()
-        mass += float(iv.grad.abs().sum())
+        mass += float(iv.grad.abs().sum()) if iv.grad is not None else 0.0      # None: no term depends on inv_s
         for k, t in named.items():
             outs.setdefault(k, []).append(t.detach())
     outs = {k: torch.cat(v) for k, v in outs.items()}

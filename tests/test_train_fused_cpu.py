@@ -156,3 +156,85 @@ def test_fuse_objective_refuses_unsupported_objectives(cfgs, head):
 def test_objective_without_per_sample_terms_fuses_to_nothing():
     from selfocc_b200.loss import fuse_objective
     assert fuse_objective(_head(), _multiloss([dict(type='SecondGradLoss')])) == dict(mode=None, img_size=None, eikonal=False)
+
+
+# ------------------------------------------------------------------------------------------------ fp64 objective oracle
+def _tiny_objective_scene(mode):
+    """2 cameras x 4 x 3 rays x 16 samples on a small analytic volume with 3 colour channels, the temporal rig of the
+    cameras and textured neighbour frames: (render args, objective, cotangents)."""
+    import torch
+    from oracle import rays as orays
+    from oracle.mapping import GridMeterMappingRef
+    from selfocc_b200 import synth
+    margs, aabb = synth.small_mapping(10, 6, rng=20.0, z0=-2.0, z1=4.0)
+    m = GridMeterMappingRef(**margs)
+    g = torch.Generator().manual_seed(3)
+    sdf = synth.analytic_sdf_volume(m, noise=0.02, seed=2)
+    vol = torch.cat([sdf[None], 0.7 * torch.randn(3, *sdf.shape, generator=g)]).double()
+    yaws = synth.NUSC_YAWS[:2]
+    _, i2l = synth.camera_rig(yaws, f=126.6, cx=80., cy=45., height=0.5, radius=0.2)
+    prev, nxt = synth.temporal_rig(yaws, f=126.6, cx=80., cy=45., height=0.5, radius=0.2)
+    pix = orays.fixed_ray_grid([3, 4], [90, 160]) + 0.37
+    origin, direction = orays.img2lidar_rays(torch.tensor(i2l, dtype=torch.float32)[None], pix)
+    o, d, nrm = orays.flatten_rays(origin.double(), direction.double())
+    n, S, R = o.shape[0], 16, pix.shape[0]
+    imgs = synth.textured_images(6, 30, 50, seed=4).double().reshape(3, 2, 3, 30, 50)
+    obj = dict(mode=mode, eikonal=True, images=tuple(imgs), img2prev=torch.from_numpy(prev), img2next=torch.from_numpy(nxt),
+               img_size=(90, 160), cam=torch.arange(2).repeat_interleave(R), pix=pix.double().repeat(2, 1))
+    sets = 1 if mode == 'combine' else 2
+    cot = dict(depth=torch.randn(n, generator=g, dtype=torch.float64), acc=torch.randn(n, generator=g, dtype=torch.float64),
+               rgb=torch.randn(n, 3, generator=g, dtype=torch.float64),
+               reproj_stats=torch.randn(n, 6 * sets, generator=g, dtype=torch.float64), eikonal_mean=torch.tensor(0.7))
+    jitter = torch.rand(n, S + 1, generator=g, dtype=torch.float64)
+    bk = torch.rand(n, 3, generator=g, dtype=torch.float64)
+    return dict(vol=vol, m=m, o=o, d=d, nrm=nrm, aabb=aabb, S=S, R=R, jitter=jitter, bk=bk), obj, cot
+
+
+@pytest.mark.parametrize('mode', ['combine', 'multi_new'])
+def test_objective_oracle_equals_render_then_statistics_then_eikonal(mode):
+    """oracle.train_objective's chunked composition (chunks of 5 rays: they straddle the camera boundary) equals the
+    plain fp64 render of every ray at once followed by ray_stats_ref and eikonal_ref: outputs and d/d volume, d/d inv_s."""
+    import torch
+    from oracle import losses as olosses, render as orender, reproj as oreproj, train_parity as tp
+    from oracle.train_objective import oracle_objective
+    sc, obj, cot = _tiny_objective_scene(mode)
+    o, d, nrm, S, R, inv_s = sc['o'], sc['d'], sc['nrm'], sc['S'], sc['R'], 20.0
+    _, clip = tp.sample_geometry(sc['m'], o, d, sc['aabb'], S, sc['jitter'])
+    got, g_vol, g_inv, _ = oracle_objective(sc['vol'], sc['m'], o, d, nrm, sc['aabb'], inv_s, S, cot, obj, jitter=sc['jitter'],
+                                            color_dims=3, bkgd_rand=sc['bk'], depth_clip=clip, chunk=5)
+    vol = sc['vol'].clone().requires_grad_(True)
+    invs = torch.tensor(inv_s, dtype=torch.float64, requires_grad=True)
+    r = orender.neus_render_chunk(vol, sc['m'], o, d, nrm, sc['aabb'], invs, S=S, training=True, jitter=sc['jitter'],
+                                  color_dims=3, bkgd='random', bkgd_rand=sc['bk'], differentiable=True, depth_clip=clip)
+    ts = (r['starts'] + r['ends']) / 2 / nrm
+    w = r['weights']
+    stats, cols = oreproj.ray_stats_ref(mode, *obj['images'], list(w.reshape(2, R * S)), list(ts.reshape(2, R * S)),
+                                        obj['img2prev'], obj['img2next'], obj['pix'][:R], obj['img_size'])
+    eik = olosses.eikonal_ref(r['eik_grad'])
+    loss = (r['depth'] * cot['depth']).sum() + (r['accumulation'] * cot['acc']).sum() + (r['rgb'] * cot['rgb']).sum() + \
+        (stats.reshape(-1, stats.shape[-1]) * cot['reproj_stats']).sum() + eik * cot['eikonal_mean']
+    ref_vol, ref_inv = torch.autograd.grad(loss, [vol, invs])
+    assert (stats[..., 5::6] == 1).any() and (stats[..., 0] > 1e-3).any()        # the scene exercises the reprojection
+    close = lambda a, b: torch.allclose(a, b.detach().reshape(a.shape), rtol=1e-10, atol=1e-12)
+    assert close(got['reproj_stats'], stats) and close(got['reproj_colours'], cols)
+    assert close(got['eikonal_mean'], eik) and close(got['depth'], r['depth']) and close(got['rgb'], r['rgb'])
+    assert close(g_vol, ref_vol) and close(g_inv, ref_inv)
+    assert ref_vol.abs().max() > 0 and ref_inv.abs() > 0
+    # the valid-sample counts: the W column of the statistics at unit weights
+    ones, _ = oreproj.ray_stats_ref(mode, *obj['images'], list(torch.ones(2, R * S, dtype=torch.float64)), list(ts.reshape(2, R * S)),
+                                    obj['img2prev'], obj['img2next'], obj['pix'][:R], obj['img_size'])
+    assert torch.equal(got['reproj_valid'], ones.reshape(2 * R, -1)[:, 0::6])
+
+
+def test_reproj_guard_flags_samples_on_an_image_bound_or_at_zero_depth():
+    """With img2prev = img2next = identity a sample (u t, v t, t, 1) reprojects to pixel (u, v) at depth t."""
+    import torch
+    from oracle.train_objective import reproj_guard_rays, GUARD_PX, GUARD_Z
+    eye = torch.eye(4, dtype=torch.float64)[None]
+    pix = torch.tensor([[50., 40.], [0.0, 40.], [160. - GUARD_PX / 2, 40.], [50., 90.], [50., 40.], [50., 40.], [0.01, 89.9]],
+                       dtype=torch.float64)
+    ts = torch.tensor([[1., 2., 3.]] * 7, dtype=torch.float64)
+    ts[4, 1] = GUARD_Z / 2                  # a sample at (almost) zero depth in the other frame
+    ts[5, 2] = -3.0                         # behind the other camera: invalid whatever its pixel, never ambiguous
+    bad = reproj_guard_rays(ts, torch.zeros(7, dtype=torch.long), pix, eye, eye, (90, 160))
+    assert bad.tolist() == [False, True, True, True, True, False, False]
