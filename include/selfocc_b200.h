@@ -332,6 +332,29 @@ int so_occ_confusion(const uint8_t* pred, const uint8_t* gt, const uint8_t* mask
                      int64_t* counts, void* stream);
 
 /* ---------------------------------------------------------------------------------------
+ * Surface extraction (the mesh that vis_3d.py / vis_3d_scene.py draw as voxels from forward_occ(..., occ_only=True)):
+ * marching cubes over the lattice of so_occ_lattice_labels (axes xs [nx], ys [ny], zs [nz], layout [ny, nx, nz], values the
+ * so_field_query sdf, evaluated on the fly).  Point p = (iy, ix, iz), index (iy * nx + ix) * nz + iz, is inside when
+ * sdf <= thresh, so the surface bounds exactly the points so_occ_lattice_labels marks occupied; it is open where it leaves
+ * the lattice.  Point p owns its +x, +y and +z edges; an edge crosses when its ends lie on different sides, and its vertex
+ * is p_a + t (p_b - p_a), t = (thresh - s_a) / (s_b - s_a).  Cell p is the cube whose lowest corner is p; its triangles
+ * come from the case table of selfocc_b200/mc_table.py (csrc/mc_table.cuh), counter-clockwise seen from the outside
+ * (sdf > thresh).
+ *   so_mesh_count: counts int32 [2, N] (N = nx * ny * nz): counts[0][p] = crossing edges owned by p, counts[1][p] =
+ *     triangles of cell p (0 on the upper border); edge_mask uint8 [N], bit a = p's +a edge crosses (a = x, y, z).
+ *   so_mesh_emit: given scans = the INCLUSIVE scans of both rows of counts (int32 [2, N]), the same edge_mask and their
+ *     totals n_vertices = sum(counts[0]), n_faces = sum(counts[1]): vertices [n_vertices, 3] fp32 metres in ascending
+ *     owner index then axis, faces [n_faces, 3] int32 vertex ids in ascending cell index then table order.  One thread
+ *     writes each output: bit-identical run to run.
+ * Refused (SO_ERR_INVALID_ARG): null pointers, an axis shorter than 2, negative totals.  N >= 2^31 and totals >= 2^31
+ * (int32 ids) are SO_ERR_UNSUPPORTED.  Both checks come before any CUDA call. */
+int so_mesh_count(const float* vol_sdf, const so_volume_desc* vol_host, const float* xs, int32_t nx, const float* ys, int32_t ny,
+                  const float* zs, int32_t nz, float thresh, int32_t* counts, uint8_t* edge_mask, void* stream);
+int so_mesh_emit(const float* vol_sdf, const so_volume_desc* vol_host, const float* xs, int32_t nx, const float* ys, int32_t ny,
+                 const float* zs, int32_t nz, float thresh, const int32_t* scans, const uint8_t* edge_mask, int64_t n_vertices,
+                 int64_t n_faces, float* vertices, int32_t* faces, void* stream);
+
+/* ---------------------------------------------------------------------------------------
  * A7/A8  multi-scale deformable attention forward.  Drop-in for
  * MultiScaleDeformableAttnFunction.apply(value, spatial_shapes, level_start_index,
  * sampling_locations, attention_weights, im2col_step) of mmcv==2.0.1 (reference call sites

@@ -108,6 +108,8 @@ SIGNATURES = {
     'so_occ_lattice_labels': (C.c_int, [_P, _P, C.POINTER(VolumeDesc), _P, _I, _P, _I, _P, _I, _F, _I, _I, _P, _P, _P, _P]),
     'so_occ_sample_labels': (C.c_int, [_P, _P, C.POINTER(VolumeDesc), _P, _I, _P, _I, _P, _I, _P, _L, _F, _I, _I, _P, _P, _P, _P]),
     'so_occ_confusion': (C.c_int, [_P, _P, _P, _L, _I, _I, _P, _P]),
+    'so_mesh_count': (C.c_int, [_P, C.POINTER(VolumeDesc), _P, _I, _P, _I, _P, _I, _F, _P, _P, _P]),
+    'so_mesh_emit': (C.c_int, [_P, C.POINTER(VolumeDesc), _P, _I, _P, _I, _P, _I, _F, _P, _P, _L, _L, _P, _P, _P]),
     'so_sample_mean_forward': (C.c_int, [_P, _L, _I, _P, _P, _P]),
     'so_sample_mean_backward': (C.c_int, [_P, _L, _I, _P, _P, _P]),
     'so_sparsity_forward': (C.c_int, [_P, _L, _F, _P, _P, _P]),

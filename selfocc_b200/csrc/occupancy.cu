@@ -5,29 +5,10 @@
 //   so_occ_confusion       the confusion matrix every counter of MeanIoU / SSCMetrics is derived from
 // Lattice values are the field query of so_field_query (same device functions, same operands, same rounding), so the
 // labels equal thresholding / arg-maxing forward_occ's outputs without materialising them.
-#include "render_common.cuh"
+#include "lattice.cuh"
 #include <math.h>
 
 namespace so {
-
-struct LatticeDev {
-  const float *xs, *ys, *zs;  // lattice axes in metres: W = nx (x), H = ny (y), D = nz (z)
-  int nx, ny, nz;
-};
-
-__device__ __forceinline__ Taps lattice_taps(const VolumeDev& V, const LatticeDev& L, int iy, int ix, int iz) {
-  float kh, kw, kd;
-  float gh = axis_m2g(V.ax[0], __ldg(L.ys + iy), kh);
-  float gw = axis_m2g(V.ax[1], __ldg(L.xs + ix), kw);
-  float gd = axis_m2g(V.ax[2], __ldg(L.zs + iz), kd);
-  return make_taps(V, gh, gw, gd);
-}
-
-__device__ __forceinline__ float tap_sdf(const VolumeDev& V, const Taps& t) {
-  float s, dgh, dgw, dgd;
-  gather_sdf(V, t, s, dgh, dgw, dgd);
-  return s;
-}
 
 // running first-maximum, NaN counting as the maximum (torch.argmax)
 __device__ __forceinline__ void argmax_update(float v, int c, float& best, int& arg) {

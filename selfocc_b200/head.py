@@ -11,6 +11,7 @@ import numpy as np
 import torch
 import torch.nn as nn
 
+from . import mesh as mesh_mod
 from . import occupancy, ops
 from .encoder import _metas_matrix
 from .mapping import GridMeterMapping
@@ -474,6 +475,29 @@ class NeuSHead(nn.Module):
         occ, sem = occupancy.occupancy_labels(f.vol_sdf, f.vol_feat, f.desc, axes, thresh, sem_begin=3, n_sem=n_sem,
                                               lut=lut if n_sem else None, points_u=u)
         return {'occ': occ, 'sem': sem} if n_sem else {'occ': occ}
+
+    @torch.no_grad()
+    def mesh(self, aabb, resolution, thresh=0.0, lut=None, representation=None):
+        """The surface of the prepared frame: marching cubes on the lattice of get_uniform_sdf(aabb, resolution), the level
+        set sdf = thresh, so that it bounds exactly the points occupancy(aabb, resolution, thresh) labels occupied (the
+        reference's vis_3d.py draws those voxels from forward_occ's lattice).  ``representation``: decode it first, as
+        forward_occ does; otherwise the volume of the last prepare() / forward() is used.
+
+        Returns {'vertices': fp32 [V, 3] lidar-frame metres, 'faces': int32 [F, 3] (counter-clockwise seen from outside),
+        'normals': fp32 [V, 3] unit field gradients}, plus 'sem' uint8 [V] = lut[argmax(logits)] for return_sem heads
+        (lut None: the raw argmax) and 'rgb' fp32 [V, 3], the SH degree-0 colour, for heads with colour channels.  One
+        synchronising read per call; mesh.write_ply writes the dict to a file."""
+        f = self.model.field
+        if representation is not None:
+            f.pre_compute_density_color(representation)
+        if f.vol_sdf is None:
+            raise RuntimeError('mesh() called before prepare()/forward(): no decoded volume')
+        axes = occupancy.lattice_axes(aabb, resolution, f.vol_sdf.device)
+        vertices, faces = mesh_mod.marching_cubes(f.vol_sdf, f.desc, axes, thresh)
+        n_sem = f.color_dims - 3 if self.return_sem else 0
+        attrs = mesh_mod.vertex_attributes(f.vol_sdf, f.vol_feat, f.desc, vertices, n_sem=n_sem, lut=lut,
+                                           rgb=f.color_dims >= 3, sh_act=f.sh_act)
+        return dict(vertices=vertices, faces=faces, **attrs)
 
     def forward(self, representation, metas=None, **kwargs):
         """neus_head.py:473-713 (training form: per-sample weights / ts / deltas / eik_grad)."""
