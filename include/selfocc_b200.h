@@ -611,18 +611,26 @@ int so_adaptive_sparsity_backward(const float* sdf, const float* ts, const float
  *   eikonal (eikonal = 1): eikonal_mean [1] = mean over the call's rays x S samples of (|eik_grad| - 1)^2, as
  *     so_sample_mean_forward(EIKONAL): per-ray fp64 sums in `workspace` (8-byte aligned, >= 8 * ray_count bytes), then one
  *     index-ordered pass.  Deterministic, no float atomics, the same value on every device.
+ *   second grad (second_grad = 1): second_grad_mean [1] = mean over the call's rays x S samples x 3 of |second_grad|, as
+ *     so_field_second_grad followed by so_sample_mean_forward(ABS), with second_grad taken at the render's own sample point
+ *     (the point eik_grad is taken at: the bin mid-point, or its start with anchor_mid = 0).  Per-ray fp64 sums in
+ *     `workspace` after the eikonal sums (>= 16 * ray_count bytes with both terms, >= 8 * ray_count with this one alone),
+ *     then one index-ordered pass.  Deterministic, no float atomics.
  * The per-sample outputs of so_render_train_forward stay available and NULL = not written (a head that also needs the
  * sample positions asks for ts / deltas).
  * so_render_train_objective_backward recomputes the forward as so_render_train_backward does and forms every sample's
  * d loss / d w (the adjoint of so_reproj_stats_backward: reproj_stats = the forward's, grad_reproj_stats [rays, 6 * sets])
  * and d loss / d eik_grad (the adjoint of so_sample_mean_backward: grad_eikonal_mean [1] on the device, NULL = 0, never
- * read on the host) in registers; with the per-ray g_depth / g_acc / g_rgb / g_sem it ACCUMULATES into g_vol_sdf,
+ * read on the host) in registers; with second_grad = 1 it adds the second-grad mean's sdf-corner gradients
+ * (grad_second_grad_mean [1] / (3 rays S) * sign(second_grad), sign(0) = 0, through so_field_second_grad_backward's
+ * corner coefficients; NULL = 0, never read on the host) to each sample's sdf scatter; with the per-ray g_depth / g_acc / g_rgb / g_sem it ACCUMULATES into g_vol_sdf,
  * g_vol_feat and g_inv_s as so_render_train_backward does (the caller zero-fills them).  g_inv_s is formed from per-ray
  * fp64 values in `workspace` (as the forward's eikonal sums: >= 8 * ray_count bytes when g_inv_s != NULL) summed in ray
  * order, so it is the same on every run; g_vol_sdf / g_vol_feat are accumulated with atomics.
  * Argument errors return SO_ERR_INVALID_ARG / SO_ERR_UNSUPPORTED before any launch: the checks of so_render_train_forward /
  * _backward (S <= 256) and, for the objective, those of so_reproj_stats_forward (operands, image sizes) plus 4-byte
- * alignment of every float operand. */
+ * alignment of every float operand, eikonal and second_grad in {0, 1}, and the workspace's size and alignment.
+ * A zero-initialised descriptor tail (second_grad = 0, NULL pointers) leaves the second-grad term off. */
 #define SO_OBJECTIVE_NO_REPROJ (-1)
 typedef struct so_objective_desc {
   int32_t reproj_mode;       /* SO_REPROJ_COMBINE, SO_REPROJ_MULTI_NEW or SO_OBJECTIVE_NO_REPROJ */
@@ -635,8 +643,12 @@ typedef struct so_objective_desc {
   const float* next_imgs;
   int32_t img_h, img_w;
   float size_h, size_w;      /* the loss's img_size */
-  void* workspace;           /* forward with eikonal, backward with g_inv_s: >= 8 * ray_count bytes, 8-byte aligned */
+  void* workspace;           /* forward: >= 8 * ray_count bytes per mean computed (eikonal, second grad), backward with
+                                g_inv_s: >= 8 * ray_count bytes; 8-byte aligned */
   int64_t workspace_bytes;
+  int32_t second_grad;       /* 1: the second-grad mean is computed (forward) and differentiated (backward), 0: not */
+  float* second_grad_mean;   /* forward output [1] when second_grad = 1 */
+  const float* grad_second_grad_mean;  /* backward input [1] on the device, NULL = 0 */
 } so_objective_desc;
 int so_render_train_objective_forward(const float* vol_sdf, const float* vol_feat, const so_volume_desc* vol_host,
                                       const float* cam_mats, const float* pix, const so_ray_desc* rays_host,

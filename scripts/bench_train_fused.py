@@ -1,6 +1,6 @@
 """One training step with the objective fused into the training render (loss.fuse_objective) against the same step unfused,
 alternated in one process, on one GPU:
-    python scripts/bench_train_fused.py [--steps K] [--rounds N]
+    python scripts/bench_train_fused.py [--steps K] [--rounds N] [--second-grad]
 Two workloads, each at nuScenes sizes (6 cams x 48x100 rays x 256 samples, TPV 257x257x25, fp32):
   shipped : the bench_train_step.py --loss shipped step -- nuscenes_occ's whole MultiLoss (reprojection, RGBLossMS with
             SSIM, EikonalLoss, SecondGradLoss, SemCELossMS), 24 colour dims, semantics, second grad under its opt-in
@@ -8,7 +8,9 @@ Two workloads, each at nuScenes sizes (6 cams x 48x100 rays x 256 samples, TPV 2
   depth   : nuscenes_depth's MultiLoss (ReprojLossMonoMultiNewCombine, EikonalLoss, EdgeLoss3DMS), a 3-channel colour head.
 Each round runs K unfused steps then K fused steps per workload (device-timed, after warm-up); prints one JSON line per
 workload with the per-round ms per step (median), peak device memory of a step and library launches per step, and the
-card's name and power limit."""
+card's name and power limit.
+--second-grad: the shipped workload only, alternating three forms: unfused, fused (SecondGradLoss on the head's
+second_grad tensor) and fused with second_grad=True (SecondGradLoss's mean taken in the render)."""
 import json
 import os
 import subprocess
@@ -27,6 +29,7 @@ import selfocc_b200.segmentor  # noqa: F401,E402
 
 K = int(sys.argv[sys.argv.index('--steps') + 1]) if '--steps' in sys.argv else 5
 ROUNDS = int(sys.argv[sys.argv.index('--rounds') + 1]) if '--rounds' in sys.argv else 3
+SECOND_GRAD = '--second-grad' in sys.argv
 dev = torch.device('cuda', 0)
 margs = dict(synth.NUSC_MAPPING, h_size=[128, 0], h_range=[40.0, 0], w_size=[128, 0], w_range=[40.0, 0], d_size=[24, 0],
              d_range=[-1.0, 5.4, 5.4])
@@ -67,10 +70,12 @@ def workload(name):
     else:
         objective = LOSSES.build(dict(type='MultiLoss', loss_cfgs=NUSC_DEPTH))
     opt = torch.optim.AdamW(model.parameters(), lr=1e-4)
-    fused_rec = fuse_objective(model.head, objective)
+    recs = {False: None, True: fuse_objective(model.head, objective)}
+    if shipped:
+        recs['sg'] = fuse_objective(model.head, objective, second_grad=True)
 
     def step(fused):
-        model.head.fused_objective = fused_rec if fused else None
+        model.head.fused_objective = recs[fused]
         opt.zero_grad(set_to_none=True)
         out = model(ms_img_feats=feats, metas=metas, curr_imgs=imgs[0], prev_imgs=imgs[1], next_imgs=imgs[2])
         loss, _ = objective(dict(out, color_imgs=imgs[3]))
@@ -105,19 +110,22 @@ def card():
 
 
 def main():
-    for name in ('shipped', 'depth'):
+    forms = ((False, 'unfused'), (True, 'fused')) + ((('sg', 'fused_second_grad'),) if SECOND_GRAD else ())
+    for name in ('shipped',) if SECOND_GRAD else ('shipped', 'depth'):
         step = workload(name)
-        for fused in (False, True, False, True):       # warm-up of both forms
-            step(fused)
-        res = {False: [], True: []}
+        for _ in range(2):                             # warm-up of every form
+            for fused, _tag in forms:
+                step(fused)
+        res = {fused: [] for fused, _tag in forms}
         for _ in range(ROUNDS):
-            for fused in (False, True):
+            for fused, _tag in forms:
                 res[fused].append(measure(step, fused))
         out = {'workload': 'nuscenes %s training step, 1 GPU, fp32, 6x48x100 rays x 256, TPV 257x257x25' % name, 'card': card(),
                'steps_per_round': K, 'rounds': ROUNDS}
-        for fused, tag in ((False, 'unfused'), (True, 'fused')):
+        for fused, tag in forms:
             r = res[fused]
             out[tag] = {'ms_per_step': float(np.median([x[0] for x in r])), 'ms_per_step_rounds': [round(x[0], 3) for x in r],
+                        'ms_per_step_spread': round(max(x[0] for x in r) - min(x[0] for x in r), 3),
                         'peak_step_mem_gb': max(x[1] for x in r), 'library_launches_per_step': r[-1][2], 'loss': r[-1][3]}
         print(json.dumps(out), flush=True)
         del step

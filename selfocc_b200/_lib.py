@@ -37,7 +37,8 @@ class ObjectiveDesc(C.Structure):
     _fields_ = [('reproj_mode', C.c_int32), ('eikonal', C.c_int32), ('pix', C.c_void_p), ('img2prev', C.c_void_p),
                 ('img2next', C.c_void_p), ('curr_imgs', C.c_void_p), ('prev_imgs', C.c_void_p), ('next_imgs', C.c_void_p),
                 ('img_h', C.c_int32), ('img_w', C.c_int32), ('size_h', C.c_float), ('size_w', C.c_float),
-                ('workspace', C.c_void_p), ('workspace_bytes', C.c_int64)]
+                ('workspace', C.c_void_p), ('workspace_bytes', C.c_int64), ('second_grad', C.c_int32),
+                ('second_grad_mean', C.c_void_p), ('grad_second_grad_mean', C.c_void_p)]
 
 
 _P = C.c_void_p

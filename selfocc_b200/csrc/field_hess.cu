@@ -5,32 +5,9 @@
 //     d2 s / dh dw = sum_k wz_k (a11k - a10k - a01k + a00k)          (and cyclic),
 // so  second_grad = (Hxy + Hxz, Hxy + Hyz, Hxz + Hyz),  Hxy = kw kh d2s/dw dh, ...  (x <-> w, y <-> h, z <-> d).
 // Zero padding outside the volume like F.grid_sample(padding_mode='zeros', align_corners=True).  Opt-in (return_second_grad).
-#include "common.cuh"
+#include "hess_terms.cuh"
 
 namespace so {
-
-struct Corner8 { float a[2][2][2]; };
-
-__device__ __forceinline__ void hess_weights(const Taps& t, float kh, float kw, float kd, float ghw, float ghz, float gwz,
-                                             float c[2][2][2]) {
-  // contribution of corner (i, j, k) to  ghw * s_hw + ghz * s_hz + gwz * s_wz  (signs: +1 for index 1, -1 for index 0)
-#pragma unroll
-  for (int i = 0; i < 2; ++i)
-#pragma unroll
-    for (int j = 0; j < 2; ++j)
-#pragma unroll
-      for (int k = 0; k < 2; ++k) {
-        float si = i ? 1.f : -1.f, sj = j ? 1.f : -1.f, sk = k ? 1.f : -1.f;
-        float wh = i ? t.fh : 1.f - t.fh, ww = j ? t.fw : 1.f - t.fw, wz = k ? t.fz : 1.f - t.fz;
-        float m = (i ? t.mh1 : t.mh0) * (j ? t.mw1 : t.mw0) * (k ? t.mz1 : t.mz0);
-        c[i][j][k] = m * (ghw * si * sj * wz + ghz * si * sk * ww + gwz * sj * sk * wh);
-      }
-}
-
-__device__ __forceinline__ size_t corner_index(const VolumeDev& v, const Taps& t, int i, int j, int k) {
-  int h = min(max(t.h0 + i, 0), v.H - 1), w = min(max(t.w0 + j, 0), v.W - 1), z = min(max(t.z0 + k, 0), v.Z - 1);
-  return ((size_t)h * v.W + w) * v.zpitch + z;
-}
 
 __global__ void __launch_bounds__(256) field_hess_kernel(VolumeDev V, const float* __restrict__ pts, long long n,
                                                          float* __restrict__ out) {
@@ -40,24 +17,11 @@ __global__ void __launch_bounds__(256) field_hess_kernel(VolumeDev V, const floa
   float kh, kw, kd;
   float gh = axis_m2g(V.ax[0], y, kh), gw = axis_m2g(V.ax[1], x, kw), gd = axis_m2g(V.ax[2], z, kd);
   Taps t = make_taps(V, gh, gw, gd);
-  float s_hw = 0.f, s_hz = 0.f, s_wz = 0.f;
-#pragma unroll
-  for (int i = 0; i < 2; ++i)
-#pragma unroll
-    for (int j = 0; j < 2; ++j)
-#pragma unroll
-      for (int k = 0; k < 2; ++k) {
-        float m = (i ? t.mh1 : t.mh0) * (j ? t.mw1 : t.mw0) * (k ? t.mz1 : t.mz0);
-        float a = m * __ldg(V.sdf + corner_index(V, t, i, j, k));
-        float si = i ? 1.f : -1.f, sj = j ? 1.f : -1.f, sk = k ? 1.f : -1.f;
-        s_hw = fmaf(si * sj * (k ? t.fz : 1.f - t.fz), a, s_hw);
-        s_hz = fmaf(si * sk * (j ? t.fw : 1.f - t.fw), a, s_hz);
-        s_wz = fmaf(sj * sk * (i ? t.fh : 1.f - t.fh), a, s_wz);
-      }
-  float Hxy = kw * kh * s_hw, Hxz = kw * kd * s_wz, Hyz = kh * kd * s_hz;
-  out[3 * p] = Hxy + Hxz;
-  out[3 * p + 1] = Hxy + Hyz;
-  out[3 * p + 2] = Hxz + Hyz;
+  float o[3];
+  second_grad_at(V, t, kh, kw, kd, o);
+  out[3 * p] = o[0];
+  out[3 * p + 1] = o[1];
+  out[3 * p + 2] = o[2];
 }
 
 __global__ void __launch_bounds__(256) field_hess_bwd_kernel(VolumeDev V, const float* __restrict__ pts, long long n,
@@ -70,7 +34,7 @@ __global__ void __launch_bounds__(256) field_hess_bwd_kernel(VolumeDev V, const 
   Taps t = make_taps(V, gh, gw, gd);
   float g0 = g[3 * p], g1 = g[3 * p + 1], g2 = g[3 * p + 2];
   float c[2][2][2];
-  hess_weights(t, kh, kw, kd, (g0 + g1) * kw * kh, (g1 + g2) * kh * kd, (g0 + g2) * kw * kd, c);
+  second_grad_weights(t, kh, kw, kd, g0, g1, g2, c);
 #pragma unroll
   for (int i = 0; i < 2; ++i)
 #pragma unroll

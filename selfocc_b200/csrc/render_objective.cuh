@@ -1,7 +1,7 @@
 // The training objective's per-sample terms folded into the training render (SURVEY.md 8f-2, DESIGN.md section 7): the
-// reprojection statistics of so_reproj_stats_forward (deltas == NULL) and the eikonal sum of so_sample_mean_forward
-// (EIKONAL), accumulated per ray while the render walks the ray's samples, and their adjoints formed per sample in the
-// backward.  Nothing per sample reaches memory.
+// reprojection statistics of so_reproj_stats_forward (deltas == NULL), the eikonal sum of so_sample_mean_forward (EIKONAL)
+// and the second-grad sum of so_field_second_grad + so_sample_mean_forward (ABS), accumulated per ray while the render walks
+// the ray's samples, and their adjoints formed per sample in the backward.  Nothing per sample reaches memory.
 //
 // The training kernels (render_train.cu) take an OBJ template parameter: kObjOff is the plain training render; the other
 // values add the objective.  ObjFwd / ObjBwd hold one ray's state in the lanes of the warp that renders it (lane = sample),
@@ -10,6 +10,7 @@
 #pragma once
 #include "reproj_terms.cuh"
 #include "eikonal_terms.cuh"
+#include "hess_terms.cuh"
 
 namespace so {
 
@@ -28,11 +29,15 @@ struct ObjectiveDev {
   float* stats;                     // [rays, 6 * sets]
   float* colours;                   // [rays, 9] or nullptr
   double* eik_part;                 // [rays] per-ray fp64 sums of (|grad sdf| - 1)^2
+  int second_grad;                  // the second-grad term is on
+  double* sg_part;                  // [rays] per-ray fp64 sums of |second_grad| over the 3 components
   // backward inputs
   const float *stats_in, *g_stats;  // [rays, 6 * sets]
   const float* g_eik_mean;          // device scalar or nullptr (= 0)
   long long eik_count;              // samples the eikonal mean is taken over
   double* inv_part;                 // [rays] per-ray d loss / d inv_s, or nullptr (no inv_s gradient)
+  const float* g_sg_mean;           // device scalar or nullptr (= 0)
+  long long sg_count;               // elements the second-grad mean is taken over (3 per sample)
 };
 
 template <int OBJ>
@@ -65,17 +70,19 @@ struct ObjRay {
 };
 
 // forward: begin() at the ray's start, sample() for every live sample (w = weight, ts = mid / |dir|, g = metre gradient of
-// the sdf), end() once per ray with every lane of the warp
+// the sdf), sample_hess() for every live sample when D.second_grad (t = the sample's taps, k = metre->grid slopes), end()
+// once per ray with every lane of the warp
 template <int OBJ>
 struct ObjFwd {
   using T = ObjTraits<OBJ>;
   ObjRay<OBJ> ray;
   float acc[T::kSets][5];
   bool any[T::kSets];
-  double eik;
+  double eik, sg;
 
   __device__ __forceinline__ void begin(const ObjectiveDev& D, int cam, int r, long long out, int lane) {
     eik = 0.0;
+    sg = 0.0;
     if (!T::kReproj) return;
     ray.load(D, cam, r);
     if (D.colours && lane < 3) {
@@ -111,7 +118,22 @@ struct ObjFwd {
     }
   }
 
+  // |second_grad| of the sample, summed as so_sample_mean_forward(ABS) sums each element: fp64 of the fp32 magnitude
+  __device__ __forceinline__ void sample_hess(const ObjectiveDev& D, const VolumeDev& V, const Taps& t, float kh, float kw,
+                                              float kd) {
+    float h[3];
+    second_grad_at(V, t, kh, kw, kd, h);
+    sg += (double)fabsf(h[0]);
+    sg += (double)fabsf(h[1]);
+    sg += (double)fabsf(h[2]);
+  }
+
   __device__ __forceinline__ void end(const ObjectiveDev& D, long long out, int lane) {
+    if (D.second_grad) {
+#pragma unroll
+      for (int o = 16; o > 0; o >>= 1) sg += __shfl_xor_sync(0xffffffffu, sg, o);
+      if (lane == 0) D.sg_part[out] = sg;
+    }
     if (D.eikonal) {
 #pragma unroll
       for (int o = 16; o > 0; o >>= 1) eik += __shfl_xor_sync(0xffffffffu, eik, o);
@@ -140,16 +162,19 @@ struct ObjFwd {
 };
 
 // backward: begin() at the ray's start; g_w(ts) = d loss / d w of a sample (reproj_stats_backward_kernel's G),
-// add_g_eik adds d loss / d g of the eikonal mean (sample_mean_backward_kernel's x * eik_coef)
+// add_g_eik adds d loss / d g of the eikonal mean (sample_mean_backward_kernel's x * eik_coef), hess_corners gives the
+// sdf-corner gradient of the second-grad mean (sample_mean_backward_kernel's sign(x) * s, then field_hess_bwd_kernel's
+// corner coefficients)
 template <int OBJ>
 struct ObjBwd {
   using T = ObjTraits<OBJ>;
   ObjRay<OBJ> ray;
   float gW[T::kSets], gs[T::kSets][4], mean[T::kSets][4];
-  float eik_s;
+  float eik_s, sg_s;
 
   __device__ __forceinline__ void begin(const ObjectiveDev& D, int cam, int r, long long out) {
     eik_s = (D.eikonal && D.g_eik_mean) ? (float)((double)__ldg(D.g_eik_mean) / (double)D.eik_count) : 0.f;
+    sg_s = (D.second_grad && D.g_sg_mean) ? (float)((double)__ldg(D.g_sg_mean) / (double)D.sg_count) : 0.f;
     if (!T::kReproj) return;
     ray.load(D, cam, r);
 #pragma unroll
@@ -186,6 +211,15 @@ struct ObjBwd {
     if (!D.eikonal) return;
     const float k = eik_coef(gx, gy, gz, eik_s);
     ggx += gx * k; ggy += gy * k; ggz += gz * k;
+  }
+
+  __device__ __forceinline__ void hess_corners(const VolumeDev& V, const Taps& t, float kh, float kw, float kd,
+                                               float c[2][2][2]) const {
+    float h[3], g[3];
+    second_grad_at(V, t, kh, kw, kd, h);
+#pragma unroll
+    for (int i = 0; i < 3; ++i) g[i] = h[i] > 0.f ? sg_s : (h[i] < 0.f ? -sg_s : 0.f);    // sign(x) * s, 0 at 0
+    second_grad_weights(t, kh, kw, kd, g[0], g[1], g[2], c);
   }
 };
 

@@ -286,7 +286,7 @@ __global__ void __launch_bounds__(128, SEM == 24 ? SO_TRAIN_FWD24_MIN_CTAS : SO_
         float dgh, dgw, dgd;
         if (__all_sync(0xffffffffu, interior)) {
           gather_sdf_interior(V, h0, w0, z0, gh - flh, gw - flw, gd - flz, q.sdf, dgh, dgw, dgd);
-          if (HAS_RGB) q.t = make_taps(V, gh, gw, gd);
+          if (HAS_RGB || (OBJ && D.second_grad)) q.t = make_taps(V, gh, gw, gd);
         } else {
           q.t = make_taps(V, gh, gw, gd);
           gather_sdf(V, q.t, q.sdf, dgh, dgw, dgd);
@@ -310,6 +310,7 @@ __global__ void __launch_bounds__(128, SEM == 24 ? SO_TRAIN_FWD24_MIN_CTAS : SO_
         if (O.sdf) O.sdf[oidx] = q.sdf;
         if (O.eik) { O.eik[3 * oidx] = q.gx; O.eik[3 * oidx + 1] = q.gy; O.eik[3 * oidx + 2] = q.gz; }
         if (OBJ) ob.sample(D, w, ts, q.gx, q.gy, q.gz);
+        if (OBJ && D.second_grad) ob.sample_hess(D, V, q.t, q.kh, q.kw, q.kd);
         acc += w;
         dsum = fmaf(w, q.mid, dsum);
         float cand = (dl < eps ? 0.f : w) * __fdividef(1.0f, fmaxf(dl, eps));  // neus_head.py:579-587
@@ -612,6 +613,7 @@ render_train_fwd5_kernel(VolumeDev V, RayDev R, RenderDev P, const float* __rest
           if (O.sdf) __stcs(O.sdf + oidx, sdf[j]);
           if (O.eik) { __stcs(O.eik + 3 * oidx, gx[j]); __stcs(O.eik + 3 * oidx + 1, gy[j]); __stcs(O.eik + 3 * oidx + 2, gz[j]); }
           if (OBJ) ob.sample(D, w, ts, gx[j], gy[j], gz[j]);
+          if (OBJ && D.second_grad) ob.sample_hess(D, V, make_taps(V, gh[j], gw[j], gd[j]), kh, kw, kd);
           acc += w;
           dsum = fmaf(w, mid[j], dsum);
           if (want_max) {
@@ -681,6 +683,22 @@ __device__ __forceinline__ void scatter_sdf(const VolumeDev& V, float* __restric
   }
 }
 
+// scatter_sdf with a further gradient per corner (c, zero where the corner's mask is 0) added before the atomic
+__device__ __forceinline__ void scatter_sdf(const VolumeDev& V, float* __restrict__ gvol, const Taps& t, float g_s, float g_gh,
+                                            float g_gw, float g_gd, const float c[2][2][2]) {
+#pragma unroll
+  for (int k = 0; k < 8; ++k) {
+    int dh = k >> 2, dw = (k >> 1) & 1, dz = k & 1;
+    float mh = dh ? t.mh1 : t.mh0, mw = dw ? t.mw1 : t.mw0, mz = dz ? t.mz1 : t.mz0;
+    float m = mh * mw * mz;
+    if (m == 0.f) continue;
+    float wh = dh ? t.fh : 1.f - t.fh, ww = dw ? t.fw : 1.f - t.fw, wz = dz ? t.fz : 1.f - t.fz;
+    float sh = dh ? 1.f : -1.f, sw = dw ? 1.f : -1.f, sz = dz ? 1.f : -1.f;
+    float g = g_s * wh * ww * wz + g_gh * sh * ww * wz + g_gw * wh * sw * wz + g_gd * wh * ww * sz;
+    atomicAdd(gvol + ((size_t)(t.h0 + dh) * V.W + (t.w0 + dw)) * V.zpitch + (t.z0 + dz), g + c[dh][dw][dz]);
+  }
+}
+
 template <int N>
 __device__ __forceinline__ void scatter_feat(const VolumeDev& V, float* __restrict__ gfeat, const Taps& t, int c0, const float g[N]) {
 #pragma unroll
@@ -697,7 +715,8 @@ __device__ __forceinline__ void scatter_feat(const VolumeDev& V, float* __restri
 
 // FAST: recompute the samples with the arithmetic of the FAST forwards (sample_geom<true>, neus_alpha_log2).
 // OBJ: kObjOff, or the objective folded in (render_objective.cuh): the sample's d loss / d w and the eikonal gradient
-// come from the objective instead of G.g_weights / G.g_eik.
+// come from the objective instead of G.g_weights / G.g_eik; with D.second_grad the second-grad term's corner gradients join
+// the sample's sdf scatter.
 template <bool HAS_RGB, int SEM, bool FAST, int OBJ>
 __global__ void __launch_bounds__(128, SEM == 24 ? SO_TRAIN_BWD24_MIN_CTAS : 1) render_train_bwd_kernel(VolumeDev V, RayDev R, RenderDev P, const float* __restrict__ ws,
                                                                const float* __restrict__ bkgd_rand, TrainGrad G, ObjectiveDev D) {
@@ -819,7 +838,13 @@ __global__ void __launch_bounds__(128, SEM == 24 ? SO_TRAIN_BWD24_MIN_CTAS : 1) 
         if (G.g_eik) { ggx += G.g_eik[3 * oidx]; ggy += G.g_eik[3 * oidx + 1]; ggz += G.g_eik[3 * oidx + 2]; }
         if (OBJ) ob.add_g_eik(D, q.gx, q.gy, q.gz, ggx, ggy, ggz);
         // metre gradient (gx, gy, gz) = (dgw kw, dgh kh, dgd kd)
-        scatter_sdf(V, G.g_vol_sdf, q.t, g_sdf, ggy * q.kh, ggx * q.kw, ggz * q.kd);
+        if (OBJ && D.second_grad) {
+          float hc[2][2][2];
+          ob.hess_corners(V, q.t, q.kh, q.kw, q.kd, hc);
+          scatter_sdf(V, G.g_vol_sdf, q.t, g_sdf, ggy * q.kh, ggx * q.kw, ggz * q.kd, hc);
+        } else {
+          scatter_sdf(V, G.g_vol_sdf, q.t, g_sdf, ggy * q.kh, ggx * q.kw, ggz * q.kd);
+        }
         if (SEM == 24 && G.g_vol_feat && (G.g_rgb || G.g_sem)) {
           // the gradient w.r.t. the 24 interpolated channels, built in place of the gathered values
 #pragma unroll

@@ -28,7 +28,9 @@ def forward_train(head, representation, metas=None, jitter=None, bkgd_rand=None,
     ``reproj_stats`` [num_cams, R, 6 * sets], ``reproj_colours`` [num_cams, R, 9] and ``eikonal_mean`` (0-d) in place of
     ``weights``, ``ts``, ``deltas`` and ``eik_grad``.  The reprojection term's images arrive as the model kwargs
     ``curr_imgs`` / ``prev_imgs`` / ``next_imgs`` ([1, num_cams, 3, H, W]) and its matrices as metas' img2prevImg /
-    img2nextImg.
+    img2nextImg.  With ``second_grad`` fused as well (fuse_objective(..., second_grad=True)) the render also takes the
+    second-grad mean at its own sample points and the outputs carry ``second_grad_mean`` (0-d) in place of ``second_grad``;
+    no per-sample tensor is then requested from the render.
 
     Decode-sharded training (``head.decode_shard = (rank, world)``, world > 1; training mode with grad enabled): see
     decode_train.  The gathered volume feeds the render, ``uniform_sdf``, ``second_grad`` and the fused objective alike."""
@@ -77,10 +79,11 @@ def forward_train(head, representation, metas=None, jitter=None, bkgd_rand=None,
                                     bkgd=head.render_bkgd)
     rd = ops.make_ray_desc(num_cams, grid=grid, n_pix=num_rays)
     fused = getattr(head, 'fused_objective', None) if training else None
+    fused_sg = fused is not None and fused.get('second_grad', False)
     if fused is None:
         want = ['depth', 'acc', 'fars', 'weights', 'ts', 'deltas', 'eik_grad']
-    else:                                                  # sample positions only for the second-grad query
-        want = ['depth', 'acc', 'fars'] + (['ts', 'deltas'] if head.return_second_grad else [])
+    else:                                                  # sample positions only for an unfused second-grad query
+        want = ['depth', 'acc', 'fars'] + (['ts', 'deltas'] if head.return_second_grad and not fused_sg else [])
     want += ['rgb'] if has_rgb else []
     want += ['sem'] if head.return_sem else []
     want += ['max_depth'] if head.return_max_depth else []
@@ -141,10 +144,12 @@ def forward_train(head, representation, metas=None, jitter=None, bkgd_rand=None,
                            reproj_colours=res['reproj_colours'].reshape(num_cams, num_rays, 9))
         if fused['eikonal']:
             outputs['eikonal_mean'] = res['eikonal_mean']
+        if fused_sg:
+            outputs['second_grad_mean'] = res['second_grad_mean']
     outputs.update(uniform_sdf=uniform_sdf, inv_s=inv_s)
     if head.return_max_depth:
         outputs['ms_max_depths'] = [max_depth]
-    if head.return_second_grad:
+    if head.return_second_grad and not fused_sg:
         # opt-in DECLARED ASSUMPTION (so_field_second_grad): row sums of the Hessian of the trilinear field at the samples
         t_len = (ts if head.sample_anchor == 'mid' else ts - 0.5 * deltas) * direction_norm[:, None, :]      # ray length at the query point
         pos = (origin[:, None, :] + direction[:, None, :] * t_len).detach().reshape(-1, 3).contiguous()
@@ -191,8 +196,9 @@ def decode_train(head, representation):
 
 def _objective(fused, kwargs, metas, rays, num_cams, dev):
     """RenderTrainObjectiveFunction's cfg['objective'] from head.fused_objective: the reprojection term's loss pixels (the
-    rays), matrices (metas, as the loss reads them) and images (the model kwargs), and whether the eikonal mean is on."""
-    ob = dict(mode=fused['mode'], eikonal=fused['eikonal'])
+    rays), matrices (metas, as the loss reads them) and images (the model kwargs), and whether the eikonal and second-grad
+    means are on."""
+    ob = dict(mode=fused['mode'], eikonal=fused['eikonal'], second_grad=fused.get('second_grad', False))
     if fused['mode'] is None:
         return ob
     from .loss import _mats

@@ -292,6 +292,20 @@ class SecondGradLoss(_SampleMeanTerm):
     def loss_func(self, second_grad):
         return ops.SampleMeanFunction.apply(second_grad, 'abs')
 
+    # the fused objective (fuse_objective(..., second_grad=True)): the head's render has already taken the mean
+    # (inputs['second_grad_mean'])
+    def forward(self, inputs):
+        if 'second_grad_mean' in inputs:
+            return self.weight * inputs['second_grad_mean']
+        return super().forward(inputs)
+
+    def local_payload(self, inputs, shard):
+        if 'second_grad_mean' not in inputs:
+            return super().local_payload(inputs, shard)
+        n = 3 * sum(t.numel() for t in inputs['ray_indices'])    # this rank's elements (3 per sample): the mean's count
+        part = inputs['second_grad_mean'].double() * n
+        return [(torch.stack([part, part.new_full((), float(n))]).reshape(1, 1, 2), shard[1])]
+
 
 class _LatticeTerm(_Term):
     """A term on the density lattice; the shipped configs feed it uniform_sdf."""
@@ -595,7 +609,7 @@ class EdgeLoss3DMS(_Term):
 _PER_SAMPLE_KEYS = ('weights', 'ts', 'deltas', 'eik_grad', 'sample_sdf')
 
 
-def fuse_objective(head, multi_loss):
+def fuse_objective(head, multi_loss, second_grad=False):
     """Let ``head``'s training render compute ``multi_loss``'s per-sample terms itself (so_render_train_objective_forward):
     the reprojection term's per-ray statistics and the eikonal mean come out of the render, and the per-sample tensors
     weights / ts / deltas / eik_grad are never written.  The losses' values and gradients are those of the unfused step.
@@ -605,14 +619,25 @@ def fuse_objective(head, multi_loss):
     outputs, without ``deltas`` / ``sample_sdfs`` inputs or sdf_loss), at most one EikonalLoss on ``eik_grad``, any number of
     terms that read no per-sample output, and a head without two_split or return_sample_sdf; anything else raises
     NotImplementedError and leaves the head unfused.  Returns what it recorded on the head (``head.fused_objective``);
-    ``head.fused_objective = None`` undoes it.  Evaluation (head.eval()) is unaffected."""
+    ``head.fused_objective = None`` undoes it.  Evaluation (head.eval()) is unaffected.
+
+    ``second_grad=True`` fuses SecondGradLoss as well: the render takes the mean of |second_grad| at its own sample points
+    and the head emits ``second_grad_mean`` instead of the [rays, S, 3] ``second_grad`` (and no longer asks the render for ts /
+    deltas).  It accepts at most one SecondGradLoss, reading ``second_grad``, on a head with return_second_grad and the
+    declared-assumption opt-in (second_grad_assumption / SELFOCC_B200_SECOND_GRAD=1); the record then carries
+    ``second_grad=True``.  Without the keyword SecondGradLoss stays on the head's second_grad tensor, as before."""
     if head.two_split and head.img2lidar.two_split:
         raise NotImplementedError('fuse_objective: two_split=True renders half the cameras for the reprojection term')
     if head.return_sample_sdf:
         raise NotImplementedError('fuse_objective: return_sample_sdf needs the per-sample sdf tensor')
-    reproj, eik = [], []
+    reproj, eik, sg = [], [], []
     for term in multi_loss.losses:
         keys = getattr(term, 'input_dict', {})
+        if second_grad and isinstance(term, SecondGradLoss):
+            if keys != {'second_grad': 'second_grad'}:
+                raise NotImplementedError('fuse_objective: SecondGradLoss must read second_grad, got input_dict %r' % (keys,))
+            sg.append(term)
+            continue
         if isinstance(term, _ReprojLoss):
             if 'deltas' in keys or 'sample_sdfs' in keys or getattr(term, 'sdf_loss', False):
                 raise NotImplementedError('fuse_objective: %s with deltas / sample_sdfs / sdf_loss' % type(term).__name__)
@@ -629,8 +654,17 @@ def fuse_objective(head, multi_loss):
     if len(reproj) > 1 or len(eik) > 1:
         raise NotImplementedError('fuse_objective: at most one reprojection term and one EikonalLoss, got %d and %d'
                                   % (len(reproj), len(eik)))
-    head.fused_objective = dict(mode=reproj[0].MODE if reproj else None,
-                                img_size=tuple(reproj[0].img_size) if reproj else None, eikonal=bool(eik))
+    if len(sg) > 1:
+        raise NotImplementedError('fuse_objective: at most one SecondGradLoss, got %d' % len(sg))
+    if sg and not getattr(head, 'return_second_grad', False):
+        raise NotImplementedError('fuse_objective: SecondGradLoss needs a head with return_second_grad=True')
+    if sg and not getattr(head, 'second_grad_assumption', False):
+        raise NotImplementedError('fuse_objective: second_grad is a declared assumption: construct the head with '
+                                  'second_grad_assumption=True (or set SELFOCC_B200_SECOND_GRAD=1)')
+    rec = dict(mode=reproj[0].MODE if reproj else None, img_size=tuple(reproj[0].img_size) if reproj else None, eikonal=bool(eik))
+    if second_grad:
+        rec['second_grad'] = bool(sg)
+    head.fused_objective = rec
     return head.fused_objective
 
 

@@ -438,17 +438,22 @@ class RenderTrainObjectiveFunction(torch.autograd.Function):
     forward(vol_sdf, vol_feat_or_None, inv_s[1], cfg) -> ORDER; cfg = RenderTrainFunction's cfg ('want' may name the per-ray
     outputs and 'ts' / 'deltas') plus cfg['objective'] = dict(mode='combine' | 'multi_new' | None, eikonal=bool, and with a mode:
     pix=[rays_per_cam, 2] loss pixels, img2prev / img2next=[n_cam, 4, 4], images=(curr, prev, next) each [n_cam, 3, H, W],
-    img_size=(h, w) of the loss).  reproj_stats [n, 6 * sets] / reproj_colours [n, 9] are ReprojStatsFunction's (row = ray),
-    eikonal_mean a 0-d tensor = SampleMeanFunction(eik_grad, 'eikonal'); entries not computed are empty tensors."""
+    img_size=(h, w) of the loss; optional second_grad=bool).  reproj_stats [n, 6 * sets] / reproj_colours [n, 9] are
+    ReprojStatsFunction's (row = ray), eikonal_mean a 0-d tensor = SampleMeanFunction(eik_grad, 'eikonal'), second_grad_mean a
+    0-d tensor = SampleMeanFunction(FieldSecondGradFunction at the render's sample points, 'abs') (gradient to vol_sdf only);
+    entries not computed are empty tensors."""
 
-    ORDER = ('depth', 'acc', 'fars', 'max_depth', 'rgb', 'sem', 'ts', 'deltas', 'reproj_stats', 'reproj_colours', 'eikonal_mean')
+    ORDER = ('depth', 'acc', 'fars', 'max_depth', 'rgb', 'sem', 'ts', 'deltas', 'reproj_stats', 'reproj_colours', 'eikonal_mean',
+             'second_grad_mean')
 
     @staticmethod
-    def _desc(ob, workspace=None):
+    def _desc(ob, workspace=None, sg_mean=None, g_sg_mean=None):
         d = _lib.ObjectiveDesc()
         mode = ob.get('mode')
         d.reproj_mode = -1 if mode is None else REPROJ_MODES[mode]       # SO_OBJECTIVE_NO_REPROJ
         d.eikonal = int(bool(ob.get('eikonal')))
+        d.second_grad = int(bool(ob.get('second_grad')))
+        d.second_grad_mean, d.grad_second_grad_mean = (0 if t is None else t.data_ptr() for t in (sg_mean, g_sg_mean))
         if mode is not None:
             for k in ('pix', 'img2prev', 'img2next'):
                 _chk(ob[k], name=k)
@@ -473,15 +478,16 @@ class RenderTrainObjectiveFunction(torch.autograd.Function):
             assert jitter.shape == (rays.n_cam * rays.rays_per_cam, S + 1)
         mode = ob.get('mode')
         want = set(cfg['want']) | ({'reproj_stats', 'reproj_colours'} if mode is not None else set()) | \
-            ({'eikonal_mean'} if ob.get('eikonal') else set())
+            ({'eikonal_mean'} if ob.get('eikonal') else set()) | ({'second_grad_mean'} if ob.get('second_grad') else set())
         shapes = dict(depth=(n,), acc=(n,), fars=(n,), max_depth=(n,), rgb=(n, 3), sem=(n, max(desc.n_feat - 3, 0)), ts=(n, S),
                       deltas=(n, S), reproj_stats=(n, 6 * REPROJ_SETS[mode] if mode is not None else 0), reproj_colours=(n, 9),
-                      eikonal_mean=())
+                      eikonal_mean=(), second_grad_mean=())
         out = {k: (torch.empty(shapes[k], device=dev) if k in want else None) for k in RenderTrainObjectiveFunction.ORDER}
         ws = _render_ws(lib, rays, dev)
         pair = torch.empty(lib.so_render_train_pair_floats(C.byref(desc)), device=dev) if cfg.get('zpair', True) else None
-        eik_ws = torch.empty(max(n, 1), dtype=torch.float64, device=dev) if ob.get('eikonal') else None
-        d = RenderTrainObjectiveFunction._desc(ob, eik_ws)
+        sums = int(bool(ob.get('eikonal'))) + int(bool(ob.get('second_grad')))     # per-ray fp64 sums, eikonal first
+        eik_ws = torch.empty(max(sums * n, 1), dtype=torch.float64, device=dev) if sums else None
+        d = RenderTrainObjectiveFunction._desc(ob, eik_ws, sg_mean=out['second_grad_mean'])
         g = lambda k: _p(out[k])
         none = _p(None)
         _lib.check(lib.so_render_train_objective_forward(
@@ -498,7 +504,7 @@ class RenderTrainObjectiveFunction(torch.autograd.Function):
 
     @staticmethod
     @torch.autograd.function.once_differentiable
-    def backward(ctx, g_depth, g_acc, g_fars, g_maxd, g_rgb, g_sem, g_ts, g_deltas, g_stats, g_colours, g_eik):
+    def backward(ctx, g_depth, g_acc, g_fars, g_maxd, g_rgb, g_sem, g_ts, g_deltas, g_stats, g_colours, g_eik, g_sg):
         lib = _lib.load()
         cfg = ctx.cfg
         vol_sdf, vol_feat, stats = ctx.saved_tensors
@@ -514,12 +520,13 @@ class RenderTrainObjectiveFunction(torch.autograd.Function):
         if mode is not None:
             gst = _chk(g_stats.contiguous() if g_stats is not None else torch.zeros_like(stats), name='grad_stats')
         geik = _chk(g_eik.reshape(1).contiguous(), name='grad_eikonal_mean') if (ob.get('eikonal') and g_eik is not None) else None
+        gsg = _chk(g_sg.reshape(1).contiguous(), name='grad_second_grad_mean') if (ob.get('second_grad') and g_sg is not None) else None
         gvs = torch.zeros_like(vol_sdf)
         gvf = torch.zeros_like(vol_feat) if vol_feat is not None else None
         ginv = torch.zeros(1, device=vol_sdf.device)
         ws = _render_ws(lib, rays, vol_sdf.device)
         inv_ws = torch.empty(max(rays.ray_count, 1), dtype=torch.float64, device=vol_sdf.device)    # per-ray d / d inv_s
-        d = RenderTrainObjectiveFunction._desc(ob, inv_ws)
+        d = RenderTrainObjectiveFunction._desc(ob, inv_ws, g_sg_mean=gsg)
         _lib.check(lib.so_render_train_objective_backward(
             _p(vol_sdf), _p(vol_feat), C.byref(desc), _p(cfg['cam_mats']), _p(cfg.get('pix')), C.byref(rays), C.byref(params),
             _p(cfg.get('jitter')), _p(cfg.get('bkgd_rand')), C.byref(d), _p(gd), _p(ga), _p(grgb), _p(gsem),
