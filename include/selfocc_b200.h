@@ -32,7 +32,8 @@ extern "C" {
                               4: backward of the fused attention cores; 5: the colour pack holds the SH-0 colour;
                               6: reprojection-loss statistics; 7: training-render sample probe;
                               8: occupancy labels and confusion matrix; 9: per-sample loss-term means;
-                              10: test hooks so_linear_force_ss / so_tpv_decode_force_simt removed */
+                              10: test hooks so_linear_force_ss / so_tpv_decode_force_simt removed.
+                              Entry points added since (so_mesh_*, so_voxel_*) change no existing signature: same version */
 
 /* ABI version of the loaded library (compare with SO_ABI_VERSION). */
 int so_abi_version(void);
@@ -353,6 +354,45 @@ int so_mesh_count(const float* vol_sdf, const so_volume_desc* vol_host, const fl
 int so_mesh_emit(const float* vol_sdf, const so_volume_desc* vol_host, const float* xs, int32_t nx, const float* ys, int32_t ny,
                  const float* zs, int32_t nz, float thresh, const int32_t* scans, const uint8_t* edge_mask, int64_t n_vertices,
                  int64_t n_faces, float* vertices, int32_t* faces, void* stream);
+
+/* ---------------------------------------------------------------------------------------
+ * Voxel-cube drawing of a label volume (what vis_3d.py / vis_3d_scene.py draw with mayavi's cube glyphs).
+ * Grid: labels uint8 [H, W, D] contiguous on the device, the layout NeuSHead.occupancy returns; voxel (h, w, d), index
+ * (h * W + w) * D + d, is the cube of side voxel_size whose lowest corner is origin_host + (w, h, d) * voxel_size (x, y, z
+ * metres; origin_host is 3 floats in host memory).  Face code 2a + s: axis a (0 x, 1 y, 2 z), s = 0 the cube's lower
+ * face on that axis, s = 1 its upper face.  A label l is drawn when palette_host[4 l + 3] (its alpha) is non-zero
+ * (so_voxel_render) or drawn_host[l] is non-zero (the face kernels).
+ *
+ * so_voxel_render: K cameras, each 16 floats of cams (device, 16-byte aligned): origin (3), a row-major 3x3 matrix M (9),
+ *   near, far, 2 unused.  Pixel (u, v) of an img_h x img_w image (v down) is the ray o + t M (u + 1/2, v + 1/2, 1), t the
+ *   ray parameter (for look-at and Img2LiDAR cameras: the depth along the optical axis, the quantity a VTK clipping
+ *   range bounds).  The ray is clipped to the grid's box and walks its cells with an Amanatides-Woo DDA in fp64
+ *   (integer cell steps; a zero direction component never steps).  The hit is the first drawn voxel the ray enters
+ *   within [near, far]; a voxel that holds the ray's point at near was entered before near and is skipped.  Its colour is
+ *   round-half-even(palette[label].rgb * shade_host[face]) in fp32, face the face entered; a pixel with no hit gets
+ *   background_host (3 bytes).  Outputs (device, any may be null, not all): rgb uint8 [K, img_h, img_w, 3], voxel int32
+ *   [K, img_h, img_w] hit index or -1, face int8 [K, img_h, img_w] or -1, dist fp32 [K, img_h, img_w] hit t or +inf.
+ *   palette_host [256 * 4] RGBA bytes and shade_host [6] floats in [0, 1] are host memory, copied into the launch.
+ * so_voxel_faces_count: counts int32 [H W D], the number of exposed faces of each voxel: a face of a drawn voxel whose
+ *   6-neighbour is not drawn or lies outside the grid.
+ * so_voxel_faces_emit: given scans = the INCLUSIVE scan of counts and its total n_faces: each exposed face as 4 vertices
+ *   fp32 [4 n_faces, 3] and 2 triangles int32 [2 n_faces, 3], counter-clockwise seen from outside, in ascending voxel
+ *   index then face code; per vertex the outward unit normal fp32 [4 n_faces, 3] and the voxel's label (sem uint8
+ *   [4 n_faces], may be null).  Quad corners: with (b, c) = (a + 1, a + 2) mod 3, (b, c) offsets (0,0) (1,0) (1,1) (0,1)
+ *   on an upper face, (0,0) (0,1) (1,1) (1,0) on a lower one; triangles (0, 1, 2) and (0, 2, 3).
+ * One thread writes each output: bit-identical run to run, no host synchronisation.
+ * Refused (SO_ERR_INVALID_ARG) before any CUDA call: null pointers, non-positive sizes, K = 0, voxel_size not positive and
+ * finite, n_faces < 1, a shade outside [0, 1], misaligned cams (16 bytes) or 4-byte outputs.  H W D >= 2^31, K > 65535
+ * and 4 n_faces >= 2^31 are SO_ERR_UNSUPPORTED. */
+int so_voxel_render(const uint8_t* labels, int32_t H, int32_t W, int32_t D, const float* origin_host, float voxel_size,
+                    const float* cams, int32_t K, int32_t img_h, int32_t img_w, const uint8_t* palette_host,
+                    const float* shade_host, const uint8_t* background_host, uint8_t* rgb, int32_t* voxel, int8_t* face,
+                    float* dist, void* stream);
+int so_voxel_faces_count(const uint8_t* labels, int32_t H, int32_t W, int32_t D, const uint8_t* drawn_host, int32_t* counts,
+                         void* stream);
+int so_voxel_faces_emit(const uint8_t* labels, int32_t H, int32_t W, int32_t D, const float* origin_host, float voxel_size,
+                        const uint8_t* drawn_host, const int32_t* scans, int64_t n_faces, float* vertices, int32_t* faces,
+                        float* normals, uint8_t* sem, void* stream);
 
 /* ---------------------------------------------------------------------------------------
  * A7/A8  multi-scale deformable attention forward.  Drop-in for

@@ -111,6 +111,9 @@ SIGNATURES = {
     'so_occ_confusion': (C.c_int, [_P, _P, _P, _L, _I, _I, _P, _P]),
     'so_mesh_count': (C.c_int, [_P, C.POINTER(VolumeDesc), _P, _I, _P, _I, _P, _I, _F, _P, _P, _P]),
     'so_mesh_emit': (C.c_int, [_P, C.POINTER(VolumeDesc), _P, _I, _P, _I, _P, _I, _F, _P, _P, _L, _L, _P, _P, _P]),
+    'so_voxel_render': (C.c_int, [_P, _I, _I, _I, _P, _F, _P, _I, _I, _I, _P, _P, _P, _P, _P, _P, _P, _P]),
+    'so_voxel_faces_count': (C.c_int, [_P, _I, _I, _I, _P, _P, _P]),
+    'so_voxel_faces_emit': (C.c_int, [_P, _I, _I, _I, _P, _F, _P, _P, _L, _P, _P, _P, _P, _P]),
     'so_sample_mean_forward': (C.c_int, [_P, _L, _I, _P, _P, _P]),
     'so_sample_mean_backward': (C.c_int, [_P, _L, _I, _P, _P, _P]),
     'so_sparsity_forward': (C.c_int, [_P, _L, _F, _P, _P, _P]),

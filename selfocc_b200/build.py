@@ -7,7 +7,7 @@ PKG = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(PKG, 'csrc')
 LIB_DIR = os.path.join(PKG, 'lib')
 LIB = os.path.join(LIB_DIR, 'libselfocc_b200.so')
-SOURCES = ['abi.cu', 'render.cu', 'render_fast.cu', 'field_hess.cu', 'metric.cu', 'render_train.cu', 'decode.cu', 'msda.cu', 'gemm.cu', 'norm.cu', 'reproj.cu', 'occupancy.cu', 'mesh.cu', 'loss_terms.cu', 'render_objective.cu']
+SOURCES = ['abi.cu', 'render.cu', 'render_fast.cu', 'field_hess.cu', 'metric.cu', 'render_train.cu', 'decode.cu', 'msda.cu', 'gemm.cu', 'norm.cu', 'reproj.cu', 'occupancy.cu', 'mesh.cu', 'loss_terms.cu', 'render_objective.cu', 'voxel_vis.cu']
 # approx-unit math (ex2/rcp/rsq) without the denormal range-scaling wrappers: ~20 instructions per render sample
 PER_SOURCE_FLAGS = {'render.cu': ['-ftz=true'], 'render_fast.cu': ['-ftz=true'], 'render_train.cu': ['-ftz=true'], 'msda.cu': ['-ftz=true'], 'decode.cu': ['-ftz=true'],
                     # same flags as render.cu: its lattice values must round like so_field_query's

@@ -12,7 +12,7 @@ import torch
 import torch.nn as nn
 
 from . import mesh as mesh_mod
-from . import occupancy, ops
+from . import occupancy, ops, voxel_vis
 from .encoder import _metas_matrix
 from .mapping import GridMeterMapping
 from .registry import HEADS
@@ -498,6 +498,33 @@ class NeuSHead(nn.Module):
         attrs = mesh_mod.vertex_attributes(f.vol_sdf, f.vol_feat, f.desc, vertices, n_sem=n_sem, lut=lut,
                                            rgb=f.color_dims >= 3, sh_act=f.sh_act)
         return dict(vertices=vertices, faces=faces, **attrs)
+
+    @torch.no_grad()
+    def render_occupancy(self, aabb, resolution, thresh, cameras, image_size, palette, lut=None, points=None, expansion=None,
+                         origin=None, voxel_size=None, shade=None, background=voxel_vis.BACKGROUND, want=('rgb',),
+                         representation=None):
+        """Draw the frame's occupancy as vis_3d.py's voxel cubes: ``occupancy(aabb, resolution, thresh, lut, points,
+        expansion)``, then ``voxel_vis.render_voxels`` on its 'sem' labels (a return_sem head) or 'occ'.
+
+        Lattice mode: lattice point [h, w, d] is drawn as the voxel at origin + (w, h, d) * voxel_size, by default
+        aabb[:3] and ``resolution`` (vis_3d.py's voxel_origin = point_cloud_range[:3]).  With ``points`` [X, Y, Z, 3]
+        laid out x first, as ``occupancy.occ3d_lidar_points``: the labels are transposed to [Y, X, Z] as vis_3d.py:549
+        does, and origin / voxel_size default to the Occ3D grid's (-40, -40, -1) and 0.4.  Crops, lidar / camera masks
+        and the height cap stay with the caller, which slices the labels and calls render_voxels itself.
+        -> (render_voxels' dict, the labels drawn)."""
+        occ = self.occupancy(aabb, resolution, thresh=thresh, lut=lut, points=points, expansion=expansion,
+                             representation=representation)
+        labels = occ['sem'] if 'sem' in occ else occ['occ']
+        if points is not None:
+            labels = labels.permute(1, 0, 2).contiguous()
+            origin = (-40.0, -40.0, -1.0) if origin is None else origin
+            voxel_size = 0.4 if voxel_size is None else voxel_size
+        else:
+            origin = tuple(aabb[:3]) if origin is None else origin
+            voxel_size = resolution if voxel_size is None else voxel_size
+        out = voxel_vis.render_voxels(labels, origin, voxel_size, cameras, image_size, palette, shade=shade,
+                                      background=background, want=want)
+        return out, labels
 
     def forward(self, representation, metas=None, **kwargs):
         """neus_head.py:473-713 (training form: per-sample weights / ts / deltas / eik_grad)."""
